@@ -59,7 +59,7 @@ int dibr_b200_trace_end(char* names, size_t names_bytes, float* ms, int capacity
 size_t dibr_b200_workspace_bytes(int batch, int64_t total_faces, int height, int width);
 
 /* Minimum scratch + a soft-mask hit cache for `cache_tiles` 16x16 screen tiles
- * (3072*knum + 16 bytes each, + 17 412 bytes when knum <= 32).  Any workspace larger than the minimum is used by
+ * (3072*knum + 16 bytes each).  Any workspace larger than the minimum is used by
  * dibr_b200_forward (mode & SOFT_MASK) to record, per tile that has any, the
  * (pixel, face, probability, distance type) hits — what the reference stores as
  * 13*knum bytes for EVERY pixel (dibr.py:49-54) — so that dibr_b200_backward with

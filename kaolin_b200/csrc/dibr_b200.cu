@@ -7,7 +7,7 @@
 //
 // Pipeline (forward):
 //   bin_faces<count> -> scan_bins -> bin_faces<fill> -> dibr_tile_fwd_kernel
-//   -> soft_enum_kernel -> soft_eval_kernel (-> soft_tiles_fwd_kernel for leftovers)
+//   -> soft_fwd_kernel (-> soft_tiles_fwd_kernel for leftovers)
 //   * every face is turned into the exact integer pixel rectangle of the
 //     reference's float bbox test and inserted (<= 4 entries) into the finest
 //     level of a 16/64/256/... px bin pyramid where it spans <= 2x2 bins;
@@ -17,10 +17,11 @@
 //     transposes their rectangle masks into per-column/row candidate bit words and
 //     lets each thread (one pixel) walk exactly its own rectangle hits;
 //   * tiles with uncovered pixels under an enlarged (boxlen) rectangle are filed in
-//     a work list; for them the first knum faces by index of every uncovered pixel
-//     are enumerated (integer work), evaluated densely — one thread per
-//     (pixel, face) pair — and folded per pixel in face order.  The pairs stay in a
-//     per-tile cache block for the backward pass.
+//     a work list; one CTA per such tile enumerates the first knum faces by index of
+//     every uncovered pixel, stages each candidate face's per-face terms in shared
+//     memory once, evaluates the pairs densely — one thread per (pixel, face) pair —
+//     and folds them per pixel in face order.  The pairs stay in a per-tile cache
+//     block for the backward pass.
 // Backward: a pixel-parallel scatter with warp-level segmented reduction keyed
 // on the face id (rasterize branch) and a dense stream over the cached pairs
 // (soft-mask branch; tiles outside the cache are recomputed).
@@ -79,9 +80,6 @@ struct Scene {
   int* pool_ctr;          // [1] blocks handed out
   int4* pool_hdr;         // [pool_tiles] {b, tx, ty, hits}
   uint32_t* pool_data;    // [pool_tiles][3][256*K]: face | prob bits | lx|ly<<4|(dist_type)<<8
-  int* pool_na;           // [pool_tiles] uncovered pixels of the tile           } only when
-  uint32_t* pool_aux;     // [pool_tiles][256] per such pixel: lx|ly<<4 | hits<<8 } knum <= 32:
-  uint16_t* pool_slots;   // [pool_tiles][256][32] its hit slots, face order      } 3-kernel forward
   int* fb_ctr;            // [1] tiles whose hits did not fit the cache (recomputed in backward)
   int* fb_list;           // [B*nty*ntx] their linear tile ids
   int* tile_cnt;          // [B*nty*ceil(ntx/32)] bit per 16x16 tile: an enlarged face rectangle overlaps it (count pass)
@@ -1644,42 +1642,56 @@ __global__ void __launch_bounds__(kThreads, 4) soft_tiles_fwd_kernel(const __gri
 }
 
 // ---------------------------------------------------------------------------
-// Two-kernel soft-mask forward (knum <= 32, hit cache available):
-//   soft_enum_kernel : per silhouette tile, decides WHICH (pixel, face) pairs exist
-//                      (integer work only) and lays them out face-major in the tile's
-//                      cache block, with each pixel's slot list in face order;
-//   soft_eval_kernel : one thread per pair - the expensive distance / probability,
-//                      dense - then each pixel folds its probabilities in face order
-//                      (a tile's pairs are all evaluated by the CTA that folds them).
-// Tiles that do not fit the cache go to fb_list and take the single-kernel path.
-constexpr int kEnumK = 32;
-constexpr int kRunHits = 8;   // consecutive cached pairs per thread in the run kernels
+// Fused soft-mask forward (knum <= kSoftFwdK, hit cache available), persistent CTAs over the
+// work list.  Per silhouette tile the uncovered pixels are compacted and the candidates
+// collected and sorted by face index; then, per chunk of <= 256 candidates:
+//   stage    each candidate's vertices and fp64 edge divisors (soft_face) in shared memory, once;
+//   claim    every uncovered pixel takes its remaining faces of the chunk in index order
+//            (<= knum in all; positions inside a face from shared-memory atomics);
+//   lay out  the pairs face-major in the tile's cache block (pixel | candidate in the meta word);
+//   evaluate one (pixel, face) pair per thread with all 256 threads, the face part read from
+//            shared memory, and write face, probability and dist_type into the block;
+//   fold     each pixel multiplies its probabilities of the chunk, in face order, into a register.
+// Chunks and index windows come in ascending face order, so the fold is the reference's loop
+// (dibr_soft_mask_cuda.cu:174-182) term for term.  Tiles that do not fit the cache go to fb_list
+// and take the single-kernel path.
+constexpr int kSoftFwdK = 32;  // largest knum of the fused kernel (claims per pixel and chunk)
+constexpr int kRunHits = 8;    // consecutive cached pairs per thread in the run kernels
 
-struct EnumSmem {
-  unsigned long long list[kSoftCap];
+// Per-chunk face part.  The fp32 line terms of soft_face (A, B, C and their products) are
+// recomputed from the vertices per pair: seven fp32 operations cost less than loading six floats.
+struct SoftCand {
+  float4 xy0[kChunk];        // vertices a, b
+  float2 xy1[kChunk];        // vertex c
+  DRecip down64[3][kChunk];  // per edge: (double)(A^2 + B^2) + eps and its reciprocal
+};
+
+struct SoftFwdSmem {
+  union {
+    unsigned long long list[kSoftCap];  // soft_window's candidates: dead once soft_sort is done
+    SoftCand cand;                      // the current chunk
+  };
   unsigned long long sorted[kSoftCap];
-  int cface[kChunk];
   uint32_t colbits[kChunk / 32][16];
   uint32_t rowbits[kChunk / 32][16];
   int cnt_c[kChunk];
   int off_c[kChunk];
-  uint16_t claim[kThreads][kEnumK];
+  uint16_t claim[kThreads][kSoftFwdK];  // per pixel, face order: candidate | position << 8
   uint8_t apix[kThreads];
   BinRef bin[2][kMaxLevels];
-  int wcount[kThreads / 32];
   int nsoft, nent, pool_slot, npairs;
 };
 
-#ifndef DIBR_ENUM_MINB
-#define DIBR_ENUM_MINB 4   /* H100, c4_shard: 4 CTAs/SM 0.71 ms, 5: 0.73, 6: 0.76, 8: 0.84 */
+#ifndef DIBR_SOFT_FWD_MINB
+#define DIBR_SOFT_FWD_MINB 4   /* H100 (400 W), c4_shard: 4 CTAs/SM 0.81 ms, 3: 0.91, 5: 0.88, 6: 1.01 */
 #endif
-__global__ void __launch_bounds__(kThreads, DIBR_ENUM_MINB) soft_enum_kernel(const __grid_constant__ FwdArgs a) {
-  __shared__ __align__(128) EnumSmem sm;
+__global__ void __launch_bounds__(kThreads, DIBR_SOFT_FWD_MINB) soft_fwd_kernel(const __grid_constant__ FwdArgs a) {
+  __shared__ __align__(128) SoftFwdSmem sm;
   const Scene& s = a.s;
   const int K = a.K;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int total = min(*s.band_ctr, s.ntx[0] * s.nty[0] * s.B);
-  const size_t E = (size_t)256 * s.pool_K;
+  const int E = 256 * s.pool_K;   // block words per array (< 2^14): 32-bit offsets
   for (int w = blockIdx.x; w < total; w += gridDim.x) {
     // the work-list record carries the tile id, the uncovered-pixel ballots of the
     // rasterizer's 8 warps and the tile's large-bin table: one load latency, no
@@ -1698,12 +1710,12 @@ __global__ void __launch_bounds__(kThreads, DIBR_ENUM_MINB) soft_enum_kernel(con
     __syncthreads();  // previous tile's shared state fully consumed
     bins_from_record(s, rec, c.fbase, sm);
     if ((mymask >> lane) & 1u) sm.apix[before + __popc(mymask & ((1u << lane) - 1u))] = (uint8_t)(c.lx | (c.ly << 4));
-    const bool active = tid < na;
+    const bool active = tid < na;  // thread t owns the t-th uncovered pixel
     int lx = 0, ly = 0;
     int kid = 0;
+    float allprob = 1.0f;
     const int maxf = s.first ? (int)(__ldg(s.first + c.b + 1) - c.fbase) : s.F;
     uint32_t* blk = nullptr;
-    uint16_t* myslots = nullptr;
     bool first_window = true, cached = true;
     int lo = -1;
     while (true) {
@@ -1729,17 +1741,22 @@ __global__ void __launch_bounds__(kThreads, DIBR_ENUM_MINB) soft_enum_kernel(con
       if (alloc) {
         if (sm.pool_slot < 0) { cached = false; break; }  // uniform: handed over to the single-kernel path
         blk = s.pool_data + (size_t)sm.pool_slot * 3 * E;
-        myslots = s.pool_slots + ((size_t)sm.pool_slot * kThreads + tid) * kEnumK;
       }
       bool all_done = false;
       for (int c0 = 0; c0 < n && !all_done; c0 += kChunk) {
         const int cn = min(kChunk, n - c0);
         const int ngroups = (cn + 31) >> 5;
         uint32_t m = 0;
-        if (tid < cn) {
+        if (tid < cn) {  // face part of candidate tid, once per tile
           const unsigned long long key = sm.sorted[c0 + tid];
           m = (uint32_t)key;
-          sm.cface[tid] = (int)(key >> 32);
+          float v[6];
+          load_xy(s, c.fbase + (int)(key >> 32), v);
+          sm.cand.xy0[tid] = make_float4(v[0], v[1], v[2], v[3]);
+          sm.cand.xy1[tid] = make_float2(v[4], v[5]);
+          const SoftFace F = soft_face(v);
+#pragma unroll
+          for (int i = 0; i < 3; ++i) sm.cand.down64[i][tid] = F.down64[i];
         }
         if (warp < ngroups) store_bit_matrix(m, sm.colbits, sm.rowbits, warp);
         sm.cnt_c[tid] = 0;
@@ -1772,68 +1789,64 @@ __global__ void __launch_bounds__(kThreads, DIBR_ENUM_MINB) soft_enum_kernel(con
           if (lane == 31) sm.npairs = x;
         }
         __syncthreads();
-        const int ebase = sm.nent;
+        const int ebase = sm.nent, T = sm.npairs;
+        // pair -> (pixel, candidate) map in the meta words; the CTA reads it back after the barrier
         for (int i = 0; i < took; ++i) {
           const int cl = sm.claim[tid][i];
           const int j = cl & 0xff;
-          const int slot = ebase + sm.off_c[j] + (cl >> 8);
-          blk[slot] = (uint32_t)sm.cface[j];
-          blk[2 * E + slot] = (uint32_t)lx | ((uint32_t)ly << 4);
-          myslots[kid + i] = (uint16_t)slot;
+          blk[2 * E + ebase + sm.off_c[j] + (cl >> 8)] = (uint32_t)lx | ((uint32_t)ly << 4) | ((uint32_t)j << 16);
+        }
+        __syncthreads();
+        // dense evaluation: one (pixel, face) pair per thread
+#pragma unroll 1
+        for (int u = tid; u < T; u += kThreads) {
+          const int e = ebase + u;
+          const uint32_t map = blk[2 * E + e];
+          const int j = (int)(map >> 16);
+          const int plx = (int)(map & 15u), ply = (int)((map >> 4) & 15u);
+          const float4 q0 = sm.cand.xy0[j];
+          const float2 q1 = sm.cand.xy1[j];
+          const float v[6] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y};
+          SoftFace F;
+#pragma unroll
+          for (int i = 0; i < 3; ++i) { F.e[i] = soft_edge(v, i); F.down64[i] = sm.cand.down64[i][j]; }
+          int edgeid;
+          const float d2 = soft_pixel_dist(pix_x(s.grid, c.tile_x0 + plx), pix_y(s.grid, c.tile_y0 + ply), v, F,
+                                           s.multiplier, edgeid);
+          const float prob = soft_prob(d2, a.sigmainv, s.multiplier);
+          blk[e] = (uint32_t)(sm.sorted[c0 + j] >> 32);
+          blk[E + e] = __float_as_uint(prob);
+          blk[2 * E + e] = (map & 0xffu) | ((uint32_t)(edgeid + 1) << 8);
+        }
+        __syncthreads();
+        // fold: each pixel multiplies its probabilities in face order, four loads in flight
+        for (int i0 = 0; i0 < took; i0 += 4) {
+          float p[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            if (i0 + q < took) {
+              const int cl = sm.claim[tid][i0 + q];
+              p[q] = __uint_as_float(blk[E + ebase + sm.off_c[cl & 0xff] + (cl >> 8)]);
+            }
+          }
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            if (i0 + q < took) allprob = soft_accumulate(allprob, p[q]);
         }
         kid += took;
         all_done = __syncthreads_and(!active || kid >= K);
-        if (tid == 0) sm.nent = ebase + sm.npairs;
+        if (tid == 0) sm.nent = ebase + T;
       }
       if (hi == 0x7fffffff || all_done) break;
       lo = hi;
     }
     if (cached) {
-      __syncthreads();
-      s.pool_aux[(size_t)sm.pool_slot * kThreads + tid] =
-          active ? ((uint32_t)(lx | (ly << 4)) | ((uint32_t)kid << 8)) : 0u;
-      if (tid == 0) {
-        s.pool_hdr[sm.pool_slot] = make_int4(c.b, c.tx, c.ty, sm.nent);
-        s.pool_na[sm.pool_slot] = na;
-      }
+      // the tile's coordinates again from the record: cheaper than keeping them in registers
+      const TileCtx ce = tile_ctx_from_linear(s, __ldg(s.band_list + (size_t)w * kBandRec));
+      if (active) a.out_soft[((int64_t)ce.b * s.H + (ce.tile_y0 + ly)) * s.W + (ce.tile_x0 + lx)] = soft_finish(allprob);
+      if (tid == 0) s.pool_hdr[sm.pool_slot] = make_int4(ce.b, ce.tx, ce.ty, sm.nent);
     }
   }
-}
-
-__global__ void __launch_bounds__(kThreads) soft_eval_kernel(const __grid_constant__ FwdArgs a) {
-  const Scene& s = a.s;
-  const int used = min(*s.pool_ctr, s.pool_tiles);
-  if ((int)blockIdx.x >= used) return;
-  const int4 h = s.pool_hdr[blockIdx.x];  // b, tx, ty, hits
-  const size_t E = (size_t)256 * s.pool_K;
-  uint32_t* blk = s.pool_data + (size_t)blockIdx.x * 3 * E;
-  const int64_t fbase = view_fbase(s, h.x);
-  const int tid = threadIdx.x;
-  uint32_t nface = 0, nmeta = 0;
-  if (tid < h.w) { nface = blk[tid]; nmeta = blk[2 * E + tid]; }
-  for (int t = tid; t < h.w; t += kThreads) {
-    const uint32_t face = nface, meta = nmeta;
-    if (t + kThreads < h.w) { nface = blk[t + kThreads]; nmeta = blk[2 * E + t + kThreads]; }
-    const int px = h.y * kTile + (int)(meta & 15u), py = h.z * kTile + (int)((meta >> 4) & 15u);
-    float v[6];
-    load_xy(s, fbase + (int)face, v);
-    int edgeid;
-    const float d2 = soft_min_dist(pix_x(s.grid, px), pix_y(s.grid, py), v, s.multiplier, edgeid);
-    const float prob = soft_prob(d2, a.sigmainv, s.multiplier);
-    blk[E + t] = __float_as_uint(prob);
-    blk[2 * E + t] = meta | ((uint32_t)(edgeid + 1) << 8);
-  }
-  // fold: each uncovered pixel multiplies its probabilities in face order
-  // (dibr_soft_mask_cuda.cu:174-182); the tile's pairs were all evaluated by this CTA
-  __syncthreads();
-  if (tid >= s.pool_na[blockIdx.x]) return;
-  const uint32_t aux = s.pool_aux[(size_t)blockIdx.x * kThreads + tid];
-  const uint16_t* myslots = s.pool_slots + ((size_t)blockIdx.x * kThreads + tid) * kEnumK;
-  const int cnt = (int)(aux >> 8);
-  float allprob = 1.0f;
-  for (int i = 0; i < cnt; ++i) allprob = soft_accumulate(allprob, __uint_as_float(blk[E + myslots[i]]));
-  const int fx = h.y * kTile + (int)(aux & 15u), fy = h.z * kTile + (int)((aux >> 4) & 15u);
-  a.out_soft[((int64_t)h.x * s.H + fy) * s.W + fx] = soft_finish(allprob);
 }
 
 // ---------------------------------------------------------------------------
@@ -2478,11 +2491,8 @@ Layout layout_for(int B, int64_t NF, int H, int W) {
   return L;
 }
 
-size_t pool_aux_bytes(int K) {  // per-tile extras of the 3-kernel forward
-  return K <= kEnumK ? sizeof(int) + 256 * sizeof(uint32_t) + (size_t)256 * kEnumK * sizeof(uint16_t) : 0;
-}
 size_t pool_block_bytes(int K) {
-  return sizeof(int4) + pool_aux_bytes(K) + (size_t)3 * 256 * (size_t)K * sizeof(uint32_t);
+  return sizeof(int4) + (size_t)3 * 256 * (size_t)K * sizeof(uint32_t);
 }
 
 int check_dims(int B, int64_t NF, int H, int W) {
@@ -2529,17 +2539,10 @@ int setup_scene(Scene& s, int B, int64_t NF, int F, int H, int W, float multipli
   s.entries = (int4*)p; p += Lo.ent;
   p += Lo.acc;
   s.pool_tiles = 0; s.pool_K = knum > 0 ? knum : 1; s.pool_hdr = nullptr; s.pool_data = nullptr;
-  s.pool_na = nullptr; s.pool_aux = nullptr; s.pool_slots = nullptr;
   if (knum > 0) {
     const size_t left = (size_t)(end - p);
     const size_t data = (size_t)3 * 256 * (size_t)knum * sizeof(uint32_t);
-    const bool aux = knum <= kEnumK;
-    auto need = [&](size_t n) {
-      size_t b = align_up(n * sizeof(int4), 256) + n * data;
-      if (aux) b += align_up(n * sizeof(int), 256) + n * 256 * sizeof(uint32_t) +
-                    align_up(n * 256 * kEnumK * sizeof(uint16_t), 256);
-      return b;
-    };
+    auto need = [&](size_t n) { return align_up(n * sizeof(int4), 256) + n * data; };
     size_t n = left / pool_block_bytes(knum);
     const size_t tiles = (size_t)s.ntx[0] * s.nty[0] * B;
     if (n > tiles) n = tiles;
@@ -2547,11 +2550,6 @@ int setup_scene(Scene& s, int B, int64_t NF, int F, int H, int W, float multipli
     if (n > 0) {
       s.pool_tiles = (int)n;
       s.pool_hdr = (int4*)p; p += align_up(n * sizeof(int4), 256);
-      if (aux) {
-        s.pool_na = (int*)p; p += align_up(n * sizeof(int), 256);
-        s.pool_aux = (uint32_t*)p; p += n * 256 * sizeof(uint32_t);
-        s.pool_slots = (uint16_t*)p; p += align_up(n * 256 * kEnumK * sizeof(uint16_t), 256);
-      }
       s.pool_data = (uint32_t*)p;
     }
   }
@@ -2651,15 +2649,11 @@ void launch_fwd(const FwdArgs& a0, cudaStream_t st) {
   }
   if (S) {
     const unsigned g1 = persistent_grid(a.s, soft_tiles_fwd_kernel<K>, sizeof(SoftSmem));   // (sets the smem attribute once)
-    if (!K && a.cache && a.s.pool_tiles > 0 && a.s.pool_slots != nullptr) {
-      // enumerate -> evaluate densely -> fold; tiles beyond the cache take the single-kernel path
+    if (!K && a.cache && a.s.pool_tiles > 0 && a.K <= kSoftFwdK) {
+      // enumerate, evaluate densely and fold per tile; tiles beyond the cache take the single-kernel path
       {
-        Span sp("soft_enum_kernel", st);
-        soft_enum_kernel<<<persistent_grid(a.s, soft_enum_kernel), kThreads, 0, st>>>(a);
-      }
-      {
-        Span sp("soft_eval_kernel", st);
-        soft_eval_kernel<<<(unsigned)a.s.pool_tiles, kThreads, 0, st>>>(a);
+        Span sp("soft_fwd_kernel", st);
+        soft_fwd_kernel<<<persistent_grid(a.s, soft_fwd_kernel), kThreads, 0, st>>>(a);
       }
       a.from_fb = 1;
       a.cache = 0;

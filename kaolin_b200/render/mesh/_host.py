@@ -64,10 +64,10 @@ CACHE_MAX_BYTES = 4 << 30
 
 
 def cache_tiles_for(batch, height, width, knum):
-    """How many 16x16 tiles get a soft-mask hit-cache block (3072*knum + 17.4 KB each)."""
+    """How many 16x16 tiles get a soft-mask hit-cache block (3072*knum + 16 bytes each)."""
     tiles = batch * ((height + 15) // 16) * ((width + 15) // 16)
     want = max(CACHE_MIN_TILES, int(tiles * CACHE_TILE_FRACTION))
-    return min(tiles, want, max(1, CACHE_MAX_BYTES // (3072 * knum + 17500)))
+    return min(tiles, want, max(1, CACHE_MAX_BYTES // (3072 * knum + 16)))
 
 
 _ws_bytes = {}     # (batch, faces, H, W, knum, cache policy) -> bytes: a pure function of the shape
