@@ -82,7 +82,9 @@ size_t dibr_b200_workspace_bytes_cached(int batch, int64_t total_faces, int heig
  *  boxlen_m             = (float)(boxlen * multiplier)   (dibr.py:36-37)
  *  mode                 DIBR_B200_RASTER | DIBR_B200_SOFT_MASK
  *  face_idx             (B,H,W) i64: output if RASTER, else INPUT (dibr_soft_mask alone)
- *  interpolated_features(B,H,W,D) f32, output_weights (B,H,W,3) f32: outputs if RASTER
+ *  interpolated_features(B,H,W,D) f32: output if RASTER
+ *  output_weights       (B,H,W,3) f32: output if RASTER, or NULL: the weights are not
+ *                       written (dibr_b200_backward can recompute them, bit for bit)
  *  soft_mask            (B,H,W) f32: output if SOFT_MASK
  * The workspace keeps the face bins; pass it unchanged to dibr_b200_backward
  * with bins_valid = 1 to skip rebuilding them.
@@ -101,6 +103,10 @@ int dibr_b200_forward(
  * Replaces rasterization.py:355-371 + dibr.py:58-73 and the kernels behind them.
  *  grad_features  (B,H,W,D) f32 or NULL (skips the rasterize branch; grad_face_features is zeroed)
  *  grad_soft_mask (B,H,W)   f32 or NULL (skips the soft-mask branch)
+ *  output_weights forward's output, or NULL: the rasterize branch recomputes each covered
+ *                 pixel's weights from face_idx, face_vertices_image * multiplier and eps with
+ *                 the forward's arithmetic (the same bits), so multiplier and eps MUST then be
+ *                 the values the forward was called with
  *  soft_mask      forward's output (needed only with grad_soft_mask)
  *  flags          DIBR_B200_BINS_VALID: workspace still holds forward's bins for the same
  *                 inputs.  DIBR_B200_ACCUMULATE: grad_face_vertices_image is added to, not
@@ -215,7 +221,7 @@ int dibr_b200_packed_rasterize_forward(
  * (rasterization.h:34-41, rasterization.cpp:106-168).  face_vertices_image is the
  * UNSCALED (B,F,3,2) tensor; selected_face_idx holds original face ids.
  * (The reference's `interpolated_features` argument is never read by its kernel
- * and is therefore not part of this ABI.)
+ * and is therefore not part of this ABI.)  output_weights is required (not NULL).
  */
 int dibr_b200_rasterize_backward(
     int batch, int num_faces, int height, int width, int feat_dim,

@@ -1183,8 +1183,10 @@ __global__ void __launch_bounds__(kThreads, 6) dibr_tile_fwd_kernel(const __grid
     best_f = o.f;
     if (c.in_img) {
       a.idx[c.pix] = (int64_t)o.f;
-      float* wp = a.out_w + c.pix * 3;
-      wp[0] = o.w0; wp[1] = o.w1; wp[2] = o.w2;
+      if (a.out_w) {
+        float* wp = a.out_w + c.pix * 3;
+        wp[0] = o.w0; wp[1] = o.w1; wp[2] = o.w2;
+      }
       FT* fp = static_cast<FT*>(a.out_feat) + c.pix * a.D;
       const FT* feat = static_cast<const FT*>(a.feat);
       if (a.D == 3) {  // the DIB-R tutorial shape (uv + mask), fully unrolled
@@ -1397,7 +1399,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
     }
     for (int c = tid; c < kSide * kWC; c += kThreads) {
       const int r = c / kWC, ch = c - r * kWC;
-      reinterpret_cast<float4*>(a.out_w + (pix_row0 + (int64_t)r * s.W) * 3)[ch] = zero;
+      if (a.out_w) reinterpret_cast<float4*>(a.out_w + (pix_row0 + (int64_t)r * s.W) * 3)[ch] = zero;
       reinterpret_cast<float4*>(static_cast<float*>(a.out_feat) + (pix_row0 + (int64_t)r * s.W) * 3)[ch] = zero;
     }
     if (SOFT) {
@@ -1556,8 +1558,10 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
       best_f = o.f;
       if (in_img) {
         a.idx[pix] = (int64_t)o.f;
-        float* wp = a.out_w + pix * 3;
-        wp[0] = o.w0; wp[1] = o.w1; wp[2] = o.w2;
+        if (a.out_w) {
+          float* wp = a.out_w + pix * 3;
+          wp[0] = o.w0; wp[1] = o.w1; wp[2] = o.w2;
+        }
         FT* fp = static_cast<FT*>(a.out_feat) + pix * a.D;
         const FT* feat = static_cast<const FT*>(a.feat);
         if (a.D == 3) {  // the DIB-R tutorial shape (uv + mask), fully unrolled
@@ -2022,11 +2026,13 @@ __device__ __forceinline__ void reduce_peers(unsigned peers, float (&v)[N]) {
   }
 }
 
+// w == nullptr: the weights are recomputed from face_idx, xy * multiplier and the pixel grid, which
+// reproduces the forward's bits when multiplier and eps are the forward's
 struct RasterBwdArgs {
   int B, H, W, F, D;
   int ntx, nty;
   const void* grad_feat; const int64_t* idx; const float* w; const float* xy; const void* feat;  // FT
-  float eps;
+  PixelGrid grid; RasterConst rc; float multiplier;
   float* grad_xy; float* grad_feat_out;
 };
 
@@ -2041,7 +2047,7 @@ __global__ void __launch_bounds__(kThreads, 6) raster_bwd_kernel(const __grid_co
   const bool in_img = px < a.W && py < a.H;
   const int64_t pix = ((int64_t)b * a.H + py) * a.W + px;
   const int D = DT > 0 ? DT : a.D;
-  // all streaming operands of the pixel are requested together (weights and upstream
+  // all streaming operands of the pixel are requested together (given weights and upstream
   // gradient do not depend on face_idx): one exposed HBM latency instead of two
   int f = -1;
   float w0 = 0.f, w1 = 0.f, w2 = 0.f;
@@ -2049,9 +2055,11 @@ __global__ void __launch_bounds__(kThreads, 6) raster_bwd_kernel(const __grid_co
 #pragma unroll
   for (int d = 0; d < (DT > 0 ? DT : 1); ++d) gpre[d] = 0.f;
   if (in_img) {
-    const float* wp = a.w + pix * 3;
     f = (int)__ldcs(a.idx + pix);
-    w0 = __ldcs(wp); w1 = __ldcs(wp + 1); w2 = __ldcs(wp + 2);
+    if (a.w) {
+      const float* wp = a.w + pix * 3;
+      w0 = __ldcs(wp); w1 = __ldcs(wp + 1); w2 = __ldcs(wp + 2);
+    }
     if (DT > 0) {
 #pragma unroll
       for (int d = 0; d < DT; ++d) gpre[d] = Feat<FT>::ld_stream(grad_feat + pix * DT + d);
@@ -2066,7 +2074,12 @@ __global__ void __launch_bounds__(kThreads, 6) raster_bwd_kernel(const __grid_co
     const float2* pp = reinterpret_cast<const float2*>(a.xy + face * 6);
     const float2 pa = __ldg(pp), pb = __ldg(pp + 1), pc = __ldg(pp + 2);
     const float p[6] = {pa.x, pa.y, pb.x, pb.y, pc.x, pc.y};
-    raster_backward_geom(p, w0, w1, w2, a.eps, G);
+    if (!a.w) {
+      const float m = a.multiplier;
+      raster_weights_of(a.rc, pix_x(a.grid, px), pix_y(a.grid, py), fmul(p[0], m), fmul(p[1], m),
+                        fmul(p[2], m), fmul(p[3], m), fmul(p[4], m), fmul(p[5], m), w0, w1, w2);
+    }
+    raster_backward_geom(p, w0, w1, w2, a.rc.eps, G);
   }
   // lanes without a face get unique negative keys so they never merge
   const unsigned peers = __match_any_sync(kFull, cov ? (int)f : -1 - lane);
@@ -2144,12 +2157,16 @@ __global__ void __launch_bounds__(kThreads, 6) raster_bwd_kernel(const __grid_co
 //     face_idx changes it flushes them with (6+3D+3)/4 vector reductions into a padded
 //     per-face accumulator (acc[face][16] for D = 3: 64-byte records, 16-byte aligned) and
 //     reloads the face constants.  No shuffles, no match, no leader election;
-//   * the pixel streams (face_idx 8 B, weights 12 B, upstream gradient 4*D B per pixel) are
-//     staged per 4-column slab with 16-byte cp.async (LDGSTS) into rows padded to an odd
-//     number of 16-byte chunks, double buffered, and read back with LDS.128 (conflict free:
-//     8 consecutive rows cover the 32 banks).  9 KB of shared memory and <= 128 registers per
+//   * the pixel streams (face_idx 8 B, upstream gradient 4*D B per pixel) are staged per
+//     4-column slab with 16-byte cp.async (LDGSTS) into rows padded to an odd number of
+//     16-byte chunks, double buffered, and read back with LDS.128 (conflict free: 8
+//     consecutive rows cover the 32 banks).  6 KB of shared memory and <= 128 registers per
 //     single-warp CTA keep 16 warps per SM in flight (8-column slabs needed 162 registers:
 //     9 warps per SM);
+//   * the barycentric weights are not read: each covered pixel recomputes its face's weights
+//     with the forward's own arithmetic (raster_weights_of: same bits), from the face's
+//     vertices times the multiplier, which the lane holds while it walks the face's run.
+//     Weights given by the caller (the operator-level backward) are read per pixel instead;
 //   * raster_bwd_finalize_kernel unpacks acc into grad_face_vertices_image /
 //     grad_face_features (which therefore need no memset).
 // Per-pixel arithmetic is the reference's operation tree (dibr_math.cuh,
@@ -2162,7 +2179,6 @@ struct RwCfg {
   // rows padded to an ODD number of 16-byte chunks: 8 consecutive rows then cover all 32 banks
   static constexpr int pad_odd(int bytes) { return ((bytes / 16) & 1) ? bytes : bytes + 16; }
   static constexpr int kIdxPitch = pad_odd(kRwSlab * 8);        // 32 -> 48
-  static constexpr int kWPitch = pad_odd(kRwSlab * 12);         // 48
   static constexpr int kVals = 6 + 3 * DT;
   static constexpr int kAcc = (kVals + 3) & ~3;                 // floats per face record
 };
@@ -2173,7 +2189,7 @@ struct RwG {
   static constexpr int kRow = kRwSlab * DT * (int)sizeof(FT);
   static constexpr int kChunk = (kRow % 16) ? 8 : 16;
   static constexpr int kPitch = kChunk == 16 ? RwCfg<DT>::pad_odd(kRow) : kRow;
-  static constexpr int kStage = 32 * (RwCfg<DT>::kIdxPitch + RwCfg<DT>::kWPitch + kPitch);
+  static constexpr int kStage = 32 * (RwCfg<DT>::kIdxPitch + kPitch);
 };
 constexpr int kAccMax = 20;  // D = 4
 
@@ -2190,7 +2206,7 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 struct RowBwdArgs {
   int B, H, W, F, strip, jobs_x, jobs_y;
   const void* grad_feat; const int64_t* idx; const float* w; const float* xy; const void* feat;   // FT: float | bf16
-  float eps;
+  PixelGrid grid; RasterConst rc; float multiplier;   // w == nullptr: see RasterBwdArgs
   float* acc;    // [B*F][RwCfg<D>::kAcc], zeroed
   int* job_ctr;  // [1] zeroed (lives right behind the records)
 };
@@ -2198,6 +2214,7 @@ struct RowBwdArgs {
 template <int DT>
 struct RowFace {          // constants of the face a lane is currently accumulating
   float ax, ay, bx, by, cx, cy;
+  float mx[3], my[3];           // vertices * multiplier: the forward's raster coordinates
   float pp, n, m, q, k3, rk;
   float qk3, nk3n, ppk3n, mk3;  // q*k3, -(n*k3), -(pp*k3), m*k3  (dw1ds, dw1dt, dw2ds, dw2dt)
   float d1[DT], d2[DT];
@@ -2212,10 +2229,12 @@ __device__ __forceinline__ void row_face_load(const RowBwdArgs& a, int64_t face,
 #pragma unroll
   for (int d = 0; d < DT; ++d) { c0[d] = Feat<FT>::ld(cf + d); c1[d] = Feat<FT>::ld(cf + DT + d); c2[d] = Feat<FT>::ld(cf + 2 * DT + d); }
   c.ax = pa.x; c.ay = pa.y; c.bx = pb.x; c.by = pb.y; c.cx = pc.x; c.cy = pc.y;
+  c.mx[0] = fmul(pa.x, a.multiplier); c.mx[1] = fmul(pb.x, a.multiplier); c.mx[2] = fmul(pc.x, a.multiplier);
+  c.my[0] = fmul(pa.y, a.multiplier); c.my[1] = fmul(pb.y, a.multiplier); c.my[2] = fmul(pc.y, a.multiplier);
   c.pp = fsub(c.by, c.ay); c.n = fsub(c.cx, c.ax); c.m = fsub(c.bx, c.ax); c.q = fsub(c.cy, c.ay);
   float k3 = ffma(c.m, c.q, -fmul(c.pp, c.n));
   {
-    const double e = (f2u(k3) >> 31) ? -fabs((double)a.eps) : fabs((double)a.eps);
+    const double e = (f2u(k3) >> 31) ? -fabs((double)a.rc.eps) : fabs((double)a.rc.eps);
     k3 = d2f(dibr::dadd((double)k3, e));
   }
   c.k3 = k3;
@@ -2263,7 +2282,7 @@ __device__ __forceinline__ void row_pixel(const RowFace<DT>& c, float aw, float 
 }
 
 #ifndef DIBR_ROWS_MINB
-#define DIBR_ROWS_MINB 16  /* H100, c4_shard: 16 warps/SM 0.63 ms, 12: 0.63, 20: 0.69, 24 (spills): 0.72 */
+#define DIBR_ROWS_MINB 16  /* H100 700 W, c4_shard, weights recomputed: 16 warps/SM 0.452 ms, 12: 0.453, 20: 0.455 */
 #endif
 template <int DT, typename FT>
 __global__ void __launch_bounds__(32, DIBR_ROWS_MINB) raster_bwd_rows_kernel(const __grid_constant__ RowBwdArgs a) {
@@ -2289,6 +2308,8 @@ __global__ void __launch_bounds__(32, DIBR_ROWS_MINB) raster_bwd_rows_kernel(con
   const bool row_ok = row0 + lane < a.H;
   const int64_t pix0 = ((int64_t)b * a.H + row0) * a.W;  // first pixel of the job's first row
   const int64_t fbase = (int64_t)b * a.F;
+  const float y0 = pix_y(a.grid, row0 + lane);                            // the lane's row centre
+  const float* wrow = a.w ? a.w + (pix0 + (int64_t)lane * a.W) * 3 : nullptr;   // given weights
 
   auto issue = [&](int s, int buf) {
     unsigned char* base = smem + buf * G::kStage;
@@ -2300,20 +2321,13 @@ __global__ void __launch_bounds__(32, DIBR_ROWS_MINB) raster_bwd_rows_kernel(con
         cp_async16(base + r * C::kIdxPitch + ch * 16,
                    reinterpret_cast<const char*>(a.idx + pix0 + (int64_t)r * a.W + x) + ch * 16);
     }
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {           // weights: 3 chunks per row
-      const int k = lane + 32 * j, r = k / 3, ch = k - r * 3;
-      if (row0 + r < a.H)
-        cp_async16(base + 32 * C::kIdxPitch + r * C::kWPitch + ch * 16,
-                   reinterpret_cast<const char*>(a.w + (pix0 + (int64_t)r * a.W + x) * 3) + ch * 16);
-    }
     constexpr int GC = G::kRow / G::kChunk;   // upstream gradient: chunks per row
     const FT* gsrc = static_cast<const FT*>(a.grad_feat);
 #pragma unroll
     for (int j = 0; j < GC; ++j) {
       const int k = lane + 32 * j, r = k / GC, ch = k - r * GC;
       if (row0 + r < a.H) {
-        unsigned char* dst = base + 32 * (C::kIdxPitch + C::kWPitch) + r * G::kPitch + ch * G::kChunk;
+        unsigned char* dst = base + 32 * C::kIdxPitch + r * G::kPitch + ch * G::kChunk;
         const char* src = reinterpret_cast<const char*>(gsrc + (pix0 + (int64_t)r * a.W + x) * DT) + ch * G::kChunk;
         if (G::kChunk == 16) cp_async16(dst, src); else cp_async8(dst, src);
       }
@@ -2347,12 +2361,9 @@ __global__ void __launch_bounds__(32, DIBR_ROWS_MINB) raster_bwd_rows_kernel(con
 #pragma unroll
         for (int p = 0; p < 4; ++p) { f[p] = f[p] < 0 ? -1 : f[p]; any = any || f[p] >= 0; }
         if (!any) break;
-        const float4* wp = reinterpret_cast<const float4*>(base + 32 * C::kIdxPitch + lane * C::kWPitch);
-        const float4 w0 = wp[0], w1 = wp[1], w2 = wp[2];
-        const float wv[12] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w, w2.x, w2.y, w2.z, w2.w};
         float gv[4 * DT];
         {
-          const unsigned char* grow = base + 32 * (C::kIdxPitch + C::kWPitch) + lane * G::kPitch;
+          const unsigned char* grow = base + 32 * C::kIdxPitch + lane * G::kPitch;
           if (std::is_same<FT, float>::value) {
             const float4* gp = reinterpret_cast<const float4*>(grow);
 #pragma unroll
@@ -2378,7 +2389,17 @@ __global__ void __launch_bounds__(32, DIBR_ROWS_MINB) raster_bwd_rows_kernel(con
               for (int i = 0; i < C::kAcc; ++i) acc[i] = 0.f;
             }
           }
-          if (cur >= 0) row_pixel<DT>(fc, wv[3 * p], wv[3 * p + 1], wv[3 * p + 2], &gv[DT * p], acc);
+          if (cur >= 0) {
+            const int x = col0 + s * kRwSlab + p;
+            float aw, bw, cw;
+            if (wrow) {
+              aw = __ldcs(wrow + 3 * x); bw = __ldcs(wrow + 3 * x + 1); cw = __ldcs(wrow + 3 * x + 2);
+            } else {
+              raster_weights_of(a.rc, pix_x(a.grid, x), y0, fc.mx[0], fc.my[0], fc.mx[1], fc.my[1],
+                                fc.mx[2], fc.my[2], aw, bw, cw);
+            }
+            row_pixel<DT>(fc, aw, bw, cw, &gv[DT * p], acc);
+          }
         }
       } while (false);
     }
@@ -2728,7 +2749,7 @@ int launch_raster_bwd_rows(const RasterBwdArgs& r, float* acc, int accumulate_xy
   RowBwdArgs a;
   a.B = r.B; a.H = r.H; a.W = r.W; a.F = r.F;
   a.grad_feat = r.grad_feat; a.idx = r.idx; a.w = r.w; a.xy = r.xy;
-  a.feat = r.feat; a.eps = r.eps; a.acc = acc;
+  a.feat = r.feat; a.grid = r.grid; a.rc = r.rc; a.multiplier = r.multiplier; a.acc = acc;
   a.jobs_y = (r.H + 31) / 32;
   int strip = 32;   // H100, c4_shard: strips of 16 / 64 columns 1 % faster / 8 % slower
   if (const char* fs = getenv("DIBR_B200_ROWS_STRIP")) { const int v = atoi(fs); if (v >= kRwSlab && v % kRwSlab == 0) strip = v; }
@@ -2883,9 +2904,9 @@ static int forward_impl(int batch, int num_faces, int height, int width, int fea
   const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
   if ((!raster && !soft) || num_faces < 0 || feat_dim < 0 || !face_idx) return DIBR_B200_EINVAL;
   if (num_faces > 0 && !face_vertices_image) return DIBR_B200_EINVAL;
-  if (raster && (!output_weights || (feat_dim > 0 && (!interpolated_features || (num_faces > 0 && !face_features))) ||
+  if (raster && ((feat_dim > 0 && (!interpolated_features || (num_faces > 0 && !face_features))) ||
                  (num_faces > 0 && !face_vertices_z)))
-    return DIBR_B200_EINVAL;
+    return DIBR_B200_EINVAL;   // output_weights may be NULL: nothing is written there then
   if (soft && (!soft_mask || knum <= 0)) return DIBR_B200_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   FwdArgs a;
@@ -2975,16 +2996,18 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
   }
   if (NF == 0) return 0;
   if (run_raster) {
-    if (!output_weights || !face_features || !grad_face_features) return DIBR_B200_EINVAL;
+    if (!face_features || !grad_face_features) return DIBR_B200_EINVAL;
+    if (!output_weights && !(multiplier > 0.f)) return DIBR_B200_EINVAL;
     RasterBwdArgs a;
     const size_t px0 = (size_t)view_begin * height * width;
     a.B = nv; a.H = height; a.W = width; a.F = num_faces; a.D = feat_dim;
     a.ntx = (width + kTile - 1) / kTile; a.nty = (height + kTile - 1) / kTile;
     a.grad_feat = static_cast<const char*>(grad_features) + px0 * feat_dim * fsz;
-    a.idx = face_idx + px0; a.w = output_weights + px0 * 3;
+    a.idx = face_idx + px0; a.w = output_weights ? output_weights + px0 * 3 : nullptr;
     a.xy = face_vertices_image + (size_t)view_begin * num_faces * 6;
     a.feat = static_cast<const char*>(face_features) + (size_t)view_begin * num_faces * 3 * feat_dim * fsz;
-    a.eps = eps; a.grad_xy = g_xy_v;
+    a.grid = make_grid(multiplier, width, height); a.rc = make_raster_const(eps); a.multiplier = multiplier;
+    a.grad_xy = g_xy_v;
     a.grad_feat_out = g_ff_v;
     if (acc) rc = bf16 ? launch_raster_bwd_rows<__nv_bfloat16>(a, acc, (flags & DIBR_B200_ACCUMULATE) ? 1 : 0, st)
                        : launch_raster_bwd_rows<float>(a, acc, (flags & DIBR_B200_ACCUMULATE) ? 1 : 0, st);
@@ -3111,6 +3134,8 @@ int dibr_b200_rasterize_backward(int batch, int num_faces, int height, int width
                                  float eps, float* grad_face_vertices_image,
                                  float* grad_face_features, dibr_b200_stream_t stream) {
   if (!grad_interpolated_features && feat_dim > 0) return DIBR_B200_EINVAL;
+  // the packed forward's xy is premultiplied, so its weights cannot be recomputed here
+  if (!output_weights && feat_dim > 0) return DIBR_B200_EINVAL;
   // workspace is not needed for the rasterize branch
   return dibr_b200_backward(batch, num_faces, height, width, feat_dim, grad_interpolated_features,
                             nullptr, selected_face_idx, output_weights, nullptr, face_vertices_image,

@@ -92,7 +92,10 @@ def workspace(batch, total_faces, height, width, device, knum=0):
 
 def forward(mode, height, width, fvz, fvi, ff, fnz, valid_u8, multiplier, eps,
             sigmainv, boxlen_m, knum, face_idx_in=None):
-    """Calls dibr_b200_forward; returns (feat, face_idx, weights, soft, workspace)."""
+    """Calls dibr_b200_forward; returns (feat, face_idx, None, soft, workspace).
+
+    The barycentric weights are not stored (the third slot is always None): the backward
+    recomputes them bit for bit from face_idx, the vertices and the same multiplier and eps."""
     dev = fvi.device
     B, F = fvi.shape[0], fvi.shape[1]
     D = 0 if ff is None else ff.shape[-1]
@@ -101,20 +104,19 @@ def forward(mode, height, width, fvz, fvi, ff, fnz, valid_u8, multiplier, eps,
     bf16 = ff is not None and ff.dtype == torch.bfloat16
     feat = torch.empty((B, height, width, D), dtype=torch.bfloat16 if bf16 else torch.float32,
                        device=dev) if raster else None
-    wts = torch.empty((B, height, width, 3), dtype=torch.float32, device=dev) if raster else None
     idx = torch.empty((B, height, width), dtype=torch.int64, device=dev) if raster else face_idx_in
     soft = torch.empty((B, height, width), dtype=torch.float32, device=dev) if soft_on else None
     if B == 0:       # an empty view shard (batch < world size): empty images, nothing to launch
-        return feat, idx, wts, soft, None
+        return feat, idx, None, soft, None
     ws = workspace(B, B * F, height, width, dev, knum if soft_on else 0)
     with torch.cuda.device(dev):
         fn = _lib.lib().dibr_b200_forward_bf16 if bf16 else _lib.lib().dibr_b200_forward
         st = fn(
             B, F, height, width, D, ptr(fvz), ptr(fvi), ptr(ff), ptr(fnz), ptr(valid_u8),
             float(multiplier), float(eps), mode, float(sigmainv), float(boxlen_m), int(knum),
-            ptr(feat), ptr(idx), ptr(wts), ptr(soft), ptr(ws), ws.numel(), stream_ptr(dev))
+            ptr(feat), ptr(idx), None, ptr(soft), ptr(ws), ws.numel(), stream_ptr(dev))
     _lib.check(st, "dibr_b200_forward")
-    return feat, idx, wts, soft, ws
+    return feat, idx, None, soft, ws
 
 
 
@@ -144,6 +146,9 @@ def _backward_call(B, F, height, width, D, g_feat, g_soft, face_idx, wts, soft, 
 def backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multiplier, eps,
              sigmainv, boxlen_m, knum, ws, bins_valid, feature_grad_hook=None, views=None, out=None):
     """Calls dibr_b200_backward; returns (grad_face_vertices_image, grad_face_features fp32).
+
+    ``wts`` is None after ``forward`` (the kernels recompute the weights; ``multiplier`` and ``eps``
+    must then be the forward's) or the (B,H,W,3) weights of the same forward, which are read.
 
     ``views=(v0, v1)`` restricts the call to those views of the batch (dibr_b200_backward_views: all
     tensors stay the full-batch ones, only rows v0..v1-1 of the gradients are written) and ``out=

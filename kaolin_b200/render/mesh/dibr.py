@@ -165,10 +165,10 @@ class DibrRasterizationB200(Function):
         ff = face_features.contiguous()
         fnz = face_normals_z.contiguous()
         boxlen_m = boxlen * soft_multiplier
-        feat, face_idx, wts, soft, ws = _host.forward(
+        feat, face_idx, _, soft, ws = _host.forward(
             _lib.RASTER | _lib.SOFT_MASK, height, width, fvz, fvi, ff, fnz, None,
             multiplier, eps, sigmainv, boxlen_m, knum)
-        ctx.save_for_backward(face_idx, wts, soft, fvi, ff)
+        ctx.save_for_backward(face_idx, soft, fvi, ff)
         ctx.mark_non_differentiable(face_idx)
         ctx.set_materialize_grads(False)   # no 8 B/pixel zero "gradient" for face_idx
         ctx.params = (height, width, multiplier, eps, sigmainv, boxlen_m, knum)
@@ -178,7 +178,7 @@ class DibrRasterizationB200(Function):
 
     @staticmethod
     def backward(ctx, grad_features, grad_soft_mask, grad_face_idx):
-        face_idx, wts, soft, fvi, ff = ctx.saved_tensors
+        face_idx, soft, fvi, ff = ctx.saved_tensors
         height, width, multiplier, eps, sigmainv, boxlen_m, knum = ctx.params
         g_feat = None if grad_features is None else grad_features.contiguous()
         g_soft = None if grad_soft_mask is None else grad_soft_mask.contiguous()
@@ -189,12 +189,12 @@ class DibrRasterizationB200(Function):
             g_ff = torch.empty(ff.shape, dtype=torch.float32, device=ff.device)
 
             def run_chunk(c0, c1, hook):
-                _host.backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multiplier, eps, sigmainv,
+                _host.backward(height, width, g_feat, g_soft, face_idx, None, soft, fvi, ff, multiplier, eps, sigmainv,
                                boxlen_m, knum, ctx.ws, True, feature_grad_hook=hook, views=(c0, c1), out=(g_fvi, g_ff))
             pipe(fvi.shape[0], run_chunk, g_fvi, g_ff)
             return None, None, None, g_fvi, g_ff.to(ff.dtype), None, None, None, None, None, None, None
         # per-node hook (set on this node by OverlappedGradAllGather.attach, never global)
-        g_fvi, g_ff = _host.backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff,
+        g_fvi, g_ff = _host.backward(height, width, g_feat, g_soft, face_idx, None, soft, fvi, ff,
                                      multiplier, eps, sigmainv, boxlen_m, knum, ctx.ws, ctx.ws is not None,
                                      feature_grad_hook=getattr(ctx, "feature_grad_hook", None))
         g_ff = g_ff.to(ff.dtype)      # fp32 accumulation; autograd wants the input's dtype (bf16 features)

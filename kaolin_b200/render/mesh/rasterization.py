@@ -27,21 +27,22 @@ class RasterizeB200(Function):
         if valid_faces is not None:
             valid_u8 = valid_faces.contiguous()
             valid_u8 = valid_u8.view(torch.uint8) if valid_u8.dtype == torch.bool else valid_u8.ne(0).view(torch.uint8)
-        feat, face_idx, wts, _, _ = _host.forward(
+        feat, face_idx, _, _, _ = _host.forward(
             _lib.RASTER, height, width, fvz, fvi, ff, None, valid_u8, multiplier, eps, 0., 0., 0)
-        ctx.save_for_backward(face_idx, wts, fvi, ff)
+        ctx.save_for_backward(face_idx, fvi, ff)
         ctx.mark_non_differentiable(face_idx)
         ctx.set_materialize_grads(False)   # no 8 B/pixel zero "gradient" for face_idx
+        ctx.multiplier = multiplier        # the backward recomputes the weights with it
         ctx.eps = eps
         ctx.hw = (height, width)
         return feat, face_idx
 
     @staticmethod
     def backward(ctx, grad_interpolated_features, grad_face_idx):
-        face_idx, wts, fvi, ff = ctx.saved_tensors
+        face_idx, fvi, ff = ctx.saved_tensors
         g = grad_interpolated_features.contiguous()
-        g_fvi, g_ff = _host.backward(ctx.hw[0], ctx.hw[1], g, None, face_idx, wts, None, fvi, ff,
-                                     1.0, ctx.eps, 0., 0., 0, None, False)
+        g_fvi, g_ff = _host.backward(ctx.hw[0], ctx.hw[1], g, None, face_idx, None, None, fvi, ff,
+                                     ctx.multiplier, ctx.eps, 0., 0., 0, None, False)
         g_ff = g_ff.to(ff.dtype)      # fp32 accumulation; autograd wants the input's dtype (bf16 features)
         # the reference never produces a gradient for face_vertices_z (rasterization.py:370-371)
         return None, None, None, g_fvi, g_ff, None, None, None
