@@ -351,6 +351,68 @@ int dibr_b200_deftet_sparse_render_backward(
     float* grad_face_vertices_image, float* grad_face_features, dibr_b200_stream_t stream);
 
 /*
+ * Diffuse lighting (kaolin/render/lighting/sg.py, sh.py; kaolin_b200/csrc/lighting.cu).
+ *
+ * General reduced SG inner product, the operator kaolin::unbatched_reduced_sg_inner_product_
+ * {forward,backward}_cuda: sg side amplitude (N,3), direction (N,3), sharpness (N); "other" side
+ * (M,3), (M,3), (M); out (N,3) = sum_m <sg_n, other_m> with, per pair, v = lambda d + Lambda D,
+ * um = |v|, <.,.> = 2 pi a A exp(um - lambda - Lambda) (1 - exp(-2 um)) / um.  The backward writes
+ * any subset of the six gradients; a NULL gradient is not computed.  The "other"-side gradients
+ * need workspace >= dibr_b200_sg_inner_product_workspace_bytes(M) (NULL when none is requested).
+ *
+ * Diffuse shading of N points lit by L lights, `model` one of:
+ *  SG_INNER_PRODUCT  sg_diffuse_inner_product / sg_irradiance_inner_product: the cosine lobe
+ *                    (amplitude 1.17, direction = normal, sharpness 2.133) against each light,
+ *                    summed over lights, clamp(min=0), x albedo/pi.
+ *  SG_FITTED         sg_diffuse_fitted: Stephen Hill's fitted irradiance per (point, light), MEAN over
+ *                    lights, clamp(min=0), x albedo/pi.  L = 0 gives zeros (the reference's mean of an
+ *                    empty set is NaN).
+ *  SH9               sh9_diffuse / sh9_irradiance: sum_k band_k(normal) c_k lights_k, x albedo, no
+ *                    clamp; light_amplitude holds the 9 coefficients and num_lights must be 1.
+ * light_amplitude (L,3), light_direction (L,3), light_sharpness (L); normal (N,3) (not normalised);
+ * albedo (N,3) or NULL.  out (N,3); with albedo == NULL the irradiance alone: (N,3) for the SG
+ * models, (N,) for SH9.  The backward writes grad_normal, grad_albedo (both optional, per point)
+ * and the light gradients (optional; SG: amplitude, direction, sharpness; SH9: the 9 coefficients
+ * in grad_light_amplitude), which need workspace >= dibr_b200_diffuse_workspace_bytes(model, L).
+ *
+ * Light gradients are bit-reproducible: no float atomics; per-CTA partials summed in a fixed order
+ * in fp64.  The workspace does not depend on N: 264 CTA slots x 7 floats per light (SH9: 9 floats)
+ * = 7.4 KB per light.  Per-point data is read once for any L (kept in registers while the lights
+ * are streamed through shared memory); with only light gradients requested the backward reads
+ * grad_out, normal and albedo and writes nothing per point.  Clamp gradients pass where the input is
+ * >= 0, as torch.clamp's do.
+ * The formulas are the reference's, literally, in fp32.  Where the reference itself produces inf or
+ * NaN the result is unspecified: um = 0 (opposite directions of equal sharpness), sharpness 0, and
+ * sharpness so small that sqrt(1 - scale) is 0 in the fitted model.
+ */
+#define DIBR_B200_LIGHT_SG_INNER_PRODUCT 0
+#define DIBR_B200_LIGHT_SG_FITTED 1
+#define DIBR_B200_LIGHT_SH9 2
+
+size_t dibr_b200_sg_inner_product_workspace_bytes(int num_other);
+int dibr_b200_sg_inner_product_forward(
+    int64_t num_sg, int num_other, const float* amplitude, const float* direction, const float* sharpness,
+    const float* other_amplitude, const float* other_direction, const float* other_sharpness, float* out,
+    dibr_b200_stream_t stream);
+int dibr_b200_sg_inner_product_backward(
+    int64_t num_sg, int num_other, const float* grad_out, const float* amplitude, const float* direction,
+    const float* sharpness, const float* other_amplitude, const float* other_direction,
+    const float* other_sharpness, float* grad_amplitude, float* grad_direction, float* grad_sharpness,
+    float* grad_other_amplitude, float* grad_other_direction, float* grad_other_sharpness,
+    void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+size_t dibr_b200_diffuse_workspace_bytes(int model, int num_lights);
+int dibr_b200_diffuse_forward(
+    int model, int64_t num_points, int num_lights, const float* light_amplitude, const float* light_direction,
+    const float* light_sharpness, const float* normal, const float* albedo, float* out,
+    dibr_b200_stream_t stream);
+int dibr_b200_diffuse_backward(
+    int model, int64_t num_points, int num_lights, const float* light_amplitude, const float* light_direction,
+    const float* light_sharpness, const float* normal, const float* albedo, const float* grad_out,
+    float* grad_normal, float* grad_albedo, float* grad_light_amplitude, float* grad_light_direction,
+    float* grad_light_sharpness, void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
  * Exchange step of the view-sharded path (SURVEY.md 8e; kaolin_b200/csrc/peer_push.cu): the
  * reference has no multi-GPU code - its callers all-gather the per-view gradients with
  * torch.distributed.  All-gather by STORES over NVLink: copies `bytes` (multiple of 16) from the

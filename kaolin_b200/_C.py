@@ -250,8 +250,50 @@ def deftet_sparse_render_backward_cuda(grad_interpolated_features, face_idx, wei
     return [g_xy, g_ff]
 
 
-# kaolin._C.render.mesh.<op> namespace, as bindings.cpp:42,111-115 lays it out
-render = types.SimpleNamespace(mesh=types.SimpleNamespace(
+def _check_sg(fn, named):
+    """unbatched_reduced_sg_inner_product.cpp:57-103: same GPU, contiguous, same type, sizes."""
+    dev = _check_all(fn, named)
+    dtypes = {t.dtype for _, t in named}
+    if len(dtypes) > 1:
+        raise RuntimeError(f"{fn}: expected all tensors to have the same type, got {sorted(map(str, dtypes))}")
+    t = dict(named)
+    num_sg, num_other = t["intensity"].shape[0], t["other_intensity"].shape[0]
+    for name, shape in (("grad_out", (num_sg, 3)), ("intensity", (num_sg, 3)), ("direction", (num_sg, 3)),
+                        ("sharpness", (num_sg,)), ("other_intensity", (num_other, 3)),
+                        ("other_direction", (num_other, 3)), ("other_sharpness", (num_other,))):
+        if name in t:
+            _check_size(fn, name, t[name], shape)
+    return dev
+
+
+def unbatched_reduced_sg_inner_product_forward_cuda(intensity, direction, sharpness,
+                                                    other_intensity, other_direction, other_sharpness):
+    """unbatched_reduced_sg_inner_product.cpp:49-123 -> output (num_sg, 3)."""
+    from .render.lighting import sg
+    args = [("intensity", intensity), ("direction", direction), ("sharpness", sharpness),
+            ("other_intensity", other_intensity), ("other_direction", other_direction),
+            ("other_sharpness", other_sharpness)]
+    _check_sg("unbatched_reduced_sg_inner_product_forward_cuda", args)
+    return sg.forward_sg_inner_product(*[t for _, t in args])
+
+
+def unbatched_reduced_sg_inner_product_backward_cuda(grad_out, intensity, direction, sharpness,
+                                                     other_intensity, other_direction, other_sharpness):
+    """unbatched_reduced_sg_inner_product.cpp:125-218 -> [grad_intensity, grad_direction, grad_sharpness,
+    grad_other_intensity, grad_other_direction, grad_other_sharpness]."""
+    from .render.lighting import sg
+    args = [("grad_out", grad_out), ("intensity", intensity), ("direction", direction), ("sharpness", sharpness),
+            ("other_intensity", other_intensity), ("other_direction", other_direction),
+            ("other_sharpness", other_sharpness)]
+    _check_sg("unbatched_reduced_sg_inner_product_backward_cuda", args)
+    return sg.backward_sg_inner_product(*[t for _, t in args])
+
+
+# kaolin._C.render.{mesh,sg}.<op> namespaces, as bindings.cpp:42,111-115,129-133 lays them out
+render = types.SimpleNamespace(sg=types.SimpleNamespace(
+    unbatched_reduced_sg_inner_product_forward_cuda=unbatched_reduced_sg_inner_product_forward_cuda,
+    unbatched_reduced_sg_inner_product_backward_cuda=unbatched_reduced_sg_inner_product_backward_cuda,
+), mesh=types.SimpleNamespace(
     packed_rasterize_forward_cuda=packed_rasterize_forward_cuda,
     rasterize_backward_cuda=rasterize_backward_cuda,
     dibr_soft_mask_forward_cuda=dibr_soft_mask_forward_cuda,

@@ -14,7 +14,8 @@ CSRC = os.path.join(_HERE, "csrc")
 # DIBR_B200_LIB: an alternative build of the same sources (A/B experiments on the GPU box only)
 LIB_PATH = os.environ.get("DIBR_B200_LIB") or os.path.join(CSRC, "libdibr_b200.so")
 SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline.cu"),
-           os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu")]
+           os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
+           os.path.join(CSRC, "lighting.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"),
            os.path.join(_HERE, "..", "include", "dibr_b200.h")]
@@ -23,6 +24,7 @@ NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "
 
 EINVAL, EWORKSPACE, ESIZE = -1, -3, -4
 RASTER, SOFT_MASK = 1, 2
+LIGHT_SG_INNER_PRODUCT, LIGHT_SG_FITTED, LIGHT_SH9 = 0, 1, 2     # dibr_b200_diffuse_* models
 BINS_VALID, ACCUMULATE = 1, 2      # dibr_b200_backward flags
 
 _lock = threading.Lock()
@@ -81,6 +83,15 @@ SIGNATURES = {
                                                     _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dibr_b200_deftet_sparse_render_backward": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _f,
                                                      _vp, _vp, _vp]),
+    # diffuse lighting after the rasterizer (csrc/lighting.cu)
+    "dibr_b200_sg_inner_product_workspace_bytes": (_sz, [_i]),
+    "dibr_b200_sg_inner_product_forward": (_i, [_i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dibr_b200_sg_inner_product_backward": (_i, [_i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                 _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dibr_b200_diffuse_workspace_bytes": (_sz, [_i, _i]),
+    "dibr_b200_diffuse_forward": (_i, [_i, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dibr_b200_diffuse_backward": (_i, [_i, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                        _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

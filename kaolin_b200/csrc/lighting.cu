@@ -1,0 +1,674 @@
+// lighting.cu — diffuse shading right after the rasterizer (kaolin/render/lighting/sg.py, sh.py),
+// behind the C ABI of include/dibr_b200.h:
+//
+//   general reduced SG inner product   out(N,3) = sum_m <sg_n, other_m>     (the _C.render.sg operator)
+//   SG_INNER_PRODUCT                    per-point cosine lobe (1.17, normal, 2.133) . lights, clamp, albedo/pi
+//   SG_FITTED                           Stephen Hill's fitted irradiance, mean over lights, clamp, albedo/pi
+//   SH9                                 sum_k band_k(normal) c_k lights_k, x albedo
+//
+// One kernel template per direction, instantiated per Kind; the general op and SG_INNER_PRODUCT
+// differ only in where the sg side comes from (per-point arrays or the cosine lobe of the normal)
+// and in the epilogue (none, or clamp + albedo/pi).
+//
+// Layout of the work: a CTA of 256 threads takes tiles of 1024 points, four consecutive points per
+// thread, so that the 12-byte rows of a thread's points are three 16-byte loads (scalar loads when
+// the base is not 16-byte aligned or the tile is partial).  The point data stays in registers for
+// the whole light loop: it is read from HBM exactly once for every L.  Lights are staged in shared
+// memory 64 at a time, with the per-light terms the formulas share precomputed in fp32; with L <= 64
+// they are staged once per CTA, above that once per tile and chunk (from L2).
+//
+// Light gradients are deterministic: the backward grid has a fixed number of CTAs for a given N,
+// each warp sums its four-point partials with a fixed shuffle tree, the eight warps are summed in
+// warp order into a per-CTA slot of the workspace, and a finalize kernel sums the CTA slots in CTA
+// order in fp64.  No float atomics are used anywhere.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "../../include/dibr_b200.h"
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+constexpr int kPts = 4;                     // points per thread per tile
+constexpr int kTile = kThreads * kPts;
+constexpr int kChunk = 64;                  // lights staged in shared memory at a time
+constexpr int kFwdCtas = 132 * 4;           // persistent grids: 4 CTAs on each of H100's 132 SMs
+constexpr int kBwdCtas = 132 * 2;           // 2 resident CTAs per SM (__launch_bounds__ below); also the
+                                            // number of per-CTA partial slots in the workspace
+constexpr float kPi = 3.14159265358979323846f;
+constexpr float kTwoPi = 6.28318530717958647692f;
+
+enum Kind { GENERAL = 0, LOBE = 1, FITTED = 2, SH9 = 3 };
+
+template <int K> struct Cfg {
+  static constexpr int kIn = K == GENERAL ? 7 : 3;                   // per-point floats in registers
+  static constexpr int kRec = (K == GENERAL || K == LOBE) ? 8 : 16;  // floats per staged light
+  static constexpr int kAcc = K == SH9 ? 9 : 7;                      // per-light gradient partials
+};
+
+struct Args {
+  int64_t n;
+  int L;
+  const float* p_amp; const float* p_dir; const float* p_sharp;   // GENERAL: the sg side
+  const float* normal; const float* albedo;                         // shading models
+  const float* l_amp; const float* l_dir; const float* l_sharp;   // lights / "other" (SH9: l_amp = 9 coefficients)
+  float* out;
+  const float* grad_out;
+  float* g_amp; float* g_dir; float* g_sharp;                       // GENERAL: sg-side gradients
+  float* g_normal; float* g_albedo;
+  float* gl_amp; float* gl_dir; float* gl_sharp;                    // light gradients
+  float* partial;                                                   // [grid][L][kAcc]
+};
+
+// ---------------------------------------------------------------------------------------------
+// 4-point row loads / stores: three (C = 3) or one (C = 1) 16-byte accesses when aligned.
+template <int C>
+__device__ __forceinline__ void load_rows(const float* __restrict__ base, int64_t p0, int64_t n, float (&v)[kPts][C]) {
+  const float* src = base + p0 * C;
+  if (p0 + kPts <= n && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
+#pragma unroll
+    for (int q = 0; q < C; ++q) {
+      const float4 t = __ldg(reinterpret_cast<const float4*>(src) + q);
+      v[(4 * q) / C][(4 * q) % C] = t.x;
+      v[(4 * q + 1) / C][(4 * q + 1) % C] = t.y;
+      v[(4 * q + 2) / C][(4 * q + 2) % C] = t.z;
+      v[(4 * q + 3) / C][(4 * q + 3) % C] = t.w;
+    }
+  } else {
+#pragma unroll
+    for (int p = 0; p < kPts; ++p)
+#pragma unroll
+      for (int c = 0; c < C; ++c) v[p][c] = (p0 + p < n) ? __ldg(src + p * C + c) : 0.f;
+  }
+}
+
+template <int C>
+__device__ __forceinline__ void store_rows(float* __restrict__ base, int64_t p0, int64_t n, const float (&v)[kPts][C]) {
+  float* dst = base + p0 * C;
+  if (p0 + kPts <= n && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+#pragma unroll
+    for (int q = 0; q < C; ++q)
+      reinterpret_cast<float4*>(dst)[q] = make_float4(v[(4 * q) / C][(4 * q) % C], v[(4 * q + 1) / C][(4 * q + 1) % C],
+                                                      v[(4 * q + 2) / C][(4 * q + 2) % C], v[(4 * q + 3) / C][(4 * q + 3) % C]);
+  } else {
+#pragma unroll
+    for (int p = 0; p < kPts; ++p)
+      if (p0 + p < n)
+#pragma unroll
+        for (int c = 0; c < C; ++c) dst[p * C + c] = v[p][c];
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Light staging: record m of the current chunk from light `l`.
+template <int K>
+__device__ __forceinline__ void stage_light(const Args& a, int l, float* rec) {
+  if (K == SH9) {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) rec[k] = __ldg(a.l_amp + k);
+  } else if (K == FITTED) {
+    const float lb = __ldg(a.l_sharp + l);
+    const float eml = expf(-lb), em2l = eml * eml, rl = 1.f / lb;
+    const float scale = 1.f + 2.f * em2l - rl;
+    const float bias = (eml - em2l) * rl - em2l;
+    const float x = sqrtf(1.f - scale);
+    const float dscale = -4.f * em2l + rl * rl;
+    const float dbias = (2.f * em2l - eml) * rl - (eml - em2l) * rl * rl + 2.f * em2l;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      rec[k] = __ldg(a.l_dir + 3 * l + k);
+      rec[3 + k] = kTwoPi * (__ldg(a.l_amp + 3 * l + k) / lb);
+    }
+    rec[6] = scale; rec[7] = bias; rec[8] = x; rec[9] = (1.f / (4.f * 0.36f)) * x;
+    rec[10] = rl; rec[11] = dscale; rec[12] = dbias; rec[13] = -dscale / (2.f * x);
+    rec[14] = kTwoPi / lb; rec[15] = 0.f;
+  } else {
+    const float lb = __ldg(a.l_sharp + l);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      rec[k] = __ldg(a.l_amp + 3 * l + k);
+      rec[3 + k] = __ldg(a.l_dir + 3 * l + k) * lb;
+    }
+    rec[6] = lb; rec[7] = 0.f;
+  }
+}
+
+// Stage lights [c0, c0 + cnt) into shared memory (caller synchronises).
+template <int K>
+__device__ __forceinline__ void stage_chunk(const Args& a, int c0, int cnt, float* s_light) {
+  for (int m = threadIdx.x; m < cnt; m += kThreads) stage_light<K>(a, c0 + m, s_light + m * Cfg<K>::kRec);
+}
+
+// ---------------------------------------------------------------------------------------------
+// SG inner product of one (sg, other) pair: v = lambda d + Lambda D, lm = lambda + Lambda.
+struct SgTerm { float um, E, X, c; };
+
+__device__ __forceinline__ SgTerm sg_term(float vx, float vy, float vz, float lm) {
+  SgTerm t;
+  t.um = sqrtf(vx * vx + vy * vy + vz * vz);
+  t.E = expf(t.um - lm);
+  t.X = expf(-2.f * t.um);
+  t.c = kTwoPi * t.E * (1.f - t.X) / t.um;
+  return t;
+}
+
+// The sg side of point p: GENERAL reads it, LOBE builds the cosine lobe of the normal.
+template <int K>
+__device__ __forceinline__ void sg_side(const float* in, float* amp, float* dir, float& sharp) {
+  if constexpr (K == GENERAL) {
+    amp[0] = in[0]; amp[1] = in[1]; amp[2] = in[2];
+    dir[0] = in[3]; dir[1] = in[4]; dir[2] = in[5];
+    sharp = in[6];
+  } else {
+    amp[0] = amp[1] = amp[2] = 1.17f;
+    dir[0] = in[0]; dir[1] = in[1]; dir[2] = in[2];
+    sharp = 2.133f;
+  }
+}
+
+struct Fit { float mu, x0, nn, y; bool b; };
+
+__device__ __forceinline__ Fit fitted_term(const float* n, const float* r) {
+  Fit f;
+  f.mu = n[0] * r[0] + n[1] * r[1] + n[2] * r[2];
+  f.x0 = 0.36f * f.mu;
+  f.nn = f.x0 + r[9];
+  f.b = fabsf(f.x0) <= r[9];
+  f.y = f.b ? f.nn * f.nn / r[8] : fminf(fmaxf(f.mu, 0.f), 1.f);
+  return f;
+}
+
+// SH9 bands of a (not necessarily unit) normal, times the band constants c_k.
+__device__ __forceinline__ void sh9_bands(const float* n, float* b) {
+  const float x = n[0], y = n[1], z = n[2];
+  const float b1 = 2.f * kPi / 3.f, b2 = kPi / 4.f;
+  b[0] = 0.28209479177f * kPi;
+  b[1] = (-0.4886025119f * y) * b1;
+  b[2] = (0.4886025119f * z) * b1;
+  b[3] = (-0.4886025119f * x) * b1;
+  b[4] = (1.0925484305920792f * (x * y)) * b2;
+  b[5] = (-1.0925484305920792f * (y * z)) * b2;
+  b[6] = (0.94617469575f * (z * z) - 0.31539156525f) * b2;
+  b[7] = ((-1.0925484305920792f * x) * z) * b2;
+  b[8] = (0.5462742152960396f * (x * x - y * y)) * b2;
+}
+
+// Forward contribution of one light to the pre-epilogue sum of one point.
+template <int K>
+__device__ __forceinline__ void pair_fwd(const float* in, const float* r, float* acc) {
+  if constexpr (K == FITTED) {
+    const Fit f = fitted_term(in, r);
+    const float res = r[6] * f.y + r[7];
+    acc[0] += res * r[3]; acc[1] += res * r[4]; acc[2] += res * r[5];
+  } else if constexpr (K == SH9) {
+    float b[9];
+    sh9_bands(in, b);
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) s += b[k] * r[k];
+    acc[0] += s;
+  } else {
+    float amp[3], dir[3], sh;
+    sg_side<K>(in, amp, dir, sh);
+    const SgTerm t = sg_term(sh * dir[0] + r[3], sh * dir[1] + r[4], sh * dir[2] + r[5], sh + r[6]);
+    acc[0] += amp[0] * r[0] * t.c; acc[1] += amp[1] * r[1] * t.c; acc[2] += amp[2] * r[2] * t.c;
+  }
+}
+
+// Backward of one (point, light) pair: gpre = d loss / d pre-epilogue sum.  Adds the light's
+// partials to la[kAcc] and, when `point` is set, the point's gradient to pg[kIn].
+template <int K>
+__device__ __forceinline__ void pair_bwd(const float* in, const float* gpre, const float* r, float* la, float* pg, bool point) {
+  if constexpr (K == FITTED) {
+    const Fit f = fitted_term(in, r);
+    const float res = r[6] * f.y + r[7];
+    const float G = gpre[0] * r[3] + gpre[1] * r[4] + gpre[2] * r[5];
+    const float dydmu = f.b ? 2.f * f.nn * 0.36f / r[8] : ((f.mu >= 0.f && f.mu <= 1.f) ? 1.f : 0.f);
+    const float dydl = f.b ? r[13] * (f.nn / r[8]) * (2.f * (1.f / (4.f * 0.36f)) - f.nn / r[8]) : 0.f;
+    const float drdl = r[11] * f.y + r[6] * dydl + r[12];
+    const float gmu = G * (r[6] * dydmu);
+    la[0] += gpre[0] * res * r[14]; la[1] += gpre[1] * res * r[14]; la[2] += gpre[2] * res * r[14];
+    la[3] += gmu * in[0]; la[4] += gmu * in[1]; la[5] += gmu * in[2];
+    la[6] += G * drdl - G * res * r[10];
+    if (point) { pg[0] += gmu * r[0]; pg[1] += gmu * r[1]; pg[2] += gmu * r[2]; }
+  } else if constexpr (K == SH9) {
+    float b[9];
+    sh9_bands(in, b);
+#pragma unroll
+    for (int k = 0; k < 9; ++k) la[k] += gpre[0] * b[k];
+    if (point) {
+      const float x = in[0], y = in[1], z = in[2];
+      const float b1 = 2.f * kPi / 3.f, b2 = kPi / 4.f;
+      const float c1 = 0.4886025119f * b1, c2 = 1.0925484305920792f * b2;
+      const float gx = -c1 * r[3] + c2 * y * r[4] - c2 * z * r[7] + 2.f * 0.5462742152960396f * b2 * x * r[8];
+      const float gy = -c1 * r[1] + c2 * x * r[4] - c2 * z * r[5] - 2.f * 0.5462742152960396f * b2 * y * r[8];
+      const float gz = c1 * r[2] - c2 * y * r[5] + 2.f * 0.94617469575f * b2 * z * r[6] - c2 * x * r[7];
+      pg[0] += gpre[0] * gx; pg[1] += gpre[0] * gy; pg[2] += gpre[0] * gz;
+    }
+  } else {
+    float amp[3], dir[3], sh;
+    sg_side<K>(in, amp, dir, sh);
+    const float vx = sh * dir[0] + r[3], vy = sh * dir[1] + r[4], vz = sh * dir[2] + r[5];
+    const SgTerm t = sg_term(vx, vy, vz, sh + r[6]);
+    const float t0 = gpre[0] * amp[0], t1 = gpre[1] * amp[1], t2 = gpre[2] * amp[2];
+    const float Gc = t0 * r[0] + t1 * r[1] + t2 * r[2];
+    const float dcdum = t.c + (2.f * kTwoPi * t.E * t.X - t.c) / t.um;
+    const float s = Gc * dcdum / t.um;
+    const float gx = s * vx, gy = s * vy, gz = s * vz;
+    la[0] += t0 * t.c; la[1] += t1 * t.c; la[2] += t2 * t.c;
+    la[3] += gx; la[4] += gy; la[5] += gz;
+    la[6] += Gc * t.c;
+    if (point) {
+      pg[0] += gx; pg[1] += gy; pg[2] += gz;       // times the sg sharpness at the end
+      if constexpr (K == GENERAL) {
+        pg[3] += gpre[0] * r[0] * t.c; pg[4] += gpre[1] * r[1] * t.c; pg[5] += gpre[2] * r[2] * t.c;
+        pg[6] += dir[0] * gx + dir[1] * gy + dir[2] * gz - Gc * t.c;
+      }
+    }
+  }
+}
+
+template <int K>
+__device__ __forceinline__ void load_points(const Args& a, int64_t p0, float (&in)[kPts][Cfg<K>::kIn]) {
+  if constexpr (K == GENERAL) {
+    float am[kPts][3], di[kPts][3], sh[kPts][1];
+    load_rows<3>(a.p_amp, p0, a.n, am);
+    load_rows<3>(a.p_dir, p0, a.n, di);
+    load_rows<1>(a.p_sharp, p0, a.n, sh);
+#pragma unroll
+    for (int p = 0; p < kPts; ++p) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { in[p][k] = am[p][k]; in[p][3 + k] = di[p][k]; }
+      in[p][6] = sh[p][0];
+    }
+  } else {
+    load_rows<3>(a.normal, p0, a.n, in);
+  }
+}
+
+__device__ __forceinline__ float clamp0(float v) { return v < 0.f ? 0.f : v; }   // torch.clamp(min=0): NaN stays NaN
+
+// ---------------------------------------------------------------------------------------------
+template <int K>
+__global__ void __launch_bounds__(kThreads, 4) lighting_fwd_kernel(Args a) {
+  constexpr int R = Cfg<K>::kRec;
+  __shared__ __align__(16) float s_light[kChunk * R];
+  const int64_t tiles = (a.n + kTile - 1) / kTile;
+  const int nchunks = (a.L + kChunk - 1) / kChunk;
+  if (nchunks == 1) { stage_chunk<K>(a, 0, a.L, s_light); __syncthreads(); }
+  for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int64_t p0 = tile * kTile + (int64_t)threadIdx.x * kPts;
+    float in[kPts][Cfg<K>::kIn];
+    load_points<K>(a, p0, in);
+    float acc[kPts][3] = {};
+    for (int c = 0; c < nchunks; ++c) {
+      const int cnt = min(kChunk, a.L - c * kChunk);
+      if (nchunks > 1) { __syncthreads(); stage_chunk<K>(a, c * kChunk, cnt, s_light); __syncthreads(); }
+      for (int m = 0; m < cnt; ++m) {
+        float r[R];
+#pragma unroll
+        for (int q = 0; q < R / 4; ++q) *reinterpret_cast<float4*>(r + 4 * q) = reinterpret_cast<const float4*>(s_light + m * R)[q];
+#pragma unroll
+        for (int p = 0; p < kPts; ++p) pair_fwd<K>(in[p], r, acc[p]);
+      }
+    }
+    if (K == GENERAL) {
+      store_rows<3>(a.out, p0, a.n, acc);
+    } else if (K == SH9 && !a.albedo) {
+      float o[kPts][1];
+#pragma unroll
+      for (int p = 0; p < kPts; ++p) o[p][0] = acc[p][0];
+      store_rows<1>(a.out, p0, a.n, o);
+    } else {
+      float al[kPts][3] = {};
+      if (a.albedo) load_rows<3>(a.albedo, p0, a.n, al);
+      float o[kPts][3];
+#pragma unroll
+      for (int p = 0; p < kPts; ++p)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          if (K == SH9) { o[p][k] = al[p][k] * acc[p][0]; continue; }
+          const float e = clamp0(K == FITTED ? (a.L > 0 ? acc[p][k] / (float)a.L : 0.f) : acc[p][k]);
+          o[p][k] = a.albedo ? e * (al[p][k] / kPi) : e;
+        }
+      store_rows<3>(a.out, p0, a.n, o);
+    }
+  }
+}
+
+template <int K>
+__global__ void __launch_bounds__(kThreads, 2) lighting_bwd_kernel(Args a) {
+  constexpr int R = Cfg<K>::kRec, A = Cfg<K>::kAcc, I = Cfg<K>::kIn;
+  __shared__ __align__(16) float s_light[kChunk * R];
+  __shared__ float s_red[kWarps][kChunk][A];
+  const int64_t tiles = (a.n + kTile - 1) / kTile;
+  const int nchunks = (a.L + kChunk - 1) / kChunk;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const bool want_light = a.partial != nullptr;
+  const bool want_point = K == GENERAL ? (a.g_amp || a.g_dir || a.g_sharp) : a.g_normal != nullptr;
+  const bool has_albedo = a.albedo != nullptr;
+  // forward sums are needed for the clamp mask (SG models) or for grad_albedo (SH9)
+  const bool need_pre = K == LOBE || K == FITTED || (K == SH9 && a.g_albedo);
+  float* part = want_light ? a.partial + (size_t)blockIdx.x * a.L * A : nullptr;
+  if (want_light)
+    for (int i = threadIdx.x; i < a.L * A; i += kThreads) part[i] = 0.f;
+  if (nchunks == 1) { stage_chunk<K>(a, 0, a.L, s_light); }
+  __syncthreads();
+  for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int64_t p0 = tile * kTile + (int64_t)threadIdx.x * kPts;
+    float in[kPts][I];
+    load_points<K>(a, p0, in);
+    float g[kPts][3] = {}, al[kPts][3] = {};
+    if (K == SH9 && !has_albedo) {        // sh9_irradiance: grad_out is (N,)
+      float g1[kPts][1];
+      load_rows<1>(a.grad_out, p0, a.n, g1);
+#pragma unroll
+      for (int p = 0; p < kPts; ++p) g[p][0] = g1[p][0];
+    } else {
+      load_rows<3>(a.grad_out, p0, a.n, g);
+    }
+    if (has_albedo) load_rows<3>(a.albedo, p0, a.n, al);
+    // phase 1: the pre-epilogue sums
+    float pre[kPts][3] = {};
+    if (need_pre) {
+      for (int c = 0; c < nchunks; ++c) {
+        const int cnt = min(kChunk, a.L - c * kChunk);
+        if (nchunks > 1) { __syncthreads(); stage_chunk<K>(a, c * kChunk, cnt, s_light); __syncthreads(); }
+        for (int m = 0; m < cnt; ++m) {
+          float r[R];
+#pragma unroll
+          for (int q = 0; q < R / 4; ++q) *reinterpret_cast<float4*>(r + 4 * q) = reinterpret_cast<const float4*>(s_light + m * R)[q];
+#pragma unroll
+          for (int p = 0; p < kPts; ++p) pair_fwd<K>(in[p], r, pre[p]);
+        }
+      }
+    }
+    // epilogue backward: gpre = d loss / d pre, and grad_albedo
+    float gpre[kPts][3];
+    float ga[kPts][3];
+#pragma unroll
+    for (int p = 0; p < kPts; ++p) {
+      const bool valid = p0 + p < a.n;
+      if (K == SH9) {
+        gpre[p][0] = has_albedo ? g[p][0] * al[p][0] + g[p][1] * al[p][1] + g[p][2] * al[p][2] : g[p][0];
+        gpre[p][1] = gpre[p][2] = 0.f;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) ga[p][k] = g[p][k] * pre[p][0];
+      } else {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          if (K == GENERAL) { gpre[p][k] = g[p][k]; ga[p][k] = 0.f; continue; }
+          const float x = K == FITTED ? (a.L > 0 ? pre[p][k] / (float)a.L : 0.f) : pre[p][k];
+          const float gE = has_albedo ? g[p][k] * (al[p][k] / kPi) : g[p][k];
+          gpre[p][k] = x >= 0.f ? (K == FITTED ? gE / (float)a.L : gE) : 0.f;
+          ga[p][k] = g[p][k] * clamp0(x) / kPi;
+        }
+      }
+      if (!valid) gpre[p][0] = gpre[p][1] = gpre[p][2] = 0.f;
+    }
+    if (a.g_albedo) store_rows<3>(a.g_albedo, p0, a.n, ga);
+    // phase 2: light partials and per-point gradients
+    float pg[kPts][I] = {};
+    if (want_light || want_point) {
+      for (int c = 0; c < nchunks; ++c) {
+        const int cnt = min(kChunk, a.L - c * kChunk);
+        if (nchunks > 1) { __syncthreads(); stage_chunk<K>(a, c * kChunk, cnt, s_light); __syncthreads(); }
+        for (int m = 0; m < cnt; ++m) {
+          float r[R];
+#pragma unroll
+          for (int q = 0; q < R / 4; ++q) *reinterpret_cast<float4*>(r + 4 * q) = reinterpret_cast<const float4*>(s_light + m * R)[q];
+          float la[A] = {};
+#pragma unroll
+          for (int p = 0; p < kPts; ++p)
+            if (p0 + p < a.n) pair_bwd<K>(in[p], gpre[p], r, la, pg[p], want_point);
+          if (want_light) {
+#pragma unroll
+            for (int j = 0; j < A; ++j) {
+#pragma unroll
+              for (int o = 16; o > 0; o >>= 1) la[j] += __shfl_xor_sync(0xffffffffu, la[j], o);
+            }
+            if (lane == 0)
+#pragma unroll
+              for (int j = 0; j < A; ++j) s_red[warp][m][j] = la[j];
+          }
+        }
+        if (want_light) {
+          __syncthreads();
+          for (int i = threadIdx.x; i < cnt * A; i += kThreads) {
+            const int m = i / A, j = i - m * A;
+            float s = 0.f;
+#pragma unroll
+            for (int w = 0; w < kWarps; ++w) s += s_red[w][m][j];
+            part[(size_t)(c * kChunk + m) * A + j] += s;
+          }
+          __syncthreads();
+        }
+      }
+    }
+    if (want_point) {
+      if constexpr (K == GENERAL) {
+        float o[kPts][3], o1[kPts][1];
+        if (a.g_amp) {
+#pragma unroll
+          for (int p = 0; p < kPts; ++p) { o[p][0] = pg[p][3]; o[p][1] = pg[p][4]; o[p][2] = pg[p][5]; }
+          store_rows<3>(a.g_amp, p0, a.n, o);
+        }
+        if (a.g_dir) {
+#pragma unroll
+          for (int p = 0; p < kPts; ++p) { o[p][0] = in[p][6] * pg[p][0]; o[p][1] = in[p][6] * pg[p][1]; o[p][2] = in[p][6] * pg[p][2]; }
+          store_rows<3>(a.g_dir, p0, a.n, o);
+        }
+        if (a.g_sharp) {
+#pragma unroll
+          for (int p = 0; p < kPts; ++p) o1[p][0] = pg[p][6];
+          store_rows<1>(a.g_sharp, p0, a.n, o1);
+        }
+      } else {
+        float o[kPts][3];
+        const float s = K == LOBE ? 2.133f : 1.f;
+#pragma unroll
+        for (int p = 0; p < kPts; ++p) { o[p][0] = s * pg[p][0]; o[p][1] = s * pg[p][1]; o[p][2] = s * pg[p][2]; }
+        store_rows<3>(a.g_normal, p0, a.n, o);
+      }
+    }
+  }
+}
+
+// Sums the per-CTA partials of each light in CTA order, in fp64, and writes the light gradients.
+template <int K>
+__global__ void __launch_bounds__(128) lighting_finalize_kernel(Args a, int ctas) {
+  constexpr int A = Cfg<K>::kAcc;
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= a.L) return;
+  double s[A];
+#pragma unroll
+  for (int j = 0; j < A; ++j) s[j] = 0.0;
+  for (int c = 0; c < ctas; ++c) {
+    const float* q = a.partial + ((size_t)c * a.L + m) * A;
+#pragma unroll
+    for (int j = 0; j < A; ++j) s[j] += (double)q[j];
+  }
+  if (K == SH9) {
+    if (a.gl_amp)
+#pragma unroll
+      for (int j = 0; j < 9; ++j) a.gl_amp[j] = (float)s[j];
+    return;
+  }
+  if (a.gl_amp)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) a.gl_amp[3 * m + k] = (float)s[k];
+  if (K == FITTED) {
+    if (a.gl_dir)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) a.gl_dir[3 * m + k] = (float)s[3 + k];
+    if (a.gl_sharp) a.gl_sharp[m] = (float)s[6];
+    return;
+  }
+  // v = lambda d + Lambda D:  dL/dD = Lambda sum(gv),  dL/dLambda = D . sum(gv) - sum(Gc c)
+  const double lb = __ldg(a.l_sharp + m);
+  const double D0 = __ldg(a.l_dir + 3 * m), D1 = __ldg(a.l_dir + 3 * m + 1), D2 = __ldg(a.l_dir + 3 * m + 2);
+  if (a.gl_dir)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) a.gl_dir[3 * m + k] = (float)(lb * s[3 + k]);
+  if (a.gl_sharp) a.gl_sharp[m] = (float)(D0 * s[3] + D1 * s[4] + D2 * s[5] - s[6]);
+}
+
+template <int K>
+int launch_fwd(const Args& a, cudaStream_t st) {
+  const int64_t tiles = (a.n + kTile - 1) / kTile;
+  if (tiles == 0) return 0;
+  lighting_fwd_kernel<K><<<(unsigned)(tiles < kFwdCtas ? tiles : kFwdCtas), kThreads, 0, st>>>(a);
+  return (int)cudaGetLastError();
+}
+
+template <int K>
+int launch_bwd(const Args& a, cudaStream_t st) {
+  const int64_t tiles = (a.n + kTile - 1) / kTile;
+  const int ctas = (int)(tiles < kBwdCtas ? tiles : kBwdCtas);
+  if (ctas > 0) lighting_bwd_kernel<K><<<ctas, kThreads, 0, st>>>(a);
+  if (a.partial && a.L > 0) lighting_finalize_kernel<K><<<(a.L + 127) / 128, 128, 0, st>>>(a, ctas);
+  return (int)cudaGetLastError();
+}
+
+size_t partial_bytes(int slots, int lights) { return (size_t)kBwdCtas * (size_t)lights * (size_t)slots * sizeof(float); }
+
+}  // namespace
+
+extern "C" {
+
+size_t dibr_b200_sg_inner_product_workspace_bytes(int num_other) {
+  return num_other < 0 ? 0 : partial_bytes(Cfg<GENERAL>::kAcc, num_other);
+}
+
+int dibr_b200_sg_inner_product_forward(int64_t num_sg, int num_other, const float* amplitude, const float* direction,
+                                       const float* sharpness, const float* other_amplitude,
+                                       const float* other_direction, const float* other_sharpness, float* out,
+                                       dibr_b200_stream_t stream) {
+  if (num_sg < 0 || num_other < 0) return DIBR_B200_EINVAL;
+  if (num_sg == 0) return 0;
+  if (!amplitude || !direction || !sharpness || !out) return DIBR_B200_EINVAL;
+  if (num_other > 0 && (!other_amplitude || !other_direction || !other_sharpness)) return DIBR_B200_EINVAL;
+  Args a = {};
+  a.n = num_sg; a.L = num_other;
+  a.p_amp = amplitude; a.p_dir = direction; a.p_sharp = sharpness;
+  a.l_amp = other_amplitude; a.l_dir = other_direction; a.l_sharp = other_sharpness;
+  a.out = out;
+  return launch_fwd<GENERAL>(a, (cudaStream_t)stream);
+}
+
+int dibr_b200_sg_inner_product_backward(int64_t num_sg, int num_other, const float* grad_out, const float* amplitude,
+                                        const float* direction, const float* sharpness, const float* other_amplitude,
+                                        const float* other_direction, const float* other_sharpness,
+                                        float* grad_amplitude, float* grad_direction, float* grad_sharpness,
+                                        float* grad_other_amplitude, float* grad_other_direction,
+                                        float* grad_other_sharpness, void* workspace, size_t workspace_bytes,
+                                        dibr_b200_stream_t stream) {
+  if (num_sg < 0 || num_other < 0) return DIBR_B200_EINVAL;
+  if (num_sg > 0 && (!grad_out || !amplitude || !direction || !sharpness)) return DIBR_B200_EINVAL;
+  if (num_other > 0 && (!other_amplitude || !other_direction || !other_sharpness)) return DIBR_B200_EINVAL;
+  Args a = {};
+  a.n = num_sg; a.L = num_other;
+  a.p_amp = amplitude; a.p_dir = direction; a.p_sharp = sharpness;
+  a.l_amp = other_amplitude; a.l_dir = other_direction; a.l_sharp = other_sharpness;
+  a.grad_out = grad_out;
+  a.g_amp = grad_amplitude; a.g_dir = grad_direction; a.g_sharp = grad_sharpness;
+  a.gl_amp = grad_other_amplitude; a.gl_dir = grad_other_direction; a.gl_sharp = grad_other_sharpness;
+  if (num_other > 0 && (a.gl_amp || a.gl_dir || a.gl_sharp)) {
+    if (!workspace) return DIBR_B200_EINVAL;
+    if (workspace_bytes < partial_bytes(Cfg<GENERAL>::kAcc, num_other)) return DIBR_B200_EWORKSPACE;
+    a.partial = (float*)workspace;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (num_other == 0) {   // empty sum: every sg-side gradient is zero
+    const size_t b3 = (size_t)num_sg * 3 * sizeof(float);
+    if (grad_amplitude && cudaMemsetAsync(grad_amplitude, 0, b3, st) != cudaSuccess) return (int)cudaGetLastError();
+    if (grad_direction && cudaMemsetAsync(grad_direction, 0, b3, st) != cudaSuccess) return (int)cudaGetLastError();
+    if (grad_sharpness && cudaMemsetAsync(grad_sharpness, 0, b3 / 3, st) != cudaSuccess) return (int)cudaGetLastError();
+    return 0;
+  }
+  return launch_bwd<GENERAL>(a, st);
+}
+
+size_t dibr_b200_diffuse_workspace_bytes(int model, int num_lights) {
+  if (num_lights < 0) return 0;
+  switch (model) {
+    case DIBR_B200_LIGHT_SG_INNER_PRODUCT: return partial_bytes(Cfg<LOBE>::kAcc, num_lights);
+    case DIBR_B200_LIGHT_SG_FITTED: return partial_bytes(Cfg<FITTED>::kAcc, num_lights);
+    case DIBR_B200_LIGHT_SH9: return partial_bytes(Cfg<SH9>::kAcc, 1);
+    default: return 0;
+  }
+}
+
+static int diffuse_args(Args& a, int model, int64_t num_points, int num_lights, const float* light_amplitude,
+                        const float* light_direction, const float* light_sharpness, const float* normal,
+                        const float* albedo) {
+  if (num_points < 0 || num_lights < 0) return DIBR_B200_EINVAL;
+  if (model == DIBR_B200_LIGHT_SH9) {
+    if (num_lights != 1 || !light_amplitude) return DIBR_B200_EINVAL;
+  } else if (model == DIBR_B200_LIGHT_SG_INNER_PRODUCT || model == DIBR_B200_LIGHT_SG_FITTED) {
+    if (num_lights > 0 && (!light_amplitude || !light_direction || !light_sharpness)) return DIBR_B200_EINVAL;
+  } else {
+    return DIBR_B200_EINVAL;
+  }
+  if (num_points > 0 && !normal) return DIBR_B200_EINVAL;
+  a = Args{};
+  a.n = num_points; a.L = num_lights;
+  a.normal = normal; a.albedo = albedo;
+  a.l_amp = light_amplitude; a.l_dir = light_direction; a.l_sharp = light_sharpness;
+  return 0;
+}
+
+int dibr_b200_diffuse_forward(int model, int64_t num_points, int num_lights, const float* light_amplitude,
+                              const float* light_direction, const float* light_sharpness, const float* normal,
+                              const float* albedo, float* out, dibr_b200_stream_t stream) {
+  Args a;
+  const int rc = diffuse_args(a, model, num_points, num_lights, light_amplitude, light_direction, light_sharpness,
+                              normal, albedo);
+  if (rc) return rc;
+  if (num_points > 0 && !out) return DIBR_B200_EINVAL;
+  a.out = out;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (model) {
+    case DIBR_B200_LIGHT_SG_INNER_PRODUCT: return launch_fwd<LOBE>(a, st);
+    case DIBR_B200_LIGHT_SG_FITTED: return launch_fwd<FITTED>(a, st);
+    default: return launch_fwd<SH9>(a, st);
+  }
+}
+
+int dibr_b200_diffuse_backward(int model, int64_t num_points, int num_lights, const float* light_amplitude,
+                               const float* light_direction, const float* light_sharpness, const float* normal,
+                               const float* albedo, const float* grad_out, float* grad_normal, float* grad_albedo,
+                               float* grad_light_amplitude, float* grad_light_direction,
+                               float* grad_light_sharpness, void* workspace, size_t workspace_bytes,
+                               dibr_b200_stream_t stream) {
+  Args a;
+  const int rc = diffuse_args(a, model, num_points, num_lights, light_amplitude, light_direction, light_sharpness,
+                              normal, albedo);
+  if (rc) return rc;
+  if (num_points > 0 && !grad_out) return DIBR_B200_EINVAL;
+  if (grad_albedo && !albedo) return DIBR_B200_EINVAL;
+  a.grad_out = grad_out;
+  a.g_normal = grad_normal; a.g_albedo = grad_albedo;
+  a.gl_amp = grad_light_amplitude;
+  if (model != DIBR_B200_LIGHT_SH9) { a.gl_dir = grad_light_direction; a.gl_sharp = grad_light_sharpness; }
+  if (num_lights > 0 && (a.gl_amp || a.gl_dir || a.gl_sharp)) {
+    if (!workspace) return DIBR_B200_EINVAL;
+    if (workspace_bytes < dibr_b200_diffuse_workspace_bytes(model, num_lights)) return DIBR_B200_EWORKSPACE;
+    a.partial = (float*)workspace;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (num_lights == 0) {   // empty sum: zero irradiance, zero per-point gradients
+    const size_t b3 = (size_t)num_points * 3 * sizeof(float);
+    if (grad_normal && cudaMemsetAsync(grad_normal, 0, b3, st) != cudaSuccess) return (int)cudaGetLastError();
+    if (grad_albedo && cudaMemsetAsync(grad_albedo, 0, b3, st) != cudaSuccess) return (int)cudaGetLastError();
+    return 0;
+  }
+  switch (model) {
+    case DIBR_B200_LIGHT_SG_INNER_PRODUCT: return launch_bwd<LOBE>(a, st);
+    case DIBR_B200_LIGHT_SG_FITTED: return launch_bwd<FITTED>(a, st);
+    default: return launch_bwd<SH9>(a, st);
+  }
+}
+
+}  // extern "C"

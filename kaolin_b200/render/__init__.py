@@ -1,2 +1,3 @@
 from . import mesh  # noqa: F401
 from . import easy_render  # noqa: F401
+from . import lighting  # noqa: F401

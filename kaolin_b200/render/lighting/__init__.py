@@ -1,0 +1,7 @@
+"""kaolin.render.lighting drop-ins: diffuse spherical-Gaussian and SH9 shading on sm_90a kernels."""
+from .sg import (unbatched_reduced_sg_inner_product, sg_irradiance_inner_product,  # noqa: F401
+                 sg_diffuse_inner_product, sg_diffuse_fitted)
+from .sh import project_onto_sh9, sh9_irradiance, sh9_diffuse  # noqa: F401
+
+__all__ = ["unbatched_reduced_sg_inner_product", "sg_irradiance_inner_product", "sg_diffuse_inner_product",
+           "sg_diffuse_fitted", "project_onto_sh9", "sh9_irradiance", "sh9_diffuse"]
