@@ -11,8 +11,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
-# DIBR_B200_LIB: an alternative build of the same sources (A/B experiments on the GPU box only)
-LIB_PATH = os.environ.get("DIBR_B200_LIB") or os.path.join(CSRC, "libdibr_b200.so")
+LIB_PATH = os.path.join(CSRC, "libdibr_b200.so")
 SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline.cu"),
            os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
            os.path.join(CSRC, "lighting.cu")]

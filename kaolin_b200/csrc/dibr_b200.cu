@@ -266,7 +266,7 @@ __device__ __forceinline__ void bin_insert(const Scene& s, BinSmem& sm, int set,
 // AGG = false (sparse meshes, a few faces per tile): plain atomics, no table.
 template <bool FILL, bool AGG>
 __global__ void __launch_bounds__(AGG ? kBinThreadsAgg : kBinThreadsPlain, AGG ? 2 : 4)
-bin_faces_kernel(Scene s, int sets, int warp_agg) {
+bin_faces_kernel(Scene s, int sets) {
   constexpr int kBinThreads = AGG ? kBinThreadsAgg : kBinThreadsPlain;
   __shared__ typename std::conditional<AGG, BinSmem, int>::type sm;
   const int tid = threadIdx.x;
@@ -306,34 +306,11 @@ bin_faces_kernel(Scene s, int sets, int warp_agg) {
     }
     r[set] = bbox_to_rect(s.grid, xmin, ymin, xmax, ymax);
     sp[set] = bin_span(s, r[set], set ? live : valid);
-    const bool small = sp[set].bx1 - sp[set].bx0 <= 1 && sp[set].by1 - sp[set].by0 <= 1;
     bool aggregated = false;
     if constexpr (AGG) {
+      const bool small = sp[set].bx1 - sp[set].bx0 <= 1 && sp[set].by1 - sp[set].by0 <= 1;
       aggregated = __all_sync(kFull, small);
       if (aggregated) bin_insert(s, sm, set, b, sp[set], where[set]);
-    }
-    if (!aggregated && !AGG && warp_agg && __all_sync(kFull, small)) {
-      // sparse meshes: neighbours in the index buffer are neighbours on screen, so the lanes of a
-      // warp hit a handful of distinct counters; lanes that share one are found with match.any
-      // and their leader issues ONE global atomic for all of them
-      aggregated = true;
-      const int lane = tid & 31;
-      const int4 e = make_int4(f, r[set].x_lo | (r[set].x_hi << 16), r[set].y_lo | (r[set].y_hi << 16), 0);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        where[set][k] = -1;
-        const int bx = sp[set].bx0 + (k & 1), by = sp[set].by0 + (k >> 1);
-        const bool on = sp[set].has && bx <= sp[set].bx1 && by <= sp[set].by1;
-        const unsigned act = __ballot_sync(kFull, on);
-        if (!on) continue;
-        const size_t ci = ((size_t)set * s.B + b) * s.NB + s.bin_base[sp[set].l] + by * s.ntx[sp[set].l] + bx;
-        const unsigned peers = __match_any_sync(act, (unsigned long long)ci);
-        const int leader = __ffs(peers) - 1;
-        int base = 0;
-        if (lane == leader) base = atomicAdd(s.cnt + ci, __popc(peers));
-        base = __shfl_sync(peers, base, leader);
-        if (FILL) s.entries[(size_t)set * 4 * s.NF + 4 * fbase + s.off[ci] + base + __popc(peers & ((1u << lane) - 1u))] = e;
-      }
     }
     if (!aggregated) {
       // (also: a warp with a face of the coarsest level spanning more than 2x2 bins)
@@ -1254,8 +1231,8 @@ __global__ void __launch_bounds__(kThreads, 6) dibr_tile_fwd_kernel(const __grid
 // Forward tile kernel, second generation.  Same results as dibr_tile_fwd_kernel; what changed
 // is where the instructions go (in the first generation a large share of the instructions per 8x4
 // pixel block was per-tile fixed work shared by only 8 warps):
-//   * a CTA owns S x S screen tiles (S = 2: 32x32 px) and stages their candidates ONCE
-//     (bin table, TMA rounds, tile cull, face gather, bit matrices); the S*S sub-tiles are
+//   * a CTA owns 2x2 screen tiles (32x32 px) and stages their candidates ONCE
+//     (bin table, TMA rounds, tile cull, face gather, bit matrices); the 4 sub-tiles are
 //     then rasterized one after the other with the first generation's thread -> pixel mapping, so the
 //     soft-mask work list, the hit cache and every consumer keep their 16x16 tiles;
 //   * a face is inserted in up to 2x2 level-0 bins; with several of them under one CTA it is
@@ -1269,10 +1246,10 @@ __global__ void __launch_bounds__(kThreads, 6) dibr_tile_fwd_kernel(const __grid
 //   * the surviving candidates are visited in a WARP-UNIFORM loop (broadcast shared-memory
 //     reads, no per-lane bit walk); the per-pixel decision is still the exact reference
 //     arithmetic of raster_weights, so face_idx stays bit-exact.
-template <int S>
+constexpr int kSide = 2 * kTile;   // CTA tile of dibr_fwd2_kernel, in pixels
+constexpr int kSubs = 4;           // its 16x16 sub-tiles, row-major
+
 struct FwdSmem {
-  static constexpr int kSide = kTile * S;
-  static constexpr int kSubs = S * S;
   int4 stage[2][kChunk];
   float4 cxy0[kChunk];
   float4 cz[kChunk];
@@ -1323,20 +1300,15 @@ __device__ __noinline__ void make_edge_tests(const float v[6], double X0, double
                 : make_float4(INFINITY, 0.f, 0.f, 0.f);           // never culled (also NaN / Inf input)
 }
 
-#ifndef DIBR_FWD2_MINB
 #define DIBR_FWD2_MINB 4   /* H100, c4_shard: 4 CTAs/SM 0.97 ms, 5: 0.98, 6: 1.10, 8: 1.59 */
-#endif
-template <bool RASTER, bool SOFT, bool KLISTS, typename FT, int S>
+template <bool RASTER, bool SOFT, bool KLISTS, typename FT>
 __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(const __grid_constant__ FwdArgs a) {
-  using SM = FwdSmem<S>;
-  constexpr int kSubs = S * S;
-  constexpr int kSide = kTile * S;
   constexpr int kPieces = kSubs + kMaxLevels - 1;
-  __shared__ __align__(128) SM sm;
+  __shared__ __align__(128) FwdSmem sm;
   const Scene& s = a.s;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.z;
-  const int ctx0 = blockIdx.x * S, cty0 = blockIdx.y * S;   // first 16x16 tile of the CTA
+  const int ctx0 = blockIdx.x * 2, cty0 = blockIdx.y * 2;   // first 16x16 tile of the CTA
   const int cta_x0 = ctx0 * kTile, cta_y0 = cty0 * kTile;
   const int64_t fbase = view_fbase(s, b);
 
@@ -1344,7 +1316,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
   if (tid >= 64 && tid < 64 + kSubs) { sm.any_uncovered[tid - 64] = 0; sm.warps_done[tid - 64] = 0; }
   if (tid < 2 * kSubs) {
     const int set = tid / kSubs, sub = tid % kSubs;
-    const int tx = ctx0 + sub % S, ty = cty0 + sub / S;
+    const int tx = ctx0 + sub % 2, ty = cty0 + sub / 2;
     BinRef r; r.ptr = nullptr; r.n = 0;
     if (tx < s.ntx[0] && ty < s.nty[0]) r = tile_bin(s, b, tx, ty, fbase, set, 0);
     sm.bin0[set][sub] = r;
@@ -1358,7 +1330,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
   }
   __syncthreads();
 
-  // the tight bins above the CTA tile as one virtual list: S*S level-0 pieces, then levels 1..
+  // the tight bins above the CTA tile as one virtual list: 4 level-0 pieces, then levels 1..
   auto pn = [&](int p) { return p < kSubs ? sm.bin0[0][p].n : sm.bin[0][p - kSubs + 1].n; };
   int total = 0;
   if (RASTER) {
@@ -1408,7 +1380,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
         reinterpret_cast<float4*>(a.out_soft + pix_row0 + (int64_t)r * s.W)[ch] = zero;   // uncovered, no neighbour yet
       }
       if (tid < kSubs) {   // every pixel is uncovered: file the sub-tiles an enlarged face can reach
-        const int tx = ctx0 + tid % S, ty = cty0 + tid / S;
+        const int tx = ctx0 + tid % 2, ty = cty0 + tid / 2;
         const int nlarge = ((__ldg(s.tile_cnt + ((size_t)b * s.nty[0] + ty) * ((s.ntx[0] + 31) >> 5) + (tx >> 5)) >> (tx & 31)) & 1) +
                            __ldg(s.view_flag + b);
         if (nlarge > 0) {
@@ -1428,7 +1400,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
   }
 
   for (int sub = 0; sub < kSubs; ++sub) {
-    const int sx = sub % S, sy = sub / S;
+    const int sx = sub % 2, sy = sub / 2;
     const int tx = ctx0 + sx, ty = cty0 + sy;
     if (tx >= s.ntx[0] || ty >= s.nty[0]) continue;   // uniform: sub-tile outside the image
     const int lx = ((warp & 1) << 3) | (lane & 7);     // each warp owns an 8x4 pixel block
@@ -1464,19 +1436,17 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
               const int4 e = sm.stage[buf][tid];
               const int x_lo = e.y & 0xffff, x_hi = (int)((unsigned)e.y >> 16);
               const int y_lo = e.z & 0xffff, y_hi = (int)((unsigned)e.z >> 16);
+              // level-0 pieces: the face is also in the neighbouring bins it spans; take it from
+              // the first of its bins inside this CTA only
               bool take = true;
-              if (S > 1) {
-                // level-0 pieces: the face is also in the neighbouring bins it spans; take it from
-                // the first of its bins inside this CTA only
-                const int vi = k * kChunk + tid;
-                int start = 0;
+              const int vi = k * kChunk + tid;
+              int start = 0;
 #pragma unroll
-                for (int p = 0; p < kSubs; ++p) {
-                  const int np = pn(p);
-                  if (vi >= start && vi < start + np)
-                    take = (ctx0 + p % S) == max(x_lo >> 4, ctx0) && (cty0 + p / S) == max(y_lo >> 4, cty0);
-                  start += np;
-                }
+              for (int p = 0; p < kSubs; ++p) {
+                const int np = pn(p);
+                if (vi >= start && vi < start + np)
+                  take = (ctx0 + p % 2) == max(x_lo >> 4, ctx0) && (cty0 + p / 2) == max(y_lo >> 4, cty0);
+                start += np;
               }
               if (take) {
                 const int cx0 = max(x_lo - cta_x0, 0), cx1 = min(x_hi - cta_x0, kSide);
@@ -1686,9 +1656,7 @@ struct SoftFwdSmem {
   int nsoft, nent, pool_slot, npairs;
 };
 
-#ifndef DIBR_SOFT_FWD_MINB
 #define DIBR_SOFT_FWD_MINB 4   /* H100 (400 W), c4_shard: 4 CTAs/SM 0.81 ms, 3: 0.91, 5: 0.88, 6: 1.01 */
-#endif
 __global__ void __launch_bounds__(kThreads, DIBR_SOFT_FWD_MINB) soft_fwd_kernel(const __grid_constant__ FwdArgs a) {
   __shared__ __align__(128) SoftFwdSmem sm;
   const Scene& s = a.s;
@@ -1884,63 +1852,12 @@ __global__ void __launch_bounds__(kThreads) dibr_tile_soft_bwd_kernel(const __gr
   }
 }
 
-template <int N>
-__device__ __forceinline__ void reduce_peers(unsigned peers, float (&v)[N]);
-
-__global__ void __launch_bounds__(kThreads) soft_bwd_dense_kernel(const __grid_constant__ SoftBwdArgs a) {
-  const Scene& s = a.s;
-  const int used = min(*s.pool_ctr, s.pool_tiles);
-  if ((int)blockIdx.x >= used) return;
-  const int4 h = s.pool_hdr[blockIdx.x];  // b, tx, ty, hits
-  if (h.x < a.view_begin || h.x >= a.view_end) return;
-  const size_t E = (size_t)256 * s.pool_K;
-  const uint32_t* blk = s.pool_data + (size_t)blockIdx.x * 3 * E;
-  const int64_t fbase = view_fbase(s, h.x);
-  const int tid = threadIdx.x, lane = tid & 31;
-  uint32_t nface = 0, nprob = 0, nmeta = 0;
-  if (tid < h.w) { nface = __ldcs(blk + tid); nprob = __ldcs(blk + E + tid); nmeta = __ldcs(blk + 2 * E + tid); }
-  for (int base = 0; base < h.w; base += kThreads) {
-    const int t = base + tid;
-    const bool valid = t < h.w;
-    const uint32_t cface = nface, cprob = nprob, meta = nmeta;
-    if (t + kThreads < h.w) {  // next batch of hits: requested before this one is processed
-      nface = __ldcs(blk + t + kThreads); nprob = __ldcs(blk + E + t + kThreads);
-      nmeta = __ldcs(blk + 2 * E + t + kThreads);
-    }
-    int face = -1 - lane;
-    float g[6];
-#pragma unroll
-    for (int q = 0; q < 6; ++q) g[q] = 0.f;
-    if (valid) {
-      face = (int)cface;
-      const float prob = __uint_as_float(cprob);
-      const int px = h.y * kTile + (int)(meta & 15u), py = h.z * kTile + (int)((meta >> 4) & 15u);
-      const int64_t pix = ((int64_t)h.x * s.H + py) * s.W + px;
-      float v[6];
-      load_xy(s, fbase + face, v);
-      soft_backward_terms(pix_x(s.grid, px), pix_y(s.grid, py), v, (int)(meta >> 8) - 1, prob,
-                          __ldg(a.soft + pix), __ldg(a.grad_soft + pix), a.sigmainv, s.multiplier, g);
-    }
-    // hits were appended candidate by candidate: neighbouring lanes mostly share the face
-    const unsigned peers = __match_any_sync(kFull, face);
-    reduce_peers<6>(peers, g);
-    if (valid && (peers & ((1u << lane) - 1u)) == 0) {
-      float2* gx = reinterpret_cast<float2*>(a.grad_xy + (fbase + face) * 6);
-      if (g[0] != 0.f || g[1] != 0.f) atomicAdd(gx, make_float2(g[0], g[1]));
-      if (g[2] != 0.f || g[3] != 0.f) atomicAdd(gx + 1, make_float2(g[2], g[3]));
-      if (g[4] != 0.f || g[5] != 0.f) atomicAdd(gx + 2, make_float2(g[4], g[5]));
-    }
-  }
-}
-
-// Dense soft-mask backward, RUN variant: the hits of a tile lie face-major in its cache block, so
-// a thread that takes 8 CONSECUTIVE hits (two LDG.128 per array, 32 bytes per lane, 1 KB per warp
-// request) sees one or two faces.  It sums the six partials of a face in registers and flushes
-// them with three RED.v2 when the face changes - no match/shuffle reduction (30 SHFL per warp at
-// 1 SHFL per clock per SM in the kernel above) and one face-vertex load per run instead of per hit.
-#ifndef DIBR_SBWD_MINB
+// Dense soft-mask backward over the hit cache: the hits of a tile lie face-major in its cache
+// block, so a thread that takes 8 CONSECUTIVE hits (two LDG.128 per array, 32 bytes per lane, 1 KB
+// per warp request) sees one or two faces.  It sums the six partials of a face in registers and
+// flushes them with three RED.v2 when the face changes - no match/shuffle reduction (30 SHFL per
+// warp at 1 SHFL per clock per SM) and one face-vertex load per run instead of per hit.
 #define DIBR_SBWD_MINB 4   /* H100, c4_shard: 4 CTAs/SM 0.34 ms, 3: 0.38, 5: 0.35, 6: 0.36 */
-#endif
 __global__ void __launch_bounds__(kThreads, DIBR_SBWD_MINB) soft_bwd_runs_kernel(const __grid_constant__ SoftBwdArgs a) {
   const Scene& s = a.s;
   const int used = min(*s.pool_ctr, s.pool_tiles);
@@ -2281,9 +2198,7 @@ __device__ __forceinline__ void row_pixel(const RowFace<DT>& c, float aw, float 
   }
 }
 
-#ifndef DIBR_ROWS_MINB
 #define DIBR_ROWS_MINB 16  /* H100 700 W, c4_shard, weights recomputed: 16 warps/SM 0.452 ms, 12: 0.453, 20: 0.455 */
-#endif
 template <int DT, typename FT>
 __global__ void __launch_bounds__(32, DIBR_ROWS_MINB) raster_bwd_rows_kernel(const __grid_constant__ RowBwdArgs a) {
   using C = RwCfg<DT>;
@@ -2583,15 +2498,13 @@ int build_bins(const Scene& s, int sets, cudaStream_t st) {
   if (e != cudaSuccess) return (int)e;
   if (s.NF > 0) {
     const bool agg = s.NF / s.B >= (int64_t)32 * s.ntx[0] * s.nty[0];
-    const char* fb = getenv("DIBR_B200_BIN");          // "warp": match.any-aggregated atomics (an A/B switch)
-    const int warp_agg = (fb && fb[0] == 'w') ? 1 : 0;
     const int threads = agg ? kBinThreadsAgg : kBinThreadsPlain;
     const unsigned blocks = (unsigned)((s.NF + threads - 1) / threads);
     // dense meshes (tens of faces per 16x16 tile) hammer a few counters: aggregate per CTA
     {
       Span sp("bin_faces_kernel<count>", st);
-      if (agg) bin_faces_kernel<false, true><<<blocks, threads, 0, st>>>(s, sets, 0);
-      else bin_faces_kernel<false, false><<<blocks, threads, 0, st>>>(s, sets, warp_agg);
+      if (agg) bin_faces_kernel<false, true><<<blocks, threads, 0, st>>>(s, sets);
+      else bin_faces_kernel<false, false><<<blocks, threads, 0, st>>>(s, sets);
     }
     {
       Span sp("scan_bins_kernel", st);
@@ -2599,8 +2512,8 @@ int build_bins(const Scene& s, int sets, cudaStream_t st) {
     }
     {
       Span sp("bin_faces_kernel<fill>", st);
-      if (agg) bin_faces_kernel<true, true><<<blocks, threads, 0, st>>>(s, sets, 0);
-      else bin_faces_kernel<true, false><<<blocks, threads, 0, st>>>(s, sets, warp_agg);
+      if (agg) bin_faces_kernel<true, true><<<blocks, threads, 0, st>>>(s, sets);
+      else bin_faces_kernel<true, false><<<blocks, threads, 0, st>>>(s, sets);
     }
   }
   return (int)cudaGetLastError();
@@ -2645,27 +2558,21 @@ void launch_fwd(const FwdArgs& a0, cudaStream_t st) {
   FwdArgs a = a0;
   a.from_fb = 0;
   {
-    // S = 2 (32x32 px per CTA, candidates staged once for 4 tiles) when the mesh is sparse enough
-    // for a 32x32 tile's candidates to fit one staging round and the grid still fills the GPU;
-    // dense meshes / small images keep one tile per CTA.
-    const char* force = getenv("DIBR_B200_FWD");   // "old" | "s1" | "s2": A/B switches
+    // dibr_fwd2_kernel (32x32 px per CTA, candidates staged once for 4 tiles) when the mesh is
+    // sparse enough for a 32x32 tile's candidates to fit one staging round and the grid still
+    // fills the GPU; dense meshes / small images keep one tile per CTA.
     const int64_t tiles32 = (int64_t)((a.s.W + 31) / 32) * ((a.s.H + 31) / 32);
     const int64_t faces_per_view = a.s.NF / (a.s.B > 0 ? a.s.B : 1);
     // ~ faces per 32x32 tile <= 40: c4 (20 k faces at 1024^2) has 20, c3 (512^2) 80, c2 80, c5 320
-    bool two = R && faces_per_view <= 40 * tiles32 && tiles32 * a.s.B >= 2048;
-    if (force && force[0] == 's') two = force[1] == '2';
-    const bool v2_single = force && force[0] == 's' && force[1] == '1';
-    if ((force && force[0] == 'o') || (!two && !v2_single)) {
-      // one 16x16 tile per CTA: dense meshes (hundreds of candidates per tile) and small images;
-      Span sp("dibr_tile_fwd_kernel", st);
-      dibr_tile_fwd_kernel<R, S, K, FT><<<tile_grid(a.s), kThreads, 0, st>>>(a);
-    } else if (two) {
+    const bool two = R && faces_per_view <= 40 * tiles32 && tiles32 * a.s.B >= 2048;
+    if (two) {
       Span sp("dibr_fwd2_kernel<S=2>", st);
       const dim3 grid((unsigned)((a.s.ntx[0] + 1) / 2), (unsigned)((a.s.nty[0] + 1) / 2), (unsigned)a.s.B);
-      dibr_fwd2_kernel<R, S, K, FT, 2><<<grid, kThreads, 0, st>>>(a);
+      dibr_fwd2_kernel<R, S, K, FT><<<grid, kThreads, 0, st>>>(a);
     } else {
-      Span sp("dibr_fwd2_kernel<S=1>", st);
-      dibr_fwd2_kernel<R, S, K, FT, 1><<<tile_grid(a.s), kThreads, 0, st>>>(a);
+      // one 16x16 tile per CTA: dense meshes (hundreds of candidates per tile) and small images
+      Span sp("dibr_tile_fwd_kernel", st);
+      dibr_tile_fwd_kernel<R, S, K, FT><<<tile_grid(a.s), kThreads, 0, st>>>(a);
     }
   }
   if (S) {
@@ -2752,7 +2659,6 @@ int launch_raster_bwd_rows(const RasterBwdArgs& r, float* acc, int accumulate_xy
   a.feat = r.feat; a.grid = r.grid; a.rc = r.rc; a.multiplier = r.multiplier; a.acc = acc;
   a.jobs_y = (r.H + 31) / 32;
   int strip = 32;   // H100, c4_shard: strips of 16 / 64 columns 1 % faster / 8 % slower
-  if (const char* fs = getenv("DIBR_B200_ROWS_STRIP")) { const int v = atoi(fs); if (v >= kRwSlab && v % kRwSlab == 0) strip = v; }
   while (strip > kRwSlab && (int64_t)r.B * a.jobs_y * ((r.W + strip - 1) / strip) < 8192) strip >>= 1;
   a.strip = strip;
   a.jobs_x = (r.W + strip - 1) / strip;
@@ -2982,10 +2888,8 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
   float* const g_ff_v = grad_face_features ? grad_face_features + (size_t)view_begin * num_faces * 3 * feat_dim : nullptr;
   // row-walk kernel: fp32 or bf16 features, D <= 4, rows a multiple of 4 px, a workspace with the face records
   float* acc = nullptr;
-  if (run_raster && feat_dim <= 4 && (width % kRwSlab) == 0 && NF > 0) {
-    const char* force = getenv("DIBR_B200_RASTER_BWD");   // "warp": A/B against the warp-reduction kernel
-    if (!(force && force[0] == 'w')) acc = acc_region(workspace, workspace_bytes_, batch, NF, height, width);
-  }
+  if (run_raster && feat_dim <= 4 && (width % kRwSlab) == 0 && NF > 0)
+    acc = acc_region(workspace, workspace_bytes_, batch, NF, height, width);
   if (!(flags & DIBR_B200_ACCUMULATE) && !acc) {
     e = cudaMemsetAsync(g_xy_v, 0, (size_t)NFv * 6 * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
@@ -3038,14 +2942,8 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
       // forward left the bins, the hit cache and the list of tiles it could not cache
       a.from_list = 1;
       if (s.pool_tiles > 0) {
-        const char* force = getenv("DIBR_B200_SOFT_BWD");   // "dense": A/B against the shuffle-reduction kernel
-        if (force && force[0] == 'd') {
-          Span sp("soft_bwd_dense_kernel", st);
-          soft_bwd_dense_kernel<<<(unsigned)s.pool_tiles, kThreads, 0, st>>>(a);
-        } else {
-          Span sp("soft_bwd_runs_kernel", st);
-          soft_bwd_runs_kernel<<<(unsigned)s.pool_tiles, kThreads, 0, st>>>(a);
-        }
+        Span sp("soft_bwd_runs_kernel", st);
+        soft_bwd_runs_kernel<<<(unsigned)s.pool_tiles, kThreads, 0, st>>>(a);
       }
       Span sp("dibr_tile_soft_bwd_kernel<leftovers>", st);
       dibr_tile_soft_bwd_kernel<<<persistent, kThreads, 0, st>>>(a);

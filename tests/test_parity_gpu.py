@@ -705,15 +705,15 @@ def test_graphed_fast_path_equals_eager():
 
 
 @pytest.mark.parametrize("variant", ["rows", "warp", "bf16"])
-def test_view_chunked_backward_equals_full_backward(variant, monkeypatch):
+def test_view_chunked_backward_equals_full_backward(variant):
     """dibr_b200_backward_views: the backward of views [0,2), [2,5) written into shared full-batch buffers
-    (with the feature-gradient hook between the branches) equals one full backward."""
+    (with the feature-gradient hook between the branches) equals one full backward.  The "warp" variant
+    reaches the warp-reduction rasterize backward through a width that is not a multiple of 4."""
+    from kaolin_b200 import _lib
     from kaolin_b200.render.mesh import _host
-    if variant == "warp":
-        monkeypatch.setenv("DIBR_B200_RASTER_BWD", "warp")
     fvz, fvi, fnz = synthetic.icosphere_views(5, 4, seed=71)
     B, F = fvz.shape[:2]
-    H, W = 144, 160
+    H, W = 144, (150 if variant == "warp" else 160)
     dt = torch.bfloat16 if variant == "bf16" else torch.float32
     ff = T(synthetic.random_features(B, F, 3, seed=72)).to(dt)
     gen = torch.Generator(device=DEV); gen.manual_seed(73)
@@ -721,7 +721,10 @@ def test_view_chunked_backward_equals_full_backward(variant, monkeypatch):
     g_soft = torch.rand((B, H, W), device=DEV, generator=gen)
     t_fvz, t_fvi, t_fnz = T(fvz), T(fvi), T(fnz)
     feat, idx, wts, soft, ws = _host.forward(3, H, W, t_fvz, t_fvi, ff, t_fnz, None, 1000., 1e-8, 7000., 20., 30)
+    _lib.trace_begin()
     ref_fvi, ref_ff = _host.backward(H, W, g_feat, g_soft, idx, wts, soft, t_fvi, ff, 1000., 1e-8, 7000., 20., 30, ws, True)
+    ran = [name for name, _ in _lib.trace_end()]
+    assert ("raster_bwd_kernel" if variant == "warp" else "raster_bwd_rows_kernel") in ran, ran
     g_fvi = torch.full_like(t_fvi, float("nan"))
     g_ff = torch.full(ff.shape, float("nan"), dtype=torch.float32, device=DEV)
     hooks = []

@@ -43,25 +43,23 @@ def rel(a, b):
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
-CASES = [  # (id, D, dtype, W, multiplier, raster backward kernel forced to the warp reduction)
-    ("rows_D1", 1, torch.float32, 160, 1000., False),
-    ("rows_D2", 2, torch.float32, 160, 1000., False),
-    ("rows_D3", 3, torch.float32, 160, 1000., False),
-    ("rows_D4", 4, torch.float32, 160, 1000., False),
-    ("rows_D3_mult100", 3, torch.float32, 160, 100., False),
-    ("rows_bf16_D3", 3, torch.bfloat16, 160, 1000., False),
-    ("warp_D5", 5, torch.float32, 160, 1000., False),
-    ("warp_odd_width", 3, torch.float32, 151, 1000., False),
-    ("warp_forced", 3, torch.float32, 160, 1000., True),
-    ("warp_forced_bf16", 2, torch.bfloat16, 160, 1000., True),
+CASES = [  # (id, D, dtype, W, multiplier); D > 4 or a width that is not a multiple of 4 selects the warp reduction
+    ("rows_D1", 1, torch.float32, 160, 1000.),
+    ("rows_D2", 2, torch.float32, 160, 1000.),
+    ("rows_D3", 3, torch.float32, 160, 1000.),
+    ("rows_D4", 4, torch.float32, 160, 1000.),
+    ("rows_D3_mult100", 3, torch.float32, 160, 100.),
+    ("rows_bf16_D3", 3, torch.bfloat16, 160, 1000.),
+    ("warp_D5", 5, torch.float32, 160, 1000.),
+    ("warp_odd_width", 3, torch.float32, 151, 1000.),
+    ("warp_odd_width_D1", 1, torch.float32, 151, 1000.),
+    ("warp_odd_width_bf16", 2, torch.bfloat16, 151, 1000.),
 ]
 
 
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
-def test_backward_without_weights_equals_backward_with_weights(case, monkeypatch):
-    _, D, dt, W, mult, warp = case
-    if warp:
-        monkeypatch.setenv("DIBR_B200_RASTER_BWD", "warp")
+def test_backward_without_weights_equals_backward_with_weights(case):
+    name, D, dt, W, mult = case
     fvz, fvi, fnz = synthetic.icosphere_views(5, 4, seed=81)
     B, F = fvz.shape[:2]
     H = 144
@@ -87,8 +85,11 @@ def test_backward_without_weights_equals_backward_with_weights(case, monkeypatch
     a_fvi, a_ff = bwd(wts)
     b_fvi, b_ff = bwd(wts)
     spread = max(rel(a_fvi, b_fvi), rel(a_ff, b_ff))
+    _lib.trace_begin()
     r_fvi, r_ff = bwd(None)
-    print(f"[{case[0]}] same backward twice: {spread:.2e}; recomputed vs given: "
+    ran = [k for k, _ in _lib.trace_end()]
+    assert ("raster_bwd_rows_kernel" if name.startswith("rows") else "raster_bwd_kernel") in ran, ran
+    print(f"[{name}] same backward twice: {spread:.2e}; recomputed vs given: "
           f"fvi {rel(r_fvi, a_fvi):.2e} ff {rel(r_ff, a_ff):.2e}")
     assert rel(r_fvi, a_fvi) <= 1e-6 and rel(r_ff, a_ff) <= 1e-6
 
