@@ -413,6 +413,40 @@ int dibr_b200_diffuse_backward(
     float* grad_light_sharpness, void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
 
 /*
+ * Specular lighting (kaolin/render/lighting/sg.py sg_warp_specular_term; kaolin_b200/csrc/lighting.cu):
+ * the Cook-Torrance SG specular term of DIB-R++ for N points lit by L spherical-Gaussian lights
+ * light_amplitude (L,3), light_direction (L,3), light_sharpness (L).  Per point: normal n (N,3), not
+ * normalised; roughness r (N); view v (N,3), the direction towards the camera; spec_albedo s (N,3).
+ *   m2 = r^2; lobe amplitude a = 1 / (pi m2) in all three channels;
+ *   w  = -v - 2 ((-v).n) n;  ws = (2 / m2) / (4 max(n.v, 1e-4))
+ *   acc = sum_l <(a, w, ws), light_l>   (the SG inner product of the general operator above)
+ *   ndl = clamp(n.w, 0, 1), ndv = clamp(n.v, 0, 1), h = (w + v) / sqrt((w + v).(w + v)),
+ *   ldh = clamp(w.h, 0, 1), V(x) = 1 / (x + sqrt(m2 + (1 - m2) x^2))
+ *   out (N,3) = clamp(acc V(ndl) V(ndv) (s + (1 - s) (1 - ldh)^5) ndl, min=0)
+ * in fp32, with the reference's formulas and nothing normalised that the reference does not
+ * normalise.  The backward writes any subset of grad_normal (N,3), grad_roughness (N), grad_view
+ * (N,3), grad_spec_albedo (N,3) and the light gradients; a NULL gradient is not computed, and with
+ * only light gradients requested nothing is written per point.  Clamp gradients pass where
+ * min <= x <= max, as torch.clamp's do.  Light gradients need workspace >=
+ * dibr_b200_specular_workspace_bytes(L) = 264 CTA slots x 7 floats = 7.4 KB per light, independent
+ * of N; they are bit-reproducible, as the diffuse models' are.  L = 0 gives zero output and zero
+ * per-point gradients (the reference's empty sum); N = 0 does nothing per point.
+ * Unspecified, as the reference itself gives inf or NaN there: roughness 0, and w + v = 0 (a unit
+ * normal exactly perpendicular to the view).
+ */
+size_t dibr_b200_specular_workspace_bytes(int num_lights);
+int dibr_b200_specular_forward(
+    int64_t num_points, int num_lights, const float* light_amplitude, const float* light_direction,
+    const float* light_sharpness, const float* normal, const float* roughness, const float* view,
+    const float* spec_albedo, float* out, dibr_b200_stream_t stream);
+int dibr_b200_specular_backward(
+    int64_t num_points, int num_lights, const float* light_amplitude, const float* light_direction,
+    const float* light_sharpness, const float* normal, const float* roughness, const float* view,
+    const float* spec_albedo, const float* grad_out, float* grad_normal, float* grad_roughness,
+    float* grad_view, float* grad_spec_albedo, float* grad_light_amplitude, float* grad_light_direction,
+    float* grad_light_sharpness, void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
  * Exchange step of the view-sharded path (SURVEY.md 8e; kaolin_b200/csrc/peer_push.cu): the
  * reference has no multi-GPU code - its callers all-gather the per-view gradients with
  * torch.distributed.  All-gather by STORES over NVLink: copies `bytes` (multiple of 16) from the

@@ -91,6 +91,10 @@ SIGNATURES = {
     "dibr_b200_diffuse_forward": (_i, [_i, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dibr_b200_diffuse_backward": (_i, [_i, _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dibr_b200_specular_workspace_bytes": (_sz, [_i]),
+    "dibr_b200_specular_forward": (_i, [_i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dibr_b200_specular_backward": (_i, [_i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                         _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

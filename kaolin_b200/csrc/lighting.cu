@@ -5,10 +5,12 @@
 //   SG_INNER_PRODUCT                    per-point cosine lobe (1.17, normal, 2.133) . lights, clamp, albedo/pi
 //   SG_FITTED                           Stephen Hill's fitted irradiance, mean over lights, clamp, albedo/pi
 //   SH9                                 sum_k band_k(normal) c_k lights_k, x albedo
+//   SPECULAR                            sg_warp_specular_term: the GGX lobe of (normal, roughness) warped
+//                                       by the view . lights, times Smith visibility, Fresnel and n.l
 //
-// One kernel template per direction, instantiated per Kind; the general op and SG_INNER_PRODUCT
-// differ only in where the sg side comes from (per-point arrays or the cosine lobe of the normal)
-// and in the epilogue (none, or clamp + albedo/pi).
+// One kernel template per direction, instantiated per Kind; the general op, SG_INNER_PRODUCT and
+// SPECULAR differ only in where the sg side comes from (per-point arrays, the cosine lobe of the
+// normal, or the warped distribution lobe) and in the epilogue.
 //
 // Layout of the work: a CTA of 256 threads takes tiles of 1024 points, four consecutive points per
 // thread, so that the 12-byte rows of a thread's points are three 16-byte loads (scalar loads when
@@ -33,33 +35,42 @@ constexpr int kWarps = kThreads / 32;
 constexpr int kPts = 4;                     // points per thread per tile
 constexpr int kTile = kThreads * kPts;
 constexpr int kChunk = 64;                  // lights staged in shared memory at a time
-constexpr int kFwdCtas = 132 * 4;           // persistent grids: 4 CTAs on each of H100's 132 SMs
-constexpr int kBwdCtas = 132 * 2;           // 2 resident CTAs per SM (__launch_bounds__ below); also the
+constexpr int kSms = 132;                   // persistent grids: Cfg::kFwdBlocks CTAs on each of H100's 132 SMs
+constexpr int kBwdCtas = kSms * 2;          // 2 resident CTAs per SM (__launch_bounds__ below); also the
                                             // number of per-CTA partial slots in the workspace
 constexpr float kPi = 3.14159265358979323846f;
 constexpr float kTwoPi = 6.28318530717958647692f;
 
-enum Kind { GENERAL = 0, LOBE = 1, FITTED = 2, SH9 = 3 };
+enum Kind { GENERAL = 0, LOBE = 1, FITTED = 2, SH9 = 3, SPECULAR = 4 };
 
 template <int K> struct Cfg {
-  static constexpr int kIn = K == GENERAL ? 7 : 3;                   // per-point floats in registers
-  static constexpr int kRec = (K == GENERAL || K == LOBE) ? 8 : 16;  // floats per staged light
+  // per-point floats in registers (SPECULAR: the warped lobe a, w, ws, then V(ndl) V(ndv), (1-ldh)^5, ndl)
+  static constexpr int kIn = K == GENERAL ? 7 : K == SPECULAR ? 8 : 3;
+  static constexpr int kRec = (K == GENERAL || K == LOBE || K == SPECULAR) ? 8 : 16;  // floats per staged light
   static constexpr int kAcc = K == SH9 ? 9 : 7;                      // per-light gradient partials
+  // resident forward CTAs per SM: the SPECULAR prologue needs more than 64 registers
+  static constexpr int kFwdBlocks = K == SPECULAR ? 3 : 4;
 };
 
 struct Args {
   int64_t n;
   int L;
-  const float* p_amp; const float* p_dir; const float* p_sharp;   // GENERAL: the sg side
+  // GENERAL: the sg side; SPECULAR: view and roughness in the slots GENERAL's direction and sharpness
+  // use (the layout, and with it every kernel's parameter offsets, is the same for all kinds)
+  const float* p_amp;
+  union { const float* p_dir; const float* view; };
+  union { const float* p_sharp; const float* rough; };
   const float* normal; const float* albedo;                         // shading models
   const float* l_amp; const float* l_dir; const float* l_sharp;   // lights / "other" (SH9: l_amp = 9 coefficients)
   float* out;
   const float* grad_out;
-  float* g_amp; float* g_dir; float* g_sharp;                       // GENERAL: sg-side gradients
+  float* g_amp;                                                     // GENERAL: sg-side gradients
+  union { float* g_dir; float* g_view; };
+  union { float* g_sharp; float* g_rough; };
   float* g_normal; float* g_albedo;
   float* gl_amp; float* gl_dir; float* gl_sharp;                    // light gradients
   float* partial;                                                   // [grid][L][kAcc]
-};
+};                                  // SPECULAR: albedo = spec_albedo, g_albedo = grad_spec_albedo
 
 // ---------------------------------------------------------------------------------------------
 // 4-point row loads / stores: three (C = 3) or one (C = 1) 16-byte accesses when aligned.
@@ -160,6 +171,10 @@ __device__ __forceinline__ void sg_side(const float* in, float* amp, float* dir,
     amp[0] = in[0]; amp[1] = in[1]; amp[2] = in[2];
     dir[0] = in[3]; dir[1] = in[4]; dir[2] = in[5];
     sharp = in[6];
+  } else if constexpr (K == SPECULAR) {
+    amp[0] = amp[1] = amp[2] = in[0];
+    dir[0] = in[1]; dir[1] = in[2]; dir[2] = in[3];
+    sharp = in[4];
   } else {
     amp[0] = amp[1] = amp[2] = 1.17f;
     dir[0] = in[0]; dir[1] = in[1]; dir[2] = in[2];
@@ -264,9 +279,131 @@ __device__ __forceinline__ void pair_bwd(const float* in, const float* gpre, con
       if constexpr (K == GENERAL) {
         pg[3] += gpre[0] * r[0] * t.c; pg[4] += gpre[1] * r[1] * t.c; pg[5] += gpre[2] * r[2] * t.c;
         pg[6] += dir[0] * gx + dir[1] * gy + dir[2] * gz - Gc * t.c;
+      } else if constexpr (K == SPECULAR) {     // one amplitude for the three channels
+        pg[3] += (gpre[0] * r[0] + gpre[1] * r[1] + gpre[2] * r[2]) * t.c;
+        pg[4] += dir[0] * gx + dir[1] * gy + dir[2] * gz - Gc * t.c;
       }
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// SPECULAR (sg_warp_specular_term), the reference's arithmetic in fp32.  x = normal n, roughness,
+// view v of one point.  The lobe of sg_distribution_term is (1 / (pi m2), n, 2 / m2) with m2 =
+// roughness^2; sg_warp_distribution turns it into (a, w, ws) with w = -v - 2 ((-v).n) n and
+// ws = (2 / m2) / (4 max(n.v, 1e-4)).  The epilogue multiplies the lights' sum by the Smith terms
+// V(ndl) V(ndv), Fresnel s + (1 - s) (1 - ldh)^5 and ndl.
+__device__ __forceinline__ float clamp01(float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); }   // NaN stays NaN
+__device__ __forceinline__ bool in01(float v) { return v >= 0.f && v <= 1.f; }   // where torch.clamp(v, 0, 1) passes a gradient
+
+struct Spec {
+  float m2, a, sh0, nv, cnv, ws, w[3];                                      // the warped lobe
+  float ndl_raw, ndl, ndv, q1, q2, V1, V2, hat[3], hn, ldh_raw, om, p5;    // the epilogue's factors
+};
+
+__device__ __forceinline__ Spec spec_geom(const float* x) {
+  Spec s;
+  const float* n = x;
+  const float* v = x + 4;
+  s.m2 = x[3] * x[3];
+  s.sh0 = 2.f / s.m2;
+  s.a = 1.f / (kPi * s.m2);
+  s.nv = n[0] * v[0] + n[1] * v[1] + n[2] * v[2];
+  s.cnv = s.nv < 1e-4f ? 1e-4f : s.nv;
+  s.ws = s.sh0 / (4.f * s.cnv);
+  const float t = 2.f * -s.nv;                       // 2 ((-v).n)
+#pragma unroll
+  for (int k = 0; k < 3; ++k) s.w[k] = -v[k] - t * n[k];
+  s.ndl_raw = n[0] * s.w[0] + n[1] * s.w[1] + n[2] * s.w[2];
+  s.ndl = clamp01(s.ndl_raw);
+  s.ndv = clamp01(s.nv);
+  const float h0 = s.w[0] + v[0], h1 = s.w[1] + v[1], h2 = s.w[2] + v[2];
+  s.hn = sqrtf(h0 * h0 + h1 * h1 + h2 * h2);
+  s.hat[0] = h0 / s.hn; s.hat[1] = h1 / s.hn; s.hat[2] = h2 / s.hn;
+  s.ldh_raw = s.w[0] * s.hat[0] + s.w[1] * s.hat[1] + s.w[2] * s.hat[2];
+  s.q1 = sqrtf(s.m2 + (1.f - s.m2) * s.ndl * s.ndl);
+  s.q2 = sqrtf(s.m2 + (1.f - s.m2) * s.ndv * s.ndv);
+  s.V1 = 1.f / (s.ndl + s.q1);
+  s.V2 = 1.f / (s.ndv + s.q2);
+  s.om = 1.f - clamp01(s.ldh_raw);
+  const float om2 = s.om * s.om;
+  s.p5 = om2 * om2 * s.om;
+  return s;
+}
+
+__device__ __forceinline__ void load_spec_raw(const Args& a, int64_t p0, float (&x)[kPts][7]) {
+  float n[kPts][3], r[kPts][1], v[kPts][3];
+  load_rows<3>(a.normal, p0, a.n, n);
+  load_rows<1>(a.rough, p0, a.n, r);
+  load_rows<3>(a.view, p0, a.n, v);
+#pragma unroll
+  for (int p = 0; p < kPts; ++p) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { x[p][k] = n[p][k]; x[p][4 + k] = v[p][k]; }
+    x[p][3] = r[p][0];
+  }
+}
+
+// Epilogue backward of one point: from the lights' sums acc, grad_out g and spec albedo sa, the
+// gradient gpre of the sums, grad_spec_albedo gs, and eg = d loss / d (n.w, n.v, ldh) where their
+// clamps pass a gradient, and d loss / d m2 through the Smith terms.
+__device__ __forceinline__ void spec_epilogue_bwd(const Spec& s, const float* acc, const float* g, const float* sa,
+                                                  float* gpre, float* gs, float* eg) {
+  const float G = s.V1 * s.V2;
+  float gG = 0.f, gndl = 0.f, gp5 = 0.f;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float F = sa[k] + (1.f - sa[k]) * s.p5;
+    const float gy = ((acc[k] * G) * F) * s.ndl >= 0.f ? g[k] : 0.f;   // clamp(min=0)
+    gpre[k] = gy * G * F * s.ndl;
+    const float gF = gy * acc[k] * G * s.ndl;
+    gs[k] = gF * (1.f - s.p5);
+    gp5 += gF * (1.f - sa[k]);
+    gG += gy * acc[k] * F * s.ndl;
+    gndl += gy * acc[k] * G * F;
+  }
+  // V(x) = 1 / (x + q), q = sqrt(m2 + (1 - m2) x^2):  dV = -V^2 ((1 + (1 - m2) x / q) dx + (1 - x^2) / (2 q) dm2)
+  const float d1 = -gG * s.V2 * s.V1 * s.V1, d2 = -gG * s.V1 * s.V2 * s.V2;
+  gndl += d1 * (1.f + (1.f - s.m2) * s.ndl / s.q1);
+  const float gndv = d2 * (1.f + (1.f - s.m2) * s.ndv / s.q2);
+  eg[3] = d1 * (1.f - s.ndl * s.ndl) / (2.f * s.q1) + d2 * (1.f - s.ndv * s.ndv) / (2.f * s.q2);
+  const float om2 = s.om * s.om;
+  eg[0] = in01(s.ndl_raw) ? gndl : 0.f;
+  eg[1] = in01(s.nv) ? gndv : 0.f;
+  eg[2] = in01(s.ldh_raw) ? -5.f * (om2 * om2) * gp5 : 0.f;
+}
+
+// Prologue backward of one point: pg holds the light loop's d loss / d (ws w) (3), d / da and d / dws;
+// writes d loss / d normal, roughness, view.
+__device__ __forceinline__ void spec_point_bwd(const float* x, const Spec& s, const float* pg, const float* eg,
+                                               float* gn, float& gr, float* gv) {
+  const float* n = x;
+  const float* v = x + 4;
+  float gw[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) gw[k] = s.ws * pg[k];
+  const float gsh0 = pg[4] / (4.f * s.cnv);
+  const float gm2 = eg[3] - pg[3] * s.a / s.m2 - gsh0 * s.sh0 / s.m2;
+  float gnv = eg[1] + (s.nv >= 1e-4f ? -pg[4] * s.ws / s.cnv : 0.f);
+  // ldh = w . hat, hat = h / |h|, h = w + v
+  const float hg = s.hat[0] * s.w[0] + s.hat[1] * s.w[1] + s.hat[2] * s.w[2];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float gh = eg[2] * (s.w[k] - s.hat[k] * hg) / s.hn;
+    gw[k] += eg[2] * s.hat[k] + gh;
+    gv[k] = gh;
+  }
+  // ndl = n . w
+#pragma unroll
+  for (int k = 0; k < 3; ++k) { gn[k] = eg[0] * s.w[k]; gw[k] += eg[0] * n[k]; }
+  // w = -v + 2 (n.v) n, and every n.v
+  gnv += 2.f * (gw[0] * n[0] + gw[1] * n[1] + gw[2] * n[2]);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    gn[k] += 2.f * s.nv * gw[k] + gnv * v[k];
+    gv[k] += gnv * n[k] - gw[k];
+  }
+  gr = gm2 * 2.f * x[3];
 }
 
 template <int K>
@@ -282,6 +419,15 @@ __device__ __forceinline__ void load_points(const Args& a, int64_t p0, float (&i
       for (int k = 0; k < 3; ++k) { in[p][k] = am[p][k]; in[p][3 + k] = di[p][k]; }
       in[p][6] = sh[p][0];
     }
+  } else if constexpr (K == SPECULAR) {
+    float x[kPts][7];
+    load_spec_raw(a, p0, x);
+#pragma unroll
+    for (int p = 0; p < kPts; ++p) {
+      const Spec s = spec_geom(x[p]);
+      in[p][0] = s.a; in[p][1] = s.w[0]; in[p][2] = s.w[1]; in[p][3] = s.w[2]; in[p][4] = s.ws;
+      in[p][5] = s.V1 * s.V2; in[p][6] = s.p5; in[p][7] = s.ndl;
+    }
   } else {
     load_rows<3>(a.normal, p0, a.n, in);
   }
@@ -291,7 +437,7 @@ __device__ __forceinline__ float clamp0(float v) { return v < 0.f ? 0.f : v; }  
 
 // ---------------------------------------------------------------------------------------------
 template <int K>
-__global__ void __launch_bounds__(kThreads, 4) lighting_fwd_kernel(Args a) {
+__global__ void __launch_bounds__(kThreads, Cfg<K>::kFwdBlocks) lighting_fwd_kernel(Args a) {
   constexpr int R = Cfg<K>::kRec;
   __shared__ __align__(16) float s_light[kChunk * R];
   const int64_t tiles = (a.n + kTile - 1) / kTile;
@@ -313,7 +459,16 @@ __global__ void __launch_bounds__(kThreads, 4) lighting_fwd_kernel(Args a) {
         for (int p = 0; p < kPts; ++p) pair_fwd<K>(in[p], r, acc[p]);
       }
     }
-    if (K == GENERAL) {
+    if constexpr (K == SPECULAR) {
+      float sa[kPts][3], o[kPts][3];
+      load_rows<3>(a.albedo, p0, a.n, sa);
+#pragma unroll
+      for (int p = 0; p < kPts; ++p)
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+          o[p][k] = clamp0(((acc[p][k] * in[p][5]) * (sa[p][k] + (1.f - sa[p][k]) * in[p][6])) * in[p][7]);
+      store_rows<3>(a.out, p0, a.n, o);
+    } else if (K == GENERAL) {
       store_rows<3>(a.out, p0, a.n, acc);
     } else if (K == SH9 && !a.albedo) {
       float o[kPts][1];
@@ -346,10 +501,12 @@ __global__ void __launch_bounds__(kThreads, 2) lighting_bwd_kernel(Args a) {
   const int nchunks = (a.L + kChunk - 1) / kChunk;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool want_light = a.partial != nullptr;
-  const bool want_point = K == GENERAL ? (a.g_amp || a.g_dir || a.g_sharp) : a.g_normal != nullptr;
+  const bool want_point = K == GENERAL    ? (a.g_amp || a.g_dir || a.g_sharp)
+                          : K == SPECULAR ? (a.g_normal || a.g_rough || a.g_view)
+                                          : a.g_normal != nullptr;
   const bool has_albedo = a.albedo != nullptr;
   // forward sums are needed for the clamp mask (SG models) or for grad_albedo (SH9)
-  const bool need_pre = K == LOBE || K == FITTED || (K == SH9 && a.g_albedo);
+  const bool need_pre = K == LOBE || K == FITTED || K == SPECULAR || (K == SH9 && a.g_albedo);
   float* part = want_light ? a.partial + (size_t)blockIdx.x * a.L * A : nullptr;
   if (want_light)
     for (int i = threadIdx.x; i < a.L * A; i += kThreads) part[i] = 0.f;
@@ -387,10 +544,15 @@ __global__ void __launch_bounds__(kThreads, 2) lighting_bwd_kernel(Args a) {
     // epilogue backward: gpre = d loss / d pre, and grad_albedo
     float gpre[kPts][3];
     float ga[kPts][3];
+    float eg[kPts][4];                      // SPECULAR: spec_epilogue_bwd
+    float sx[kPts][7];
+    if constexpr (K == SPECULAR) load_spec_raw(a, p0, sx);
 #pragma unroll
     for (int p = 0; p < kPts; ++p) {
       const bool valid = p0 + p < a.n;
-      if (K == SH9) {
+      if constexpr (K == SPECULAR) {
+        spec_epilogue_bwd(spec_geom(sx[p]), pre[p], g[p], al[p], gpre[p], ga[p], eg[p]);
+      } else if (K == SH9) {
         gpre[p][0] = has_albedo ? g[p][0] * al[p][0] + g[p][1] * al[p][1] + g[p][2] * al[p][2] : g[p][0];
         gpre[p][1] = gpre[p][2] = 0.f;
 #pragma unroll
@@ -464,6 +626,14 @@ __global__ void __launch_bounds__(kThreads, 2) lighting_bwd_kernel(Args a) {
           for (int p = 0; p < kPts; ++p) o1[p][0] = pg[p][6];
           store_rows<1>(a.g_sharp, p0, a.n, o1);
         }
+      } else if constexpr (K == SPECULAR) {
+        load_spec_raw(a, p0, sx);
+        float on[kPts][3], orr[kPts][1], ov[kPts][3];
+#pragma unroll
+        for (int p = 0; p < kPts; ++p) spec_point_bwd(sx[p], spec_geom(sx[p]), pg[p], eg[p], on[p], orr[p][0], ov[p]);
+        if (a.g_normal) store_rows<3>(a.g_normal, p0, a.n, on);
+        if (a.g_rough) store_rows<1>(a.g_rough, p0, a.n, orr);
+        if (a.g_view) store_rows<3>(a.g_view, p0, a.n, ov);
       } else {
         float o[kPts][3];
         const float s = K == LOBE ? 2.133f : 1.f;
@@ -518,7 +688,8 @@ template <int K>
 int launch_fwd(const Args& a, cudaStream_t st) {
   const int64_t tiles = (a.n + kTile - 1) / kTile;
   if (tiles == 0) return 0;
-  lighting_fwd_kernel<K><<<(unsigned)(tiles < kFwdCtas ? tiles : kFwdCtas), kThreads, 0, st>>>(a);
+  const int64_t ctas = (int64_t)kSms * Cfg<K>::kFwdBlocks;
+  lighting_fwd_kernel<K><<<(unsigned)(tiles < ctas ? tiles : ctas), kThreads, 0, st>>>(a);
   return (int)cudaGetLastError();
 }
 
@@ -669,6 +840,68 @@ int dibr_b200_diffuse_backward(int model, int64_t num_points, int num_lights, co
     case DIBR_B200_LIGHT_SG_FITTED: return launch_bwd<FITTED>(a, st);
     default: return launch_bwd<SH9>(a, st);
   }
+}
+
+size_t dibr_b200_specular_workspace_bytes(int num_lights) {
+  return num_lights < 0 ? 0 : partial_bytes(Cfg<SPECULAR>::kAcc, num_lights);
+}
+
+static int specular_args(Args& a, int64_t num_points, int num_lights, const float* light_amplitude,
+                         const float* light_direction, const float* light_sharpness, const float* normal,
+                         const float* roughness, const float* view, const float* spec_albedo) {
+  if (num_points < 0 || num_lights < 0) return DIBR_B200_EINVAL;
+  if (num_lights > 0 && (!light_amplitude || !light_direction || !light_sharpness)) return DIBR_B200_EINVAL;
+  if (num_points > 0 && (!normal || !roughness || !view || !spec_albedo)) return DIBR_B200_EINVAL;
+  a = Args{};
+  a.n = num_points; a.L = num_lights;
+  a.normal = normal; a.rough = roughness; a.view = view; a.albedo = spec_albedo;
+  a.l_amp = light_amplitude; a.l_dir = light_direction; a.l_sharp = light_sharpness;
+  return 0;
+}
+
+int dibr_b200_specular_forward(int64_t num_points, int num_lights, const float* light_amplitude,
+                               const float* light_direction, const float* light_sharpness, const float* normal,
+                               const float* roughness, const float* view, const float* spec_albedo, float* out,
+                               dibr_b200_stream_t stream) {
+  Args a;
+  const int rc = specular_args(a, num_points, num_lights, light_amplitude, light_direction, light_sharpness, normal,
+                               roughness, view, spec_albedo);
+  if (rc) return rc;
+  if (num_points > 0 && !out) return DIBR_B200_EINVAL;
+  a.out = out;
+  return launch_fwd<SPECULAR>(a, (cudaStream_t)stream);
+}
+
+int dibr_b200_specular_backward(int64_t num_points, int num_lights, const float* light_amplitude,
+                                const float* light_direction, const float* light_sharpness, const float* normal,
+                                const float* roughness, const float* view, const float* spec_albedo,
+                                const float* grad_out, float* grad_normal, float* grad_roughness, float* grad_view,
+                                float* grad_spec_albedo, float* grad_light_amplitude, float* grad_light_direction,
+                                float* grad_light_sharpness, void* workspace, size_t workspace_bytes,
+                                dibr_b200_stream_t stream) {
+  Args a;
+  const int rc = specular_args(a, num_points, num_lights, light_amplitude, light_direction, light_sharpness, normal,
+                               roughness, view, spec_albedo);
+  if (rc) return rc;
+  if (num_points > 0 && !grad_out) return DIBR_B200_EINVAL;
+  a.grad_out = grad_out;
+  a.g_normal = grad_normal; a.g_rough = grad_roughness; a.g_view = grad_view; a.g_albedo = grad_spec_albedo;
+  a.gl_amp = grad_light_amplitude; a.gl_dir = grad_light_direction; a.gl_sharp = grad_light_sharpness;
+  if (num_lights > 0 && (a.gl_amp || a.gl_dir || a.gl_sharp)) {
+    if (!workspace) return DIBR_B200_EINVAL;
+    if (workspace_bytes < dibr_b200_specular_workspace_bytes(num_lights)) return DIBR_B200_EWORKSPACE;
+    a.partial = (float*)workspace;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (num_lights == 0) {   // empty sum: zero output, zero per-point gradients
+    const size_t b1 = (size_t)num_points * sizeof(float), b3 = 3 * b1;
+    if (grad_normal && cudaMemsetAsync(grad_normal, 0, b3, st) != cudaSuccess) return (int)cudaGetLastError();
+    if (grad_roughness && cudaMemsetAsync(grad_roughness, 0, b1, st) != cudaSuccess) return (int)cudaGetLastError();
+    if (grad_view && cudaMemsetAsync(grad_view, 0, b3, st) != cudaSuccess) return (int)cudaGetLastError();
+    if (grad_spec_albedo && cudaMemsetAsync(grad_spec_albedo, 0, b3, st) != cudaSuccess) return (int)cudaGetLastError();
+    return 0;
+  }
+  return launch_bwd<SPECULAR>(a, st);
 }
 
 }  // extern "C"

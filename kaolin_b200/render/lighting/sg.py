@@ -1,12 +1,16 @@
-"""Spherical-Gaussian diffuse lighting — drop-ins for kaolin.render.lighting.sg
+"""Spherical-Gaussian lighting — drop-ins for kaolin.render.lighting.sg
 (``unbatched_reduced_sg_inner_product``, ``sg_irradiance_inner_product``,
-``sg_diffuse_inner_product``, ``sg_diffuse_fitted``).  Each is one sm_90a kernel each way
-(kaolin_b200/csrc/lighting.cu) instead of the reference's chains of torch kernels and their
-(N, L, 3) temporaries.  Same signatures, shape assertions and return shapes.
+``sg_diffuse_inner_product``, ``sg_diffuse_fitted``, ``sg_warp_specular_term``).  Each is one sm_90a
+kernel each way (kaolin_b200/csrc/lighting.cu) instead of the reference's chains of torch kernels and
+their (N, L, 3) temporaries.  Same signatures, shape assertions and return shapes.  The building
+blocks of the specular term (``sg_distribution_term``, ``sg_warp_distribution``, ``fresnel``) are
+plain torch and run on any device.
 
 Inputs must be float32 CUDA tensors.  The reference's operator is float-only too, but below 8 lights
 its torch path would also accept float64; here float64 raises RuntimeError.
 """
+import math
+
 import torch
 from torch.autograd import Function
 
@@ -14,7 +18,7 @@ from ... import _lib
 from ..mesh import _host
 
 __all__ = ["unbatched_reduced_sg_inner_product", "sg_irradiance_inner_product", "sg_diffuse_inner_product",
-           "sg_diffuse_fitted"]
+           "sg_diffuse_fitted", "sg_distribution_term", "sg_warp_distribution", "fresnel", "sg_warp_specular_term"]
 
 
 def _c(t):
@@ -156,3 +160,91 @@ def sg_diffuse_fitted(amplitude, direction, sharpness, normal, albedo):
     reference's mean over an empty set is NaN)."""
     _check_lights("sg_diffuse_fitted", amplitude, direction, sharpness, normal, albedo)
     return DiffuseB200.apply(_lib.LIGHT_SG_FITTED, amplitude, direction, sharpness, normal, albedo)
+
+
+class SpecularB200(Function):
+    """sg_warp_specular_term of N points under L lights."""
+
+    @staticmethod
+    def forward(ctx, amplitude, direction, sharpness, normal, roughness, view, spec_albedo):
+        ins = [_c(t) for t in (amplitude, direction, sharpness, normal, roughness, view, spec_albedo)]
+        out = torch.empty_like(ins[3])
+        with torch.cuda.device(out.device):
+            st = _lib.lib().dibr_b200_specular_forward(
+                out.shape[0], ins[0].shape[0], *[_host.ptr(t) for t in ins], _host.ptr(out),
+                _host.stream_ptr(out.device))
+        _lib.check(st, "dibr_b200_specular_forward")
+        ctx.save_for_backward(*ins)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        ins = ctx.saved_tensors
+        wants = ctx.needs_input_grad
+        grads = [torch.empty_like(t) if w else None for t, w in zip(ins, wants)]
+        dev = ins[3].device
+        ws = _workspace(_lib.lib().dibr_b200_specular_workspace_bytes(ins[0].shape[0]) if any(wants[:3]) else 0, dev)
+        g_amp, g_dir, g_sharp, g_n, g_r, g_v, g_s = grads
+        with torch.cuda.device(dev):
+            st = _lib.lib().dibr_b200_specular_backward(
+                ins[3].shape[0], ins[0].shape[0], *[_host.ptr(t) for t in ins], _host.ptr(grad_out.contiguous()),
+                _host.ptr(g_n), _host.ptr(g_r), _host.ptr(g_v), _host.ptr(g_s), _host.ptr(g_amp), _host.ptr(g_dir),
+                _host.ptr(g_sharp), _host.ptr(ws), ws.numel(), _host.stream_ptr(dev))
+        _lib.check(st, "dibr_b200_specular_backward")
+        return tuple(grads)
+
+
+def sg_distribution_term(direction, roughness):
+    r"""One spherical Gaussian approximating the GGX (Trowbridge-Reitz) normal distribution around
+    ``direction`` (num_points, 3) for ``roughness`` (num_points,): with m2 = roughness^2, amplitude
+    1 / (pi m2) in each of the three channels (num_points, 3), the input direction, and sharpness
+    2 / m2 (num_points,)."""
+    assert direction.ndim == 2 and direction.shape[-1]
+    assert roughness.shape == direction.shape[:1]
+    m2 = roughness * roughness
+    amplitude = (1. / (math.pi * m2))[:, None].expand(-1, 3)
+    return amplitude, direction, 2. / m2
+
+
+def _dot(a, b):
+    return (a * b).sum(-1)
+
+
+def sg_warp_distribution(amplitude, direction, sharpness, view):
+    r"""The distribution lobe (amplitude, direction (num_sg, 3), sharpness (num_sg,)) turned towards
+    the slice of the BRDF seen from ``view`` (num_sg, 3) by Wang et al.'s warp: the direction is the
+    reflection of -view about ``direction``, and the sharpness is divided by 4 max(direction . view,
+    1e-4).  The amplitude is returned as it is."""
+    assert amplitude.ndim == 2 and amplitude.shape[-1] == 3
+    assert direction.shape == amplitude.shape
+    assert sharpness.shape == amplitude.shape[:1]
+    assert view.shape == amplitude.shape
+    incoming = -view
+    warped = incoming - (2 * _dot(incoming, direction))[:, None] * direction
+    return amplitude, warped, sharpness / (4. * torch.clamp(_dot(direction, view), min=1e-4))
+
+
+def fresnel(ldh, spec_albedo):
+    r"""Schlick's Fresnel term: spec_albedo + (1 - spec_albedo) (1 - ldh)^5."""
+    return spec_albedo + (1. - spec_albedo) * torch.pow(1. - ldh, 5)
+
+
+def sg_warp_specular_term(amplitude, direction, sharpness, normal, roughness, view, spec_albedo):
+    r"""Cook-Torrance specular reflectance (num_points, 3) of surface points lit by spherical-Gaussian
+    lights (amplitude, direction (num_sg, 3), sharpness (num_sg,)): the GGX distribution of
+    ``normal`` (num_points, 3) and ``roughness`` (num_points,) as one spherical Gaussian, warped by
+    ``view`` (num_points, 3, towards the camera), its inner product with every light summed, times
+    the Smith visibility of the light and view directions, Fresnel with ``spec_albedo``
+    (num_points, 3) and n . l, clamped at 0 (the specular term of DIB-R++).  One kernel each way;
+    the light gradients are bit-reproducible."""
+    assert amplitude.ndim == 2 and amplitude.shape[-1] == 3
+    assert direction.shape == amplitude.shape
+    assert sharpness.shape == amplitude.shape[:1]
+    assert normal.ndim == 2 and normal.shape[-1] == 3
+    assert roughness.shape == normal.shape[:1]
+    assert view.shape == normal.shape
+    assert spec_albedo.shape == normal.shape
+    _host.check_tensors("sg_warp_specular_term", [
+        ("amplitude", amplitude), ("direction", direction), ("sharpness", sharpness), ("normal", normal),
+        ("roughness", roughness), ("view", view), ("spec_albedo", spec_albedo)])
+    return SpecularB200.apply(amplitude, direction, sharpness, normal, roughness, view, spec_albedo)
