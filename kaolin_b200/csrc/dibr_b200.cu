@@ -6,25 +6,30 @@
 //   kaolin/render/mesh/rasterization.py:273-371, kaolin/render/mesh/dibr.py:29-73
 //
 // Pipeline (forward):
-//   bin_faces<count> -> scan_bins -> bin_faces<fill> -> dibr_tile_fwd_kernel
+//   bin_faces<count> -> scan_bins -> bin_faces<fill>
+//   -> dibr_fwd2_kernel (sparse meshes on large images) | dibr_tile_fwd_kernel
 //   -> soft_fwd_kernel (-> soft_tiles_fwd_kernel for leftovers)
 //   * every face is turned into the exact integer pixel rectangle of the
 //     reference's float bbox test and inserted (<= 4 entries) into the finest
 //     level of a 16/64/256/... px bin pyramid where it spans <= 2x2 bins;
-//   * one CTA per 16x16 screen tile streams the (<= 6) bins above it into
-//     shared memory with TMA bulk copies (cp.async.bulk + mbarrier, double
-//     buffered), culls them against the tile, stages the surviving face records,
-//     transposes their rectangle masks into per-column/row candidate bit words and
-//     lets each thread (one pixel) walk exactly its own rectangle hits;
+//   * one CTA per 16x16 screen tile (dibr_tile_fwd_kernel) or per 32x32 block of four
+//     such tiles (dibr_fwd2_kernel) streams the bins above it into shared memory with
+//     TMA bulk copies (cp.async.bulk + mbarrier, double buffered), culls them against
+//     the tile, stages the surviving face records and transposes their rectangle masks
+//     into per-column/row candidate bit words; each thread (one pixel) then visits
+//     exactly its own rectangle hits;
 //   * tiles with uncovered pixels under an enlarged (boxlen) rectangle are filed in
 //     a work list; one CTA per such tile enumerates the first knum faces by index of
 //     every uncovered pixel, stages each candidate face's per-face terms in shared
 //     memory once, evaluates the pairs densely — one thread per (pixel, face) pair —
 //     and folds them per pixel in face order.  The pairs stay in a per-tile cache
 //     block for the backward pass.
-// Backward: a pixel-parallel scatter with warp-level segmented reduction keyed
-// on the face id (rasterize branch) and a dense stream over the cached pairs
-// (soft-mask branch; tiles outside the cache are recomputed).
+// Backward: the rasterize branch walks image rows (raster_bwd_rows_kernel: one warp per
+// 32 rows, per-face sums in registers flushed with vector reductions into per-face records;
+// raster_bwd_kernel, a pixel-parallel scatter with a warp-level segmented reduction, when
+// the shape or the workspace rules the row walk out).  The soft-mask branch is a dense
+// stream over the cached pairs (soft_bwd_runs_kernel); tiles outside the cache are
+// recomputed (dibr_tile_soft_bwd_kernel).
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <type_traits>
@@ -439,9 +444,9 @@ struct TileCtx {
   int64_t fbase, pix;
 };
 
-__device__ __forceinline__ TileCtx make_tile_ctx(const Scene& s) {
+__device__ __forceinline__ TileCtx make_tile_ctx(const Scene& s, int b, int tx, int ty) {
   TileCtx c;
-  c.tx = blockIdx.x; c.ty = blockIdx.y; c.b = blockIdx.z;   // grid = (tiles_x, tiles_y, views)
+  c.tx = tx; c.ty = ty; c.b = b;
   c.tile_x0 = c.tx * kTile;
   c.tile_y0 = c.ty * kTile;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -471,26 +476,19 @@ __device__ __forceinline__ BinRef tile_bin(const Scene& s, int b, int tx, int ty
   return r;
 }
 
-// Shared memory of the tile kernels.
+// Shared memory of the soft-mask backward tile kernel and of the float64 kernel.
 struct TileSmem {
-  int4 stage[2][kChunk];                 // TMA landing buffers (bin entries)
   float4 cxy0[kChunk];                   // ax ay bx by
-  float4 cz[kChunk];                     // az bz cz (pad)
   float2 cxy1[kChunk];                   // cx cy
   uint32_t cmask[kChunk];                // col mask | row mask << 16 (tile local)
   int cface[kChunk];
   unsigned long long list[kSoftCap];     // (face << 32) | mask, unsorted
   unsigned long long sorted[kSoftCap];
   float acc[kChunk][6];                  // soft-mask backward per-candidate sums
-  unsigned long long bar[2];
   BinRef bin[2][kMaxLevels];             // the tile's bins (set, level): filled once by warp 0
   uint8_t apix[kThreads];                // compacted uncovered pixels of the tile: lx | ly << 4
   int wcount[kThreads / 32];
-  int ncand;
   int nsoft;
-  int nent;                              // hits appended to the cache block
-  int pool_slot;                         // cache block of this tile (-1: none)
-  int npairs;                            // (pixel, face) pairs of the current round
 };
 
 // Shared memory of the rasterizing tile kernel (a subset: 4-5 CTAs more per SM).
@@ -720,33 +718,38 @@ __device__ __forceinline__ int tile_linear(const Scene& s, const TileCtx& c) {
   return (c.b * s.nty[0] + c.ty) * s.ntx[0] + c.tx;
 }
 
-struct SoftIO {
-  float* out_soft;                                   // forward
-  SoftFwdOut kl;                                     // forward, operator contract (nullable)
-  const float* grad_soft; const float* soft;         // backward
-  float* grad_xy;                                    // backward
+// Arguments of the forward tile kernels.
+struct FwdArgs {
+  Scene s;
+  RasterConst rc;
+  int D;
+  const void* feat;         // (NF,3,D) FT
+  float sigmainv; int K;
+  int cache;                // fill the soft-mask hit cache
+  int from_fb;              // soft_tiles_fwd_kernel: walk fb_list instead of band_list
+  void* out_feat;           // (B,H,W,D) FT
+  int64_t* idx; float* out_w; float* out_soft;  // idx: output if RASTER else input
+  SoftFwdOut kl;
 };
 
-// Soft mask of one tile.  `uncovered` is the calling thread's own pixel; the
-// uncovered pixels of the tile are first compacted so that the expensive
-// per-(pixel, face) distance work runs on densely packed warps (thread t owns the
-// t-th uncovered pixel).  Covered pixels (soft = 1) are written by their own thread.
-// CACHE (forward only): every hit (pixel, face, prob, dist_type) is appended to the
-// tile's block of the hit cache so that the backward pass is a dense stream over
-// hits instead of a second walk (the reference stores 13*knum bytes per pixel).
-template <bool BWD, bool KLISTS>
-__device__ __forceinline__ void soft_tile(const Scene& s, const TileCtx& c, TileSmem& sm, bool uncovered,
-                                          float sigmainv, int K, bool cache, const SoftIO& io) {
+// Arguments of the soft-mask backward: (1) dense kernel over the hit cache; (2) the recompute
+// tile kernel for the tiles the cache could not hold (fb_list) or, with no forward state, for
+// every tile.  Persistent CTAs walk the work list.
+struct SoftBwdArgs {
+  Scene s;
+  float sigmainv; int K;
+  int from_list;             // 1: tiles of fb_list only; 0: every tile
+  int view_begin, view_end;  // only tiles / cache blocks of these views (dibr_b200_backward_views)
+  const float* grad_soft; const float* soft; const int64_t* idx;
+  float* grad_xy;
+};
+
+// Compacts the uncovered pixels of the tile (`uncovered`: the calling thread's own pixel) into
+// sm.apix, lx | ly << 4 in thread order, and returns their number (uniform).  The caller orders
+// the apix writes with a barrier of its own.
+template <typename SM>
+__device__ __forceinline__ int compact_uncovered(const TileCtx& c, SM& sm, bool uncovered) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (!BWD && c.in_img && !uncovered) {
-    io.out_soft[c.pix] = 1.0f;
-    if (KLISTS) {  // padding the reference gets from at::zeros / at::full(-1)
-      for (int k = 0; k < K; ++k) {
-        const int64_t o = c.pix * K + k;
-        io.kl.prob[o] = 0.f; io.kl.idx[o] = -1; io.kl.type[o] = 0;
-      }
-    }
-  }
   const unsigned av = __ballot_sync(kFull, uncovered);
   if (lane == 0) sm.wcount[warp] = __popc(av);
   __syncthreads();
@@ -757,11 +760,48 @@ __device__ __forceinline__ void soft_tile(const Scene& s, const TileCtx& c, Tile
     if (w < warp) before += cw;
     na += cw;
   }
-  if (na == 0) return;  // uniform
   if (uncovered) sm.apix[before + __popc(av & ((1u << lane) - 1u))] = (uint8_t)(c.lx | (c.ly << 4));
-  if (BWD) {
-    for (int i = tid; i < kChunk * 6; i += kThreads) (&sm.acc[0][0])[i] = 0.f;
+  return na;
+}
+
+// The tile's block of the soft-mask hit cache (called by one thread): a slot from pool_ctr, or
+// -1 when the cache is full, with the tile filed in fb_list to be recomputed in backward.
+__device__ __forceinline__ int claim_cache_block(const Scene& s, const TileCtx& c) {
+  int slot = atomicAdd(s.pool_ctr, 1);
+  if (slot >= s.pool_tiles) {
+    slot = -1;
+    s.fb_list[atomicAdd(s.fb_ctr, 1)] = tile_linear(s, c);
   }
+  return slot;
+}
+
+// Face-major pair offsets (warp 0): exclusive scan of the claims per candidate cnt_c[0..cn) into
+// off_c, their total into npairs.
+template <typename SM>
+__device__ __forceinline__ void pair_offsets(SM& sm, int cn) {
+  const int lane = threadIdx.x & 31;
+  int v[8], sum = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { const int j = lane * 8 + i; v[i] = j < cn ? sm.cnt_c[j] : 0; sum += v[i]; }
+  int x = sum;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(kFull, x, d); if (lane >= d) x += y; }
+  int run = x - sum;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { const int j = lane * 8 + i; if (j < cn) sm.off_c[j] = run; run += v[i]; }
+  if (lane == 31) sm.npairs = x;
+}
+
+// Soft-mask gradient of one tile, recomputed from the large bins.  `uncovered` is the calling
+// thread's own pixel; the uncovered pixels of the tile are first compacted so that the expensive
+// per-(pixel, face) distance work runs on densely packed warps (thread t owns the t-th uncovered
+// pixel).
+__device__ __forceinline__ void soft_tile_bwd(const SoftBwdArgs& a, const TileCtx& c, TileSmem& sm, bool uncovered) {
+  const Scene& s = a.s;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int na = compact_uncovered(c, sm, uncovered);
+  if (na == 0) return;  // uniform
+  for (int i = tid; i < kChunk * 6; i += kThreads) (&sm.acc[0][0])[i] = 0.f;
   __syncthreads();
   // thread t now owns the t-th uncovered pixel
   const bool active = tid < na;
@@ -772,35 +812,14 @@ __device__ __forceinline__ void soft_tile(const Scene& s, const TileCtx& c, Tile
   const uint32_t sel = (1u << lx) | (1u << (16 + ly));
   const int64_t pix = ((int64_t)c.b * s.H + py) * s.W + px;
   float dLdp = 0.f, soft_saved = 0.f;
-  if (BWD && active) { dLdp = io.grad_soft[pix]; soft_saved = io.soft[pix]; }
+  if (active) { dLdp = a.grad_soft[pix]; soft_saved = a.soft[pix]; }
 
-  float allprob = 1.0f;
   int kid = 0;
   const int maxf = s.first ? (int)(__ldg(s.first + c.b + 1) - c.fbase) : s.F;
-  const size_t E = (size_t)256 * s.pool_K;
-  uint32_t* blk = nullptr;
-  bool first_window = true;
   int lo = -1;
   while (true) {
     int hi;
     int n = soft_window(s, c, sm, lo, maxf, hi);
-    if (!BWD && cache && first_window) {
-      first_window = false;
-      if (tid == 0) {
-        int slot = -1;
-        if (n > 0) {
-          slot = atomicAdd(s.pool_ctr, 1);
-          if (slot >= s.pool_tiles) {   // cache full: this tile is recomputed in backward
-            slot = -1;
-            s.fb_list[atomicAdd(s.fb_ctr, 1)] = tile_linear(s, c);
-          }
-        }
-        sm.pool_slot = slot;
-        sm.nent = 0;
-      }
-      __syncthreads();
-      if (sm.pool_slot >= 0) blk = s.pool_data + (size_t)sm.pool_slot * 3 * E;
-    }
     soft_sort(sm, n);  // by face index
     bool all_done = false;
     for (int c0 = 0; c0 < n && !all_done; c0 += kChunk) {
@@ -818,81 +837,42 @@ __device__ __forceinline__ void soft_tile(const Scene& s, const TileCtx& c, Tile
       __syncthreads();
       if (warp * 32 < na) {  // warps that own no uncovered pixel have nothing to do
         for (int j = 0; j < cn; ++j) {
-          const bool hit = active && kid < K && ((sm.cmask[j] & sel) == sel);
+          const bool hit = active && kid < a.K && ((sm.cmask[j] & sel) == sel);
           float g[6];
-          float prob = 0.f;
-          int edgeid = 0;
           if (hit) {
             const float4 q0 = sm.cxy0[j];
             const float2 q1 = sm.cxy1[j];
             const float v[6] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y};
+            int edgeid;
             const float d2 = soft_min_dist(x0, y0, v, s.multiplier, edgeid);
-            prob = soft_prob(d2, sigmainv, s.multiplier);
-            if (!BWD) {
-              allprob = soft_accumulate(allprob, prob);
-              if (KLISTS) {
-                const int64_t o = pix * K + kid;
-                io.kl.prob[o] = prob; io.kl.idx[o] = sm.cface[j]; io.kl.type[o] = (uint8_t)(edgeid + 1);
-              }
-            } else {
-              soft_backward_terms(x0, y0, v, edgeid, prob, soft_saved, dLdp, sigmainv, s.multiplier, g);
-            }
+            const float prob = soft_prob(d2, a.sigmainv, s.multiplier);
+            soft_backward_terms(x0, y0, v, edgeid, prob, soft_saved, dLdp, a.sigmainv, s.multiplier, g);
             ++kid;
           }
-          if (!BWD && blk != nullptr) {
-            const unsigned vote = __ballot_sync(kFull, hit);
-            if (vote) {
-              int wb = 0;
-              if (lane == 0) wb = atomicAdd(&sm.nent, __popc(vote));
-              wb = __shfl_sync(kFull, wb, 0);
-              if (hit) {
-                const size_t e = (size_t)wb + __popc(vote & ((1u << lane) - 1u));
-                blk[e] = (uint32_t)sm.cface[j];
-                blk[E + e] = __float_as_uint(prob);
-                blk[2 * E + e] = (uint32_t)lx | ((uint32_t)ly << 4) | ((uint32_t)(edgeid + 1) << 8);
-              }
-            }
-          }
-          if (BWD) {
-            if (__any_sync(kFull, hit)) {
+          if (__any_sync(kFull, hit)) {
 #pragma unroll
-              for (int q = 0; q < 6; ++q) {
-                float x = hit ? g[q] : 0.f;
+            for (int q = 0; q < 6; ++q) {
+              float x = hit ? g[q] : 0.f;
 #pragma unroll
-                for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(kFull, x, d);
-                if (lane == 0 && x != 0.f) atomicAdd(&sm.acc[j][q], x);
-              }
+              for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(kFull, x, d);
+              if (lane == 0 && x != 0.f) atomicAdd(&sm.acc[j][q], x);
             }
           }
         }
       }
-      all_done = __syncthreads_and(!active || kid >= K);
-      if (BWD) {
-        if (tid < cn) {
-          float* gp = io.grad_xy + (c.fbase + sm.cface[tid]) * 6;
+      all_done = __syncthreads_and(!active || kid >= a.K);
+      if (tid < cn) {
+        float* gp = a.grad_xy + (c.fbase + sm.cface[tid]) * 6;
 #pragma unroll
-          for (int q = 0; q < 6; ++q) {
-            const float x = sm.acc[tid][q];
-            if (x != 0.f) { atomicAdd(gp + q, x); sm.acc[tid][q] = 0.f; }
-          }
+        for (int q = 0; q < 6; ++q) {
+          const float x = sm.acc[tid][q];
+          if (x != 0.f) { atomicAdd(gp + q, x); sm.acc[tid][q] = 0.f; }
         }
-        __syncthreads();
       }
+      __syncthreads();
     }
     if (hi == 0x7fffffff || all_done) break;
     lo = hi;
-  }
-  if (!BWD) {
-    if (active) {
-      io.out_soft[pix] = soft_finish(allprob);
-      if (KLISTS) {
-        for (int k = kid; k < K; ++k) {
-          const int64_t o = pix * K + k;
-          io.kl.prob[o] = 0.f; io.kl.idx[o] = -1; io.kl.type[o] = 0;
-        }
-      }
-    }
-    if (blk != nullptr && tid == 0) s.pool_hdr[sm.pool_slot] = make_int4(c.b, c.tx, c.ty, sm.nent);
   }
 }
 
@@ -926,21 +906,13 @@ struct SoftSmem {
 };
 
 template <bool KLISTS>
-__device__ __forceinline__ void soft_tile_fwd(const Scene& s, const TileCtx& c, SoftSmem& sm, bool uncovered,
-                                              float sigmainv, int K, bool cache, const SoftIO& io) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const unsigned av = __ballot_sync(kFull, uncovered);
-  if (lane == 0) sm.wcount[warp] = __popc(av);
-  __syncthreads();
-  int before = 0, na = 0;
-#pragma unroll
-  for (int w = 0; w < kThreads / 32; ++w) {
-    const int cw = sm.wcount[w];
-    if (w < warp) before += cw;
-    na += cw;
-  }
+__device__ __forceinline__ void soft_tile_fwd(const FwdArgs& a, const TileCtx& c, SoftSmem& sm, bool uncovered) {
+  const Scene& s = a.s;
+  const int K = a.K;
+  const bool cache = !KLISTS && a.cache != 0;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  const int na = compact_uncovered(c, sm, uncovered);
   if (na == 0) return;  // uniform
-  if (uncovered) sm.apix[before + __popc(av & ((1u << lane) - 1u))] = (uint8_t)(c.lx | (c.ly << 4));
   __syncthreads();
   const bool active = tid < na;  // thread t owns the t-th uncovered pixel
   int lx = 0, ly = 0;
@@ -960,15 +932,7 @@ __device__ __forceinline__ void soft_tile_fwd(const Scene& s, const TileCtx& c, 
     if (first_window) {
       first_window = false;
       if (tid == 0) {
-        int slot = -1;
-        if (cache && n > 0) {
-          slot = atomicAdd(s.pool_ctr, 1);
-          if (slot >= s.pool_tiles) {   // cache full: this tile is recomputed in backward
-            slot = -1;
-            s.fb_list[atomicAdd(s.fb_ctr, 1)] = tile_linear(s, c);
-          }
-        }
-        sm.pool_slot = slot;
+        sm.pool_slot = cache && n > 0 ? claim_cache_block(s, c) : -1;
         sm.nent = 0;
       }
       __syncthreads();
@@ -1010,19 +974,7 @@ __device__ __forceinline__ void soft_tile_fwd(const Scene& s, const TileCtx& c, 
           }
         }
         if (!__syncthreads_or(took > 0)) break;
-        // face-major offsets
-        if (warp == 0) {
-          int v[8], sum = 0;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const int j = lane * 8 + i; v[i] = j < cn ? sm.cnt_c[j] : 0; sum += v[i]; }
-          int x = sum;
-#pragma unroll
-          for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(kFull, x, d); if (lane >= d) x += y; }
-          int run = x - sum;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const int j = lane * 8 + i; if (j < cn) sm.off_c[j] = run; run += v[i]; }
-          if (lane == 31) sm.npairs = x;
-        }
+        if (warp == 0) pair_offsets(sm, cn);
         __syncthreads();
         const int T = sm.npairs;
         const int ebase = sm.nent;
@@ -1047,7 +999,7 @@ __device__ __forceinline__ void soft_tile_fwd(const Scene& s, const TileCtx& c, 
           int edgeid;
           const float d2 = soft_min_dist(pix_x(s.grid, c.tile_x0 + plx), pix_y(s.grid, c.tile_y0 + ply), v,
                                          s.multiplier, edgeid);
-          const float prob = soft_prob(d2, sigmainv, s.multiplier);
+          const float prob = soft_prob(d2, a.sigmainv, s.multiplier);
           sm.res_prob[u] = prob;
           sm.res_type[u] = (uint8_t)(edgeid + 1);
           if (blk != nullptr) {
@@ -1066,7 +1018,7 @@ __device__ __forceinline__ void soft_tile_fwd(const Scene& s, const TileCtx& c, 
           allprob = soft_accumulate(allprob, prob);
           if (KLISTS) {
             const int64_t o = pix * K + kid;
-            io.kl.prob[o] = prob; io.kl.idx[o] = sm.cface[sm.pair_cand[slot]]; io.kl.type[o] = sm.res_type[slot];
+            a.kl.prob[o] = prob; a.kl.idx[o] = sm.cface[sm.pair_cand[slot]]; a.kl.type[o] = sm.res_type[slot];
           }
           ++kid;
         }
@@ -1076,7 +1028,7 @@ __device__ __forceinline__ void soft_tile_fwd(const Scene& s, const TileCtx& c, 
     if (hi == 0x7fffffff || all_done) break;
     lo = hi;
   }
-  if (active) io.out_soft[pix] = soft_finish(allprob);
+  if (active) a.out_soft[pix] = soft_finish(allprob);
   if (blk != nullptr && tid == 0) s.pool_hdr[sm.pool_slot] = make_int4(c.b, c.tx, c.ty, sm.nent);
 }
 
@@ -1093,22 +1045,11 @@ __device__ __forceinline__ void bins_from_record(const Scene& s, const int* rec,
 }
 
 __device__ __forceinline__ TileCtx tile_ctx_from_linear(const Scene& s, int t) {
-  TileCtx c;
   const int tiles_xy = s.ntx[0] * s.nty[0];
-  c.b = t / tiles_xy;
-  const int r = t - c.b * tiles_xy;
-  c.ty = r / s.ntx[0];
-  c.tx = r - c.ty * s.ntx[0];
-  c.tile_x0 = c.tx * kTile; c.tile_y0 = c.ty * kTile;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  c.lx = ((warp & 1) << 3) | (lane & 7);
-  c.ly = ((warp >> 1) << 2) | (lane >> 3);
-  c.px = c.tile_x0 + c.lx; c.py = c.tile_y0 + c.ly;
-  c.in_img = c.px < s.W && c.py < s.H;
-  c.x0 = 0.f; c.y0 = 0.f; c.sel = 0;
-  c.fbase = view_fbase(s, c.b);
-  c.pix = ((int64_t)c.b * s.H + c.py) * s.W + c.px;
-  return c;
+  const int b = t / tiles_xy;
+  const int r = t - b * tiles_xy;
+  const int ty = r / s.ntx[0];
+  return make_tile_ctx(s, b, r - ty * s.ntx[0], ty);
 }
 
 // ---------------------------------------------------------------------------
@@ -1128,27 +1069,97 @@ template <> struct Feat<__nv_bfloat16> {
   static __device__ __forceinline__ void st(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 };
 
+// Rasterize outputs of one pixel: face index, the optional weights and the interpolated features
+// (zeros where no face covers the pixel).
+template <typename FT>
+__device__ __forceinline__ void store_raster_pixel(const FwdArgs& a, int64_t pix, int64_t fbase, const RasterOut& o) {
+  a.idx[pix] = (int64_t)o.f;
+  if (a.out_w) {
+    float* wp = a.out_w + pix * 3;
+    wp[0] = o.w0; wp[1] = o.w1; wp[2] = o.w2;
+  }
+  FT* fp = static_cast<FT*>(a.out_feat) + pix * a.D;
+  const FT* feat = static_cast<const FT*>(a.feat);
+  if (a.D == 3) {  // the DIB-R tutorial shape (uv + mask), fully unrolled
+    float r[3] = {0.f, 0.f, 0.f};
+    if (o.f >= 0) {
+      const FT* ff = feat + (fbase + o.f) * 9;
+#pragma unroll
+      for (int d = 0; d < 3; ++d)
+        r[d] = raster_interp(Feat<FT>::ld(ff + d), Feat<FT>::ld(ff + 3 + d), Feat<FT>::ld(ff + 6 + d),
+                             o.w0, o.w1, o.w2);
+    }
+    Feat<FT>::st(fp, r[0]); Feat<FT>::st(fp + 1, r[1]); Feat<FT>::st(fp + 2, r[2]);
+  } else if (o.f >= 0) {
+    const FT* ff = feat + (fbase + o.f) * 3 * a.D;
+    for (int d = 0; d < a.D; ++d)
+      Feat<FT>::st(fp + d, raster_interp(Feat<FT>::ld(ff + d), Feat<FT>::ld(ff + a.D + d),
+                                         Feat<FT>::ld(ff + 2 * a.D + d), o.w0, o.w1, o.w2));
+  } else {
+    for (int d = 0; d < a.D; ++d) Feat<FT>::st(fp + d, 0.f);
+  }
+}
+
+// Files 16x16 tile (tx, ty) of view b in the soft-mask work list when an enlarged face rectangle
+// can reach it.  The record carries everything the soft-mask kernels need to start without
+// re-reading face_idx or the bin tables: the linear tile id, the uncovered-pixel ballots of its
+// 8 warps (ballot(q) for warp q) and its large-bin table (level 0: `bin0`, levels >= 1: `bins`)
+// as (offset, size) pairs.
+template <typename Ballot>
+__device__ __forceinline__ void file_band_tile(const Scene& s, int b, int tx, int ty, int64_t fbase, Ballot ballot,
+                                               const BinRef& bin0, const BinRef* bins) {
+  const int nlarge = ((__ldg(s.tile_cnt + ((size_t)b * s.nty[0] + ty) * ((s.ntx[0] + 31) >> 5) + (tx >> 5)) >> (tx & 31)) & 1) +
+                     __ldg(s.view_flag + b);
+  if (nlarge > 0) {
+    int* rec = s.band_list + (size_t)atomicAdd(s.band_ctr, 1) * kBandRec;
+    const int4* ebase = s.entries + (size_t)4 * s.NF + 4 * fbase;
+    rec[0] = (b * s.nty[0] + ty) * s.ntx[0] + tx;
+    for (int q = 0; q < kThreads / 32; ++q) rec[1 + q] = ballot(q);
+    for (int l = 0; l < kMaxLevels; ++l) {
+      const BinRef br = l == 0 ? bin0 : bins[l];
+      rec[9 + 2 * l] = br.n > 0 ? (int)(br.ptr - ebase) : 0;
+      rec[10 + 2 * l] = br.n;
+    }
+  }
+}
+
+// Soft-mask defaults of one pixel of 16x16 tile (tx, ty) (covered: 1; uncovered with no neighbour:
+// 1 - 1 = 0) and its K-list padding; tiles where an uncovered pixel may lie under an enlarged face
+// go to the soft-mask work list.  No CTA barrier: warps retire independently through the tile's
+// shared `uncmask`, `any_uncovered` and `warps_done`, and the last one to finish files the tile.
+template <bool KLISTS>
+__device__ __forceinline__ void soft_defaults(const FwdArgs& a, int b, int tx, int ty, int64_t fbase, bool in_img,
+                                              int64_t pix, int best_f, unsigned* uncmask, int* any_uncovered,
+                                              int* warps_done, const BinRef& bin0, const BinRef* bins) {
+  const bool uncovered = in_img && best_f < 0;
+  if (in_img) {
+    a.out_soft[pix] = uncovered ? 0.0f : 1.0f;
+    if (KLISTS) {  // padding the reference gets from at::zeros / at::full(-1)
+      for (int k = 0; k < a.K; ++k) {
+        const int64_t o = pix * a.K + k;
+        a.kl.prob[o] = 0.f; a.kl.idx[o] = -1; a.kl.type[o] = 0;
+      }
+    }
+  }
+  const int tid = threadIdx.x;
+  const unsigned wv = __ballot_sync(kFull, uncovered);
+  if ((tid & 31) == 0) {
+    uncmask[tid >> 5] = wv;
+    if (wv) atomicOr(any_uncovered, 1);
+    __threadfence_block();
+    if (atomicAdd(warps_done, 1) == kThreads / 32 - 1 && atomicOr(any_uncovered, 0))
+      file_band_tile(a.s, b, tx, ty, fbase, [&](int q) { return (int)atomicOr(uncmask + q, 0u); }, bin0, bins);
+  }
+}
+
 // ---------------------------------------------------------------------------
 // Forward tile kernel.
-struct FwdArgs {
-  Scene s;
-  RasterConst rc;
-  int D;
-  const void* feat;         // (NF,3,D) FT
-  float sigmainv; int K;
-  int cache;                // fill the soft-mask hit cache
-  int from_fb;              // soft_tiles_fwd_kernel: walk fb_list instead of band_list
-  void* out_feat;           // (B,H,W,D) FT
-  int64_t* idx; float* out_w; float* out_soft;  // idx: output if RASTER else input
-  SoftFwdOut kl;
-};
-
 template <bool RASTER, bool SOFT, bool KLISTS, typename FT>
 __global__ void __launch_bounds__(kThreads, 6) dibr_tile_fwd_kernel(const __grid_constant__ FwdArgs a) {
   __shared__ __align__(128) RasterSmem sm;
   const Scene& s = a.s;
   const int tid = threadIdx.x;
-  const TileCtx c = make_tile_ctx(s);
+  const TileCtx c = make_tile_ctx(s, blockIdx.z, blockIdx.x, blockIdx.y);   // grid = (tiles_x, tiles_y, views)
   if (RASTER && tid == 32) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); mbar_fence_init(); }
   if (tid == 64) { sm.any_uncovered = 0; sm.warps_done = 0; }
   load_bin_table(s, c, sm);
@@ -1158,73 +1169,13 @@ __global__ void __launch_bounds__(kThreads, 6) dibr_tile_fwd_kernel(const __grid
     RasterOut o;
     raster_tile(s, c, a.rc, sm, o);
     best_f = o.f;
-    if (c.in_img) {
-      a.idx[c.pix] = (int64_t)o.f;
-      if (a.out_w) {
-        float* wp = a.out_w + c.pix * 3;
-        wp[0] = o.w0; wp[1] = o.w1; wp[2] = o.w2;
-      }
-      FT* fp = static_cast<FT*>(a.out_feat) + c.pix * a.D;
-      const FT* feat = static_cast<const FT*>(a.feat);
-      if (a.D == 3) {  // the DIB-R tutorial shape (uv + mask), fully unrolled
-        float r[3] = {0.f, 0.f, 0.f};
-        if (o.f >= 0) {
-          const FT* ff = feat + (c.fbase + o.f) * 9;
-#pragma unroll
-          for (int d = 0; d < 3; ++d)
-            r[d] = raster_interp(Feat<FT>::ld(ff + d), Feat<FT>::ld(ff + 3 + d), Feat<FT>::ld(ff + 6 + d),
-                                 o.w0, o.w1, o.w2);
-        }
-        Feat<FT>::st(fp, r[0]); Feat<FT>::st(fp + 1, r[1]); Feat<FT>::st(fp + 2, r[2]);
-      } else if (o.f >= 0) {
-        const FT* ff = feat + (c.fbase + o.f) * 3 * a.D;
-        for (int d = 0; d < a.D; ++d)
-          Feat<FT>::st(fp + d, raster_interp(Feat<FT>::ld(ff + d), Feat<FT>::ld(ff + a.D + d),
-                                             Feat<FT>::ld(ff + 2 * a.D + d), o.w0, o.w1, o.w2));
-      } else {
-        for (int d = 0; d < a.D; ++d) Feat<FT>::st(fp + d, 0.f);
-      }
-    }
+    if (c.in_img) store_raster_pixel<FT>(a, c.pix, c.fbase, o);
   } else {
     best_f = c.in_img ? (int)a.idx[c.pix] : 0;
   }
-  if (SOFT) {
-    // defaults (covered: 1; uncovered with no neighbour: 1 - 1 = 0) and K-list padding; tiles
-    // where an uncovered pixel may lie under an enlarged face go to the soft-mask work list
-    const bool uncovered = c.in_img && best_f < 0;
-    if (c.in_img) {
-      a.out_soft[c.pix] = uncovered ? 0.0f : 1.0f;
-      if (KLISTS) {  // padding the reference gets from at::zeros / at::full(-1)
-        for (int k = 0; k < a.K; ++k) {
-          const int64_t o = c.pix * a.K + k;
-          a.kl.prob[o] = 0.f; a.kl.idx[o] = -1; a.kl.type[o] = 0;
-        }
-      }
-    }
-    // no CTA barrier: warps retire independently; the last one to finish files the tile
-    const unsigned wv = __ballot_sync(kFull, uncovered);
-    if ((tid & 31) == 0) {
-      sm.uncmask[tid >> 5] = wv;
-      if (wv) atomicOr(&sm.any_uncovered, 1);
-      __threadfence_block();
-      if (atomicAdd(&sm.warps_done, 1) == kThreads / 32 - 1 && atomicOr(&sm.any_uncovered, 0)) {
-        const int nlarge = ((__ldg(s.tile_cnt + ((size_t)c.b * s.nty[0] + c.ty) * ((s.ntx[0] + 31) >> 5) + (c.tx >> 5)) >> (c.tx & 31)) & 1) +
-                           __ldg(s.view_flag + c.b);
-        if (nlarge > 0) {
-          // work-list record: everything the soft-mask kernels need to start without
-          // re-reading face_idx or the bin tables
-          int* rec = s.band_list + (size_t)atomicAdd(s.band_ctr, 1) * kBandRec;
-          const int4* ebase = s.entries + (size_t)4 * s.NF + 4 * c.fbase;
-          rec[0] = tile_linear(s, c);
-          for (int q = 0; q < kThreads / 32; ++q) rec[1 + q] = (int)atomicOr(&sm.uncmask[q], 0u);
-          for (int l = 0; l < kMaxLevels; ++l) {
-            rec[9 + 2 * l] = sm.bin[1][l].n > 0 ? (int)(sm.bin[1][l].ptr - ebase) : 0;
-            rec[10 + 2 * l] = sm.bin[1][l].n;
-          }
-        }
-      }
-    }
-  }
+  if (SOFT)
+    soft_defaults<KLISTS>(a, c.b, c.tx, c.ty, c.fbase, c.in_img, c.pix, best_f, sm.uncmask, &sm.any_uncovered,
+                          &sm.warps_done, sm.bin[1][0], sm.bin[1]);
 }
 
 // ---------------------------------------------------------------------------
@@ -1301,7 +1252,7 @@ __device__ __noinline__ void make_edge_tests(const float v[6], double X0, double
 }
 
 #define DIBR_FWD2_MINB 4   /* H100, c4_shard: 4 CTAs/SM 0.97 ms, 5: 0.98, 6: 1.10, 8: 1.59 */
-template <bool RASTER, bool SOFT, bool KLISTS, typename FT>
+template <bool SOFT, typename FT>
 __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(const __grid_constant__ FwdArgs a) {
   constexpr int kPieces = kSubs + kMaxLevels - 1;
   __shared__ __align__(128) FwdSmem sm;
@@ -1312,7 +1263,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
   const int cta_x0 = ctx0 * kTile, cta_y0 = cty0 * kTile;
   const int64_t fbase = view_fbase(s, b);
 
-  if (RASTER && tid == 32) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); mbar_fence_init(); }
+  if (tid == 32) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); mbar_fence_init(); }
   if (tid >= 64 && tid < 64 + kSubs) { sm.any_uncovered[tid - 64] = 0; sm.warps_done[tid - 64] = 0; }
   if (tid < 2 * kSubs) {
     const int set = tid / kSubs, sub = tid % kSubs;
@@ -1333,10 +1284,8 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
   // the tight bins above the CTA tile as one virtual list: 4 level-0 pieces, then levels 1..
   auto pn = [&](int p) { return p < kSubs ? sm.bin0[0][p].n : sm.bin[0][p - kSubs + 1].n; };
   int total = 0;
-  if (RASTER) {
 #pragma unroll
-    for (int p = 0; p < kPieces; ++p) total += pn(p);
-  }
+  for (int p = 0; p < kPieces; ++p) total += pn(p);
   const int nrounds = (total + kChunk - 1) / kChunk;
   int issued = 0, waited = 0;       // staging iterations (thread 0 / everyone): buffer = n & 1, parity = (n >> 1) & 1
   auto issue = [&](int k) {          // thread 0 only
@@ -1359,7 +1308,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
 
   // ---- CTA tiles that no valid face touches (40 % of them on the benchmark scene): the outputs are
   // constants, written as full 16-byte vectors row by row (9 stores per thread instead of 32)
-  if (RASTER && !KLISTS && total == 0 && cta_x0 + kSide <= s.W && cta_y0 + kSide <= s.H && (s.W & 3) == 0 &&
+  if (total == 0 && cta_x0 + kSide <= s.W && cta_y0 + kSide <= s.H && (s.W & 3) == 0 &&
       std::is_same<FT, float>::value && a.D == 3) {
     const int64_t pix_row0 = ((int64_t)b * s.H + cta_y0) * s.W + cta_x0;
     const int4 neg = make_int4(-1, -1, -1, -1);
@@ -1379,22 +1328,9 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
         const int r = c / kSC, ch = c - r * kSC;
         reinterpret_cast<float4*>(a.out_soft + pix_row0 + (int64_t)r * s.W)[ch] = zero;   // uncovered, no neighbour yet
       }
-      if (tid < kSubs) {   // every pixel is uncovered: file the sub-tiles an enlarged face can reach
-        const int tx = ctx0 + tid % 2, ty = cty0 + tid / 2;
-        const int nlarge = ((__ldg(s.tile_cnt + ((size_t)b * s.nty[0] + ty) * ((s.ntx[0] + 31) >> 5) + (tx >> 5)) >> (tx & 31)) & 1) +
-                           __ldg(s.view_flag + b);
-        if (nlarge > 0) {
-          int* rec = s.band_list + (size_t)atomicAdd(s.band_ctr, 1) * kBandRec;
-          const int4* ebase = s.entries + (size_t)4 * s.NF + 4 * fbase;
-          rec[0] = (b * s.nty[0] + ty) * s.ntx[0] + tx;
-          for (int q = 0; q < kThreads / 32; ++q) rec[1 + q] = -1;
-          for (int l = 0; l < kMaxLevels; ++l) {
-            const BinRef br = l == 0 ? sm.bin0[1][tid] : sm.bin[1][l];
-            rec[9 + 2 * l] = br.n > 0 ? (int)(br.ptr - ebase) : 0;
-            rec[10 + 2 * l] = br.n;
-          }
-        }
-      }
+      // every pixel is uncovered: file the sub-tiles an enlarged face can reach
+      if (tid < kSubs)
+        file_band_tile(s, b, ctx0 + tid % 2, cty0 + tid / 2, fbase, [](int) { return -1; }, sm.bin0[1][tid], sm.bin[1]);
     }
     return;
   }
@@ -1408,192 +1344,125 @@ __global__ void __launch_bounds__(kThreads, DIBR_FWD2_MINB) dibr_fwd2_kernel(con
     const int px = tx * kTile + lx, py = ty * kTile + ly;
     const bool in_img = px < s.W && py < s.H;
     const int64_t pix = ((int64_t)b * s.H + py) * s.W + px;
-    int best_f;
-    if (RASTER) {
-      RasterOut o;
-      o.z = -INFINITY; o.f = -1; o.w0 = o.w1 = o.w2 = 0.f;
-      if (total > 0) {
-        const float x0 = pix_x(s.grid, px), y0 = pix_y(s.grid, py);
-        const int clx = sx * kTile + lx, cly = sy * kTile + ly;
-        const float fbx0 = (float)(sx * kTile + ((warp & 1) << 3)), fbx1 = fbx0 + 7.f;
-        const float fby0 = (float)(sy * kTile + ((warp >> 1) << 2)), fby1 = fby0 + 3.f;
-        for (int k = 0; k < nrounds; ++k) {
-          const int cnt = min(kChunk, total - k * kChunk);
-          if (!(staged && nrounds == 1)) {
-            // ---- stage round k: TMA -> cull against the CTA tile -> face records, edge tests, bit matrices
-            if (tid == 0) {
-              if (k == 0) issue(0);
-              if (k + 1 < nrounds) issue(k + 1);   // its buffer was released by the barrier ending round k-1
-            }
-            const int buf = waited & 1;
-            // only the warps that read the landing buffer poll the mbarrier; the others go
-            // straight to the CTA barrier below and sleep there (256 polling threads cost 5 % of
-            // the kernel's instructions in the first version)
-            if ((tid & ~31) < cnt) mbar_wait(&sm.bar[buf], (uint32_t)((waited >> 1) & 1));
-            ++waited;
-            uint32_t cm = 0, rm = 0;
-            if (tid < cnt) {
-              const int4 e = sm.stage[buf][tid];
-              const int x_lo = e.y & 0xffff, x_hi = (int)((unsigned)e.y >> 16);
-              const int y_lo = e.z & 0xffff, y_hi = (int)((unsigned)e.z >> 16);
-              // level-0 pieces: the face is also in the neighbouring bins it spans; take it from
-              // the first of its bins inside this CTA only
-              bool take = true;
-              const int vi = k * kChunk + tid;
-              int start = 0;
-#pragma unroll
-              for (int p = 0; p < kSubs; ++p) {
-                const int np = pn(p);
-                if (vi >= start && vi < start + np)
-                  take = (ctx0 + p % 2) == max(x_lo >> 4, ctx0) && (cty0 + p / 2) == max(y_lo >> 4, cty0);
-                start += np;
-              }
-              if (take) {
-                const int cx0 = max(x_lo - cta_x0, 0), cx1 = min(x_hi - cta_x0, kSide);
-                const int cy0 = max(y_lo - cta_y0, 0), cy1 = min(y_hi - cta_y0, kSide);
-                if (cx1 > cx0 && cy1 > cy0) {
-                  cm = (uint32_t)(((1ull << cx1) - 1ull) & ~((1ull << cx0) - 1ull));
-                  rm = (uint32_t)(((1ull << cy1) - 1ull) & ~((1ull << cy0) - 1ull));
-                }
-              }
-              if (cm) {
-                const int64_t g = fbase + e.x;
-                float v[6];
-                load_xy(s, g, v);
-                const float* zp = s.z + g * 3;
-                sm.cxy0[tid] = make_float4(v[0], v[1], v[2], v[3]);
-                sm.cxy1[tid] = make_float2(v[4], v[5]);
-                sm.cz[tid] = make_float4(__ldg(zp), __ldg(zp + 1), __ldg(zp + 2), 0.f);
-                sm.cface[tid] = e.x;
-                float4 et[3];
-                make_edge_tests(v, (double)pix_x(s.grid, cta_x0), (double)pix_y(s.grid, cta_y0),
-                                2.0 * (double)s.grid.inv_w, 2.0 * (double)s.grid.inv_h, kSide, et);
-                sm.cedge[tid][0] = et[0]; sm.cedge[tid][1] = et[1]; sm.cedge[tid][2] = et[2];
-              }
-            }
-            if ((tid & ~31) < cnt) {
-              // transpose the rectangle masks of this warp's 32 candidates into per-column / per-row words
-              const int g = tid >> 5;
-              if (__any_sync(kFull, cm != 0)) {
-                uint32_t mine_c = 0, mine_r = 0;
-#pragma unroll
-                for (int q = 0; q < kSide; ++q) {
-                  const uint32_t c = __ballot_sync(kFull, (cm >> q) & 1u);
-                  const uint32_t r = __ballot_sync(kFull, (rm >> q) & 1u);
-                  if (lane == (q & 31)) { mine_c = c; mine_r = r; }
-                }
-                if (lane < kSide) { sm.colbits[g][lane] = mine_c; sm.rowbits[g][lane] = mine_r; }
-              } else if (lane < kSide) {
-                sm.colbits[g][lane] = 0; sm.rowbits[g][lane] = 0;
-              }
-            }
-            __syncthreads();
+    RasterOut o;
+    o.z = -INFINITY; o.f = -1; o.w0 = o.w1 = o.w2 = 0.f;
+    if (total > 0) {
+      const float x0 = pix_x(s.grid, px), y0 = pix_y(s.grid, py);
+      const int clx = sx * kTile + lx, cly = sy * kTile + ly;
+      const float fbx0 = (float)(sx * kTile + ((warp & 1) << 3)), fbx1 = fbx0 + 7.f;
+      const float fby0 = (float)(sy * kTile + ((warp >> 1) << 2)), fby1 = fby0 + 3.f;
+      for (int k = 0; k < nrounds; ++k) {
+        const int cnt = min(kChunk, total - k * kChunk);
+        if (!(staged && nrounds == 1)) {
+          // ---- stage round k: TMA -> cull against the CTA tile -> face records, edge tests, bit matrices
+          if (tid == 0) {
+            if (k == 0) issue(0);
+            if (k + 1 < nrounds) issue(k + 1);   // its buffer was released by the barrier ending round k-1
           }
-          // ---- rasterize this sub-tile against the staged round
-          const int ngroups = (cnt + 31) >> 5;
-          for (int g = 0; g < ngroups; ++g) {
-            const uint32_t mybits = sm.colbits[g][clx] & sm.rowbits[g][cly];
-            const uint32_t uni = __reduce_or_sync(kFull, mybits);   // candidates whose rectangle meets the block
-            if (!uni) continue;
-            bool keep = false;
-            if ((uni >> lane) & 1u) {                                 // lane j: candidate j against the block's corners
-              const float4 e0 = sm.cedge[(g << 5) + lane][0], e1 = sm.cedge[(g << 5) + lane][1],
-                           e2 = sm.cedge[(g << 5) + lane][2];
-              const float h0 = e0.x + fmaxf(e0.y * fbx0, e0.y * fbx1) + fmaxf(e0.z * fby0, e0.z * fby1);
-              const float h1 = e1.x + fmaxf(e1.y * fbx0, e1.y * fbx1) + fmaxf(e1.z * fby0, e1.z * fby1);
-              const float h2 = e2.x + fmaxf(e2.y * fbx0, e2.y * fbx1) + fmaxf(e2.z * fby0, e2.z * fby1);
-              keep = !(h0 < 0.f || h1 < 0.f || h2 < 0.f);
+          const int buf = waited & 1;
+          // only the warps that read the landing buffer poll the mbarrier; the others go
+          // straight to the CTA barrier below and sleep there (256 polling threads cost 5 % of
+          // the kernel's instructions in the first version)
+          if ((tid & ~31) < cnt) mbar_wait(&sm.bar[buf], (uint32_t)((waited >> 1) & 1));
+          ++waited;
+          uint32_t cm = 0, rm = 0;
+          if (tid < cnt) {
+            const int4 e = sm.stage[buf][tid];
+            const int x_lo = e.y & 0xffff, x_hi = (int)((unsigned)e.y >> 16);
+            const int y_lo = e.z & 0xffff, y_hi = (int)((unsigned)e.z >> 16);
+            // level-0 pieces: the face is also in the neighbouring bins it spans; take it from
+            // the first of its bins inside this CTA only
+            bool take = true;
+            const int vi = k * kChunk + tid;
+            int start = 0;
+#pragma unroll
+            for (int p = 0; p < kSubs; ++p) {
+              const int np = pn(p);
+              if (vi >= start && vi < start + np)
+                take = (ctx0 + p % 2) == max(x_lo >> 4, ctx0) && (cty0 + p / 2) == max(y_lo >> 4, cty0);
+              start += np;
             }
-            uint32_t surv = __ballot_sync(kFull, keep);
-            while (surv) {                                            // warp-uniform loop
-              const int jj = __ffs(surv) - 1;
-              surv &= surv - 1;
-              if (!((mybits >> jj) & 1u)) continue;
-              const int j = (g << 5) + jj;
-              const float4 q0 = sm.cxy0[j];
-              const float2 q1 = sm.cxy1[j];
-              float w0, w1, w2;
-              if (!raster_weights(a.rc, x0, y0, q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, w0, w1, w2)) continue;
-              const float4 zz = sm.cz[j];
-              const float zv = raster_depth(zz.x, zz.y, zz.z, w0, w1, w2);
-              const int f = sm.cface[j];
-              // reference: strict '>' in ascending face order == (z, lowest index) maximum
-              if (!(zv <= o.z) || (zv == o.z && f < o.f)) { o.z = zv; o.f = f; o.w0 = w0; o.w1 = w1; o.w2 = w2; }
+            if (take) {
+              const int cx0 = max(x_lo - cta_x0, 0), cx1 = min(x_hi - cta_x0, kSide);
+              const int cy0 = max(y_lo - cta_y0, 0), cy1 = min(y_hi - cta_y0, kSide);
+              if (cx1 > cx0 && cy1 > cy0) {
+                cm = (uint32_t)(((1ull << cx1) - 1ull) & ~((1ull << cx0) - 1ull));
+                rm = (uint32_t)(((1ull << cy1) - 1ull) & ~((1ull << cy0) - 1ull));
+              }
+            }
+            if (cm) {
+              const int64_t g = fbase + e.x;
+              float v[6];
+              load_xy(s, g, v);
+              const float* zp = s.z + g * 3;
+              sm.cxy0[tid] = make_float4(v[0], v[1], v[2], v[3]);
+              sm.cxy1[tid] = make_float2(v[4], v[5]);
+              sm.cz[tid] = make_float4(__ldg(zp), __ldg(zp + 1), __ldg(zp + 2), 0.f);
+              sm.cface[tid] = e.x;
+              float4 et[3];
+              make_edge_tests(v, (double)pix_x(s.grid, cta_x0), (double)pix_y(s.grid, cta_y0),
+                              2.0 * (double)s.grid.inv_w, 2.0 * (double)s.grid.inv_h, kSide, et);
+              sm.cedge[tid][0] = et[0]; sm.cedge[tid][1] = et[1]; sm.cedge[tid][2] = et[2];
             }
           }
-          if (nrounds > 1) __syncthreads();   // the next round overwrites the staged arrays
+          if ((tid & ~31) < cnt) {
+            // transpose the rectangle masks of this warp's 32 candidates into per-column / per-row words
+            const int g = tid >> 5;
+            if (__any_sync(kFull, cm != 0)) {
+              uint32_t mine_c = 0, mine_r = 0;
+#pragma unroll
+              for (int q = 0; q < kSide; ++q) {
+                const uint32_t c = __ballot_sync(kFull, (cm >> q) & 1u);
+                const uint32_t r = __ballot_sync(kFull, (rm >> q) & 1u);
+                if (lane == (q & 31)) { mine_c = c; mine_r = r; }
+              }
+              if (lane < kSide) { sm.colbits[g][lane] = mine_c; sm.rowbits[g][lane] = mine_r; }
+            } else if (lane < kSide) {
+              sm.colbits[g][lane] = 0; sm.rowbits[g][lane] = 0;
+            }
+          }
+          __syncthreads();
         }
-        staged = true;
+        // ---- rasterize this sub-tile against the staged round
+        const int ngroups = (cnt + 31) >> 5;
+        for (int g = 0; g < ngroups; ++g) {
+          const uint32_t mybits = sm.colbits[g][clx] & sm.rowbits[g][cly];
+          const uint32_t uni = __reduce_or_sync(kFull, mybits);   // candidates whose rectangle meets the block
+          if (!uni) continue;
+          bool keep = false;
+          if ((uni >> lane) & 1u) {                                 // lane j: candidate j against the block's corners
+            const float4 e0 = sm.cedge[(g << 5) + lane][0], e1 = sm.cedge[(g << 5) + lane][1],
+                         e2 = sm.cedge[(g << 5) + lane][2];
+            const float h0 = e0.x + fmaxf(e0.y * fbx0, e0.y * fbx1) + fmaxf(e0.z * fby0, e0.z * fby1);
+            const float h1 = e1.x + fmaxf(e1.y * fbx0, e1.y * fbx1) + fmaxf(e1.z * fby0, e1.z * fby1);
+            const float h2 = e2.x + fmaxf(e2.y * fbx0, e2.y * fbx1) + fmaxf(e2.z * fby0, e2.z * fby1);
+            keep = !(h0 < 0.f || h1 < 0.f || h2 < 0.f);
+          }
+          uint32_t surv = __ballot_sync(kFull, keep);
+          while (surv) {                                            // warp-uniform loop
+            const int jj = __ffs(surv) - 1;
+            surv &= surv - 1;
+            if (!((mybits >> jj) & 1u)) continue;
+            const int j = (g << 5) + jj;
+            const float4 q0 = sm.cxy0[j];
+            const float2 q1 = sm.cxy1[j];
+            float w0, w1, w2;
+            if (!raster_weights(a.rc, x0, y0, q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, w0, w1, w2)) continue;
+            const float4 zz = sm.cz[j];
+            const float zv = raster_depth(zz.x, zz.y, zz.z, w0, w1, w2);
+            const int f = sm.cface[j];
+            // reference: strict '>' in ascending face order == (z, lowest index) maximum
+            if (!(zv <= o.z) || (zv == o.z && f < o.f)) { o.z = zv; o.f = f; o.w0 = w0; o.w1 = w1; o.w2 = w2; }
+          }
+        }
+        if (nrounds > 1) __syncthreads();   // the next round overwrites the staged arrays
       }
-      best_f = o.f;
-      if (in_img) {
-        a.idx[pix] = (int64_t)o.f;
-        if (a.out_w) {
-          float* wp = a.out_w + pix * 3;
-          wp[0] = o.w0; wp[1] = o.w1; wp[2] = o.w2;
-        }
-        FT* fp = static_cast<FT*>(a.out_feat) + pix * a.D;
-        const FT* feat = static_cast<const FT*>(a.feat);
-        if (a.D == 3) {  // the DIB-R tutorial shape (uv + mask), fully unrolled
-          float r[3] = {0.f, 0.f, 0.f};
-          if (o.f >= 0) {
-            const FT* ff = feat + (fbase + o.f) * 9;
-#pragma unroll
-            for (int d = 0; d < 3; ++d)
-              r[d] = raster_interp(Feat<FT>::ld(ff + d), Feat<FT>::ld(ff + 3 + d), Feat<FT>::ld(ff + 6 + d),
-                                   o.w0, o.w1, o.w2);
-          }
-          Feat<FT>::st(fp, r[0]); Feat<FT>::st(fp + 1, r[1]); Feat<FT>::st(fp + 2, r[2]);
-        } else if (o.f >= 0) {
-          const FT* ff = feat + (fbase + o.f) * 3 * a.D;
-          for (int d = 0; d < a.D; ++d)
-            Feat<FT>::st(fp + d, raster_interp(Feat<FT>::ld(ff + d), Feat<FT>::ld(ff + a.D + d),
-                                               Feat<FT>::ld(ff + 2 * a.D + d), o.w0, o.w1, o.w2));
-        } else {
-          for (int d = 0; d < a.D; ++d) Feat<FT>::st(fp + d, 0.f);
-        }
-      }
-    } else {
-      best_f = in_img ? (int)a.idx[pix] : 0;
+      staged = true;
     }
-    if (SOFT) {
-      // defaults (covered: 1; uncovered with no neighbour: 1 - 1 = 0) and K-list padding; tiles
-      // where an uncovered pixel may lie under an enlarged face go to the soft-mask work list
-      const bool uncovered = in_img && best_f < 0;
-      if (in_img) {
-        a.out_soft[pix] = uncovered ? 0.0f : 1.0f;
-        if (KLISTS) {  // padding the reference gets from at::zeros / at::full(-1)
-          for (int k = 0; k < a.K; ++k) {
-            const int64_t o = pix * a.K + k;
-            a.kl.prob[o] = 0.f; a.kl.idx[o] = -1; a.kl.type[o] = 0;
-          }
-        }
-      }
-      // no CTA barrier: warps retire independently; the last one to finish files the tile
-      const unsigned wv = __ballot_sync(kFull, uncovered);
-      if (lane == 0) {
-        sm.uncmask[sub][warp] = wv;
-        if (wv) atomicOr(&sm.any_uncovered[sub], 1);
-        __threadfence_block();
-        if (atomicAdd(&sm.warps_done[sub], 1) == kThreads / 32 - 1 && atomicOr(&sm.any_uncovered[sub], 0)) {
-          const int nlarge = ((__ldg(s.tile_cnt + ((size_t)b * s.nty[0] + ty) * ((s.ntx[0] + 31) >> 5) + (tx >> 5)) >> (tx & 31)) & 1) +
-                             __ldg(s.view_flag + b);
-          if (nlarge > 0) {
-            // work-list record: everything the soft-mask kernels need to start without
-            // re-reading face_idx or the bin tables
-            int* rec = s.band_list + (size_t)atomicAdd(s.band_ctr, 1) * kBandRec;
-            const int4* ebase = s.entries + (size_t)4 * s.NF + 4 * fbase;
-            rec[0] = (b * s.nty[0] + ty) * s.ntx[0] + tx;
-            for (int q = 0; q < kThreads / 32; ++q) rec[1 + q] = (int)atomicOr(&sm.uncmask[sub][q], 0u);
-            for (int l = 0; l < kMaxLevels; ++l) {
-              const BinRef br = l == 0 ? sm.bin0[1][sub] : sm.bin[1][l];
-              rec[9 + 2 * l] = br.n > 0 ? (int)(br.ptr - ebase) : 0;
-              rec[10 + 2 * l] = br.n;
-            }
-          }
-        }
-      }
-    }
+    if (in_img) store_raster_pixel<FT>(a, pix, fbase, o);
+    if (SOFT)
+      soft_defaults<false>(a, b, tx, ty, fbase, in_img, pix, o.f, sm.uncmask[sub], &sm.any_uncovered[sub],
+                           &sm.warps_done[sub], sm.bin0[1][sub], sm.bin[1]);
   }
 }
 
@@ -1604,14 +1473,12 @@ __global__ void __launch_bounds__(kThreads, 4) soft_tiles_fwd_kernel(const __gri
   SoftSmem& sm = *reinterpret_cast<SoftSmem*>(soft_smem_raw);
   const Scene& s = a.s;
   const int total = min(a.from_fb ? *s.fb_ctr : *s.band_ctr, s.ntx[0] * s.nty[0] * s.B);
-  SoftIO io;
-  io.out_soft = a.out_soft; io.kl = a.kl; io.grad_soft = nullptr; io.soft = nullptr; io.grad_xy = nullptr;
   for (int w = blockIdx.x; w < total; w += gridDim.x) {
     const TileCtx c = tile_ctx_from_linear(s, a.from_fb ? s.fb_list[w] : s.band_list[(size_t)w * kBandRec]);
     __syncthreads();  // previous tile's shared state fully consumed
     load_bin_table(s, c, sm);
     __syncthreads();
-    soft_tile_fwd<KLISTS>(s, c, sm, c.in_img && a.idx[c.pix] < 0, a.sigmainv, a.K, !KLISTS && a.cache != 0, io);
+    soft_tile_fwd<KLISTS>(a, c, sm, c.in_img && a.idx[c.pix] < 0);
   }
 }
 
@@ -1699,13 +1566,8 @@ __global__ void __launch_bounds__(kThreads, DIBR_SOFT_FWD_MINB) soft_fwd_kernel(
         first_window = false;
         if (n == 0) { cached = false; break; }  // uncovered pixels, but no face near them: soft stays 0
         // cache block: one atomic, its round trip hidden behind the sort below
-        if (tid == 0) {
-          int slot = atomicAdd(s.pool_ctr, 1);
-          if (slot >= s.pool_tiles) {   // cache full: single-kernel path + recompute in backward
-            slot = -1;
-            s.fb_list[atomicAdd(s.fb_ctr, 1)] = tile_linear(s, c);
-          }
-          sm.pool_slot = slot;
+        if (tid == 0) {   // cache full: single-kernel path + recompute in backward
+          sm.pool_slot = claim_cache_block(s, c);
           sm.nent = 0;
         }
       }
@@ -1748,18 +1610,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_SOFT_FWD_MINB) soft_fwd_kernel(
           }
         }
         __syncthreads();
-        if (warp == 0) {  // face-major offsets
-          int v[8], sum = 0;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const int j = lane * 8 + i; v[i] = j < cn ? sm.cnt_c[j] : 0; sum += v[i]; }
-          int x = sum;
-#pragma unroll
-          for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(kFull, x, d); if (lane >= d) x += y; }
-          int run = x - sum;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const int j = lane * 8 + i; if (j < cn) sm.off_c[j] = run; run += v[i]; }
-          if (lane == 31) sm.npairs = x;
-        }
+        if (warp == 0) pair_offsets(sm, cn);
         __syncthreads();
         const int ebase = sm.nent, T = sm.npairs;
         // pair -> (pixel, candidate) map in the meta words; the CTA reads it back after the barrier
@@ -1822,18 +1673,7 @@ __global__ void __launch_bounds__(kThreads, DIBR_SOFT_FWD_MINB) soft_fwd_kernel(
 }
 
 // ---------------------------------------------------------------------------
-// Soft-mask backward.  (1) dense kernel over the hit cache; (2) the recompute tile
-// kernel for the tiles the cache could not hold (fb_list) or, with no forward state,
-// for every tile.  Persistent CTAs walk the work list.
-struct SoftBwdArgs {
-  Scene s;
-  float sigmainv; int K;
-  int from_list;             // 1: tiles of fb_list only; 0: every tile
-  int view_begin, view_end;  // only tiles / cache blocks of these views (dibr_b200_backward_views)
-  const float* grad_soft; const float* soft; const int64_t* idx;
-  float* grad_xy;
-};
-
+// Soft-mask backward: the recompute tile kernel, then the dense kernel over the hit cache.
 __global__ void __launch_bounds__(kThreads) dibr_tile_soft_bwd_kernel(const __grid_constant__ SoftBwdArgs a) {
   __shared__ __align__(128) TileSmem sm;
   const Scene& s = a.s;
@@ -1845,10 +1685,7 @@ __global__ void __launch_bounds__(kThreads) dibr_tile_soft_bwd_kernel(const __gr
     __syncthreads();  // previous tile's shared state fully consumed
     load_bin_table(s, c, sm);
     __syncthreads();
-    SoftIO io;
-    io.out_soft = nullptr; io.kl = SoftFwdOut{nullptr, nullptr, nullptr};
-    io.grad_soft = a.grad_soft; io.soft = a.soft; io.grad_xy = a.grad_xy;
-    soft_tile<true, false>(s, c, sm, c.in_img && a.idx[c.pix] < 0, a.sigmainv, a.K, false, io);
+    soft_tile_bwd(a, c, sm, c.in_img && a.idx[c.pix] < 0);
   }
 }
 
@@ -2413,7 +2250,10 @@ int bins_per_view(int H, int W) {
 //   cnt [2*B*NB] int + pool_ctr + fb_ctr + band_ctr | off [2*B*NB] int | fb_list, band_list [tiles] int |
 //   entries [2*4*NF] int4 | acc [NF][<=20] f32 (rasterize backward) | pool_hdr [pool_tiles] int4 |
 //   pool_data [pool_tiles][3][256*K] u32
-struct Layout { size_t cnt, off, mode, ent, acc, base; };
+struct Layout {
+  size_t cnt, off, mode, ent, acc, base;
+  size_t acc_at() const { return cnt + off + mode + ent; }   // offset of the face records
+};
 
 Layout layout_for(int B, int64_t NF, int H, int W) {
   Layout L;
@@ -2427,6 +2267,14 @@ Layout layout_for(int B, int64_t NF, int H, int W) {
   return L;
 }
 
+// The 256-byte aligned start of the layout's pieces in workspace `ws`, or nullptr when they do not fit.
+char* layout_origin(const Layout& Lo, void* ws, size_t ws_bytes) {
+  if (!ws) return nullptr;
+  char* p = (char*)align_up((size_t)ws, 256);
+  if (ws_bytes < Lo.base || p + Lo.acc_at() + Lo.acc > (char*)ws + ws_bytes) return nullptr;
+  return p;
+}
+
 size_t pool_block_bytes(int K) {
   return sizeof(int4) + (size_t)3 * 256 * (size_t)K * sizeof(uint32_t);
 }
@@ -2438,15 +2286,18 @@ int check_dims(int B, int64_t NF, int H, int W) {
   return 0;
 }
 
-// knum > 0 enables the hit cache in whatever the workspace holds beyond the minimum.
+// knum > 0 enables the hit cache in whatever the workspace holds beyond the minimum.  The face
+// inputs (xy, z, first, validity, given bboxes) are left empty for the caller to fill in.
 int setup_scene(Scene& s, int B, int64_t NF, int F, int H, int W, float multiplier, float margin,
                 int knum, void* ws, size_t ws_bytes) {
   if (!(multiplier > 0.f)) return DIBR_B200_EINVAL;
   if (!ws) return DIBR_B200_EINVAL;
   const Layout Lo = layout_for(B, NF, H, W);
-  char* p = (char*)align_up((size_t)ws, 256);
+  char* p = layout_origin(Lo, ws, ws_bytes);
   char* const end = (char*)ws + ws_bytes;
-  if (ws_bytes < Lo.base || p + Lo.cnt + Lo.off + Lo.mode + Lo.ent + Lo.acc > end) return DIBR_B200_EWORKSPACE;
+  if (!p) return DIBR_B200_EWORKSPACE;
+  s.first = nullptr; s.xy = nullptr; s.z = nullptr; s.premultiplied = 0;
+  s.fnz = nullptr; s.valid = nullptr; s.bbox_tight = nullptr; s.bbox_large = nullptr;
   s.B = B; s.H = H; s.W = W; s.F = F; s.NF = NF;
   s.multiplier = multiplier; s.margin = margin;
   s.grid = make_grid(multiplier, W, H);
@@ -2473,7 +2324,7 @@ int setup_scene(Scene& s, int B, int64_t NF, int F, int H, int W, float multipli
   s.band_list = (int*)(p + align_up((size_t)s.ntx[0] * s.nty[0] * B * sizeof(int), 256));
   p += Lo.mode;
   s.entries = (int4*)p; p += Lo.ent;
-  p += Lo.acc;
+  p += Lo.acc;   // face records of the rasterize backward (acc_region)
   s.pool_tiles = 0; s.pool_K = knum > 0 ? knum : 1; s.pool_hdr = nullptr; s.pool_data = nullptr;
   if (knum > 0) {
     const size_t left = (size_t)(end - p);
@@ -2521,40 +2372,45 @@ int build_bins(const Scene& s, int sets, cudaStream_t st) {
 
 dim3 tile_grid(const Scene& s) { return dim3((unsigned)s.ntx[0], (unsigned)s.nty[0], (unsigned)s.B); }
 
-// Persistent kernels: one resident wave (SMs x CTAs that fit per SM), never more than the tiles.
-// The wave size is a property of (device, kernel): queried once and cached in a per-instantiation
-// table (idempotent writes of the same value, safe from any thread) - the occupancy / attribute
+// CTAs of `kernel` resident on the current device at `threads` threads and `dyn_smem` bytes of
+// dynamic shared memory (SMs x CTAs per SM; `per_sm_guess` per SM if the query fails), for the
+// persistent kernels.  A property of (device, kernel): queried once and cached in a table
+// (idempotent writes of the same value, safe from any thread) - the occupancy / attribute
 // queries add host time to every call when repeated.
 struct WaveEntry { const void* kernel; int dev; int wave; };
-constexpr int kWaveSlots = 64;
-WaveEntry g_waves[kWaveSlots];   // append-only; a lost race re-queries and stores the same value again
+constexpr int kWaveSlots = 256;   // 12 persistent instantiations per device
+WaveEntry g_waves[kWaveSlots];    // append-only; a lost race re-queries and stores the same value again
 
 template <typename Kernel>
-unsigned persistent_grid(const Scene& s, Kernel kernel, size_t dyn_smem = 0) {
+int resident_ctas(Kernel kernel, int threads, int per_sm_guess, size_t dyn_smem = 0) {
   int dev = 0;
   cudaGetDevice(&dev);
   const void* key = reinterpret_cast<const void*>(kernel);   // kernels with one signature share this template
-  int wave = 0;
   for (int i = 0; i < kWaveSlots && g_waves[i].kernel; ++i)
-    if (g_waves[i].kernel == key && g_waves[i].dev == dev) { wave = g_waves[i].wave; break; }
-  if (wave == 0) {
-    int sms = 132, per_sm = 2;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (dyn_smem > 48 * 1024)
-      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, dyn_smem) != cudaSuccess ||
-        per_sm < 1)
-      per_sm = 2;
-    wave = sms * per_sm;
-    for (int i = 0; i < kWaveSlots; ++i)
-      if (!g_waves[i].kernel) { g_waves[i].dev = dev; g_waves[i].wave = wave; g_waves[i].kernel = key; break; }
-  }
+    if (g_waves[i].kernel == key && g_waves[i].dev == dev) return g_waves[i].wave;
+  int sms = 132, per_sm = per_sm_guess;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (dyn_smem > 48 * 1024)
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem);
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, dyn_smem) != cudaSuccess || per_sm < 1)
+    per_sm = per_sm_guess;
+  const int wave = sms * per_sm;
+  for (int i = 0; i < kWaveSlots; ++i)
+    if (!g_waves[i].kernel) { g_waves[i].dev = dev; g_waves[i].wave = wave; g_waves[i].kernel = key; break; }
+  return wave;
+}
+
+// Persistent tile kernels: one resident wave, never more than the tiles.
+template <typename Kernel>
+unsigned persistent_grid(const Scene& s, Kernel kernel, size_t dyn_smem = 0) {
+  const int wave = resident_ctas(kernel, kThreads, 2, dyn_smem);
   const int64_t ntiles = (int64_t)s.ntx[0] * s.nty[0] * s.B;
   return (unsigned)(ntiles < wave ? ntiles : wave);
 }
 
 template <bool R, bool S, bool K, typename FT = float>
 void launch_fwd(const FwdArgs& a0, cudaStream_t st) {
+  static_assert(!(R && K), "the K-lists come from the soft-mask-only forward");
   FwdArgs a = a0;
   a.from_fb = 0;
   {
@@ -2568,7 +2424,7 @@ void launch_fwd(const FwdArgs& a0, cudaStream_t st) {
     if (two) {
       Span sp("dibr_fwd2_kernel<S=2>", st);
       const dim3 grid((unsigned)((a.s.ntx[0] + 1) / 2), (unsigned)((a.s.nty[0] + 1) / 2), (unsigned)a.s.B);
-      dibr_fwd2_kernel<R, S, K, FT><<<grid, kThreads, 0, st>>>(a);
+      if constexpr (R) dibr_fwd2_kernel<S, FT><<<grid, kThreads, 0, st>>>(a);
     } else {
       // one 16x16 tile per CTA: dense meshes (hundreds of candidates per tile) and small images
       Span sp("dibr_tile_fwd_kernel", st);
@@ -2610,11 +2466,9 @@ int launch_raster_bwd(const RasterBwdArgs& a, cudaStream_t st) {
 
 // The face-record region of a workspace (nullptr: none / too small -> warp-reduction kernel).
 float* acc_region(void* ws, size_t ws_bytes, int B, int64_t NF, int H, int W) {
-  if (!ws) return nullptr;
   const Layout Lo = layout_for(B, NF, H, W);
-  char* p = (char*)align_up((size_t)ws, 256);
-  if (ws_bytes < Lo.base || p + Lo.cnt + Lo.off + Lo.mode + Lo.ent + Lo.acc > (char*)ws + ws_bytes) return nullptr;
-  return (float*)(p + Lo.cnt + Lo.off + Lo.mode + Lo.ent);
+  char* p = layout_origin(Lo, ws, ws_bytes);
+  return p ? (float*)(p + Lo.acc_at()) : nullptr;
 }
 
 template <int DT, typename FT>
@@ -2625,20 +2479,7 @@ int launch_rows_t(const RowBwdArgs& a0, int64_t NF, float* g_xy, float* g_ff, in
   if (e != cudaSuccess) return (int)e;
   {
     Span sp("raster_bwd_rows_kernel", st);
-    // resident single-warp CTAs per device: a property of (device, kernel), cached after the first
-    // query (idempotent writes of the same value: safe from any thread)
-    static int slots_of[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    int slots = slots_of[dev & 63];
-    if (slots == 0) {
-      int sms = 132, per_sm = 16;
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, raster_bwd_rows_kernel<DT, FT>, 32, 0) != cudaSuccess || per_sm < 1)
-        per_sm = 16;
-      slots = sms * per_sm;
-      slots_of[dev & 63] = slots;
-    }
+    const int slots = resident_ctas(raster_bwd_rows_kernel<DT, FT>, 32, DIBR_ROWS_MINB);
     const int64_t jobs = (int64_t)a.jobs_x * a.jobs_y * a.B;
     raster_bwd_rows_kernel<DT, FT><<<(unsigned)(jobs < slots ? jobs : slots), 32, 0, st>>>(a);
   }
@@ -2820,8 +2661,7 @@ static int forward_impl(int batch, int num_faces, int height, int width, int fea
   rc = setup_scene(s, batch, NF, num_faces, height, width, multiplier, boxlen_m, soft ? knum : 0,
                    workspace, workspace_bytes_);
   if (rc) return rc;
-  s.first = nullptr; s.xy = face_vertices_image; s.z = face_vertices_z; s.premultiplied = 0;
-  s.fnz = face_normals_z; s.valid = valid_faces; s.bbox_tight = nullptr; s.bbox_large = nullptr;
+  s.xy = face_vertices_image; s.z = face_vertices_z; s.fnz = face_normals_z; s.valid = valid_faces;
   rc = build_bins(s, (raster ? 1 : 0) | (soft ? 2 : 0), st);
   if (rc) return rc;
   a.rc = make_raster_const(eps);
@@ -2925,8 +2765,7 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
                      workspace_bytes_);
     if (rc) return rc;
     Scene& s = a.s;
-    s.first = nullptr; s.xy = face_vertices_image; s.z = nullptr; s.premultiplied = 0;
-    s.fnz = nullptr; s.valid = nullptr; s.bbox_tight = nullptr; s.bbox_large = nullptr;
+    s.xy = face_vertices_image;
     a.sigmainv = sigmainv; a.K = knum; a.grad_soft = grad_soft_mask; a.soft = soft_mask;
     a.idx = face_idx; a.grad_xy = grad_face_vertices_image;
     a.view_begin = view_begin; a.view_end = view_end;
@@ -3013,7 +2852,7 @@ int dibr_b200_packed_rasterize_forward(int batch, int64_t total_faces, int heigh
   rc = setup_scene(s, batch, total_faces, 0, height, width, multiplier, 0.f, 0, workspace, workspace_bytes_);
   if (rc) return rc;
   s.first = first_idx_face_per_mesh; s.xy = face_vertices_image; s.z = face_vertices_z;
-  s.premultiplied = 1; s.fnz = nullptr; s.valid = nullptr; s.bbox_tight = face_bboxes; s.bbox_large = nullptr;
+  s.premultiplied = 1; s.bbox_tight = face_bboxes;
   rc = build_bins(s, 1, st);
   if (rc) return rc;
   a.rc = make_raster_const(eps);
@@ -3060,8 +2899,7 @@ int dibr_b200_soft_mask_forward(int batch, int num_faces, int height, int width,
   Scene& s = a.s;
   rc = setup_scene(s, batch, NF, num_faces, height, width, multiplier, 0.f, 0, workspace, workspace_bytes_);
   if (rc) return rc;
-  s.first = nullptr; s.xy = face_vertices_image; s.z = nullptr; s.premultiplied = 1;
-  s.fnz = nullptr; s.valid = nullptr; s.bbox_tight = nullptr; s.bbox_large = face_large_bboxes;
+  s.xy = face_vertices_image; s.premultiplied = 1; s.bbox_large = face_large_bboxes;
   rc = build_bins(s, 2, st);
   if (rc) return rc;
   a.rc = make_raster_const(0.f);

@@ -93,7 +93,7 @@ template <bool BWD>
 __global__ void __launch_bounds__(kThreads) dibr_f64_kernel(const __grid_constant__ F64Args a) {
   __shared__ __align__(128) TileSmem sm;
   const Scene& s = a.s;
-  const TileCtx c = make_tile_ctx(s);
+  const TileCtx c = make_tile_ctx(s, blockIdx.z, blockIdx.x, blockIdx.y);   // grid = (tiles_x, tiles_y, views)
   load_bin_table(s, c, sm);
   __syncthreads();
   const double x0 = (double)c.x0, y0 = (double)c.y0;     // computed in float, widened (rasterization_cuda.cu:85-86)
@@ -217,8 +217,7 @@ int f64_setup(F64Args& a, int B, int F, int H, int W, const double* fvi, const d
   float* bl = (float*)(p + L.base + L.xyf + L.bt);
   uint8_t* vb = (uint8_t*)(p + L.base + L.xyf + L.bt + L.bl);
   Scene& s = a.s;
-  s.first = nullptr; s.xy = xyf; s.z = nullptr; s.premultiplied = 1; s.fnz = nullptr; s.valid = vb;
-  s.bbox_tight = bt; s.bbox_large = bl;
+  s.xy = xyf; s.premultiplied = 1; s.valid = vb; s.bbox_tight = bt; s.bbox_large = bl;
   if (rebuild) {
     if (NF > 0)
       f64_prep_kernel<<<(unsigned)((NF + 255) / 256), 256, 0, st>>>(NF, fvi, fnz, valid, multiplier, margin, xyf, bt, bl, vb);

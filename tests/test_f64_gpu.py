@@ -40,10 +40,14 @@ def _scene(views, level, seed, feat_dim=3):
 
 @pytest.mark.parametrize("views,level,H,W,feat_dim", [(2, 3, 96, 128, 3), (1, 2, 64, 64, 1), (3, 4, 160, 120, 5)])
 def test_dibr_rasterization_double_matches_reference_double(views, level, H, W, feat_dim):
+    from kaolin_b200 import _lib
     from kaolin_b200.render.mesh import dibr_rasterization
     fvz, fvi, fnz, ff = _scene(views, level, 50 + level, feat_dim)
     t_fvi, t_ff = D(fvi, True), D(ff, True)
+    _lib.trace_begin()
     feat, soft, idx = dibr_rasterization(H, W, D(fvz), t_fvi, t_ff, D(fnz))
+    ran = [name for name, _ in _lib.trace_end()]
+    assert "dibr_f64_kernel<forward>" in ran, ran
     assert feat.dtype == torch.float64 and soft.dtype == torch.float64 and idx.dtype == torch.int64
     gen = torch.Generator(device=DEV); gen.manual_seed(7)
     g_feat = torch.rand((views, H, W, feat_dim), device=DEV, generator=gen, dtype=torch.float64)

@@ -251,10 +251,15 @@ def test_bf16_feature_storage_vs_reference_cuda(D):
     assert rel_vs_reference(r, "grad_fvi", t_fvi.grad) <= GRAD_REL_REF
     assert rel_vs_reference(r, "grad_ff", t_ff.grad.float()) <= 2.0 ** -8                   # bf16 rounding of the result
     # the C ABI returns the fp32 accumulation itself
+    from kaolin_b200 import _lib
+    _lib.trace_begin()
     feat2, idx2, wts2, soft2, ws = _host.forward(3, H, W, t_fvz, t_fvi.detach(), ff16, t_fnz, None, 1000., 1e-8,
                                                  7000., 0.02 * 1000., 30)
     g_fvi, g_ff = _host.backward(H, W, g_feat16, g_soft, idx2, wts2, soft2, t_fvi.detach(), ff16, 1000., 1e-8,
                                  7000., 0.02 * 1000., 30, ws, True)
+    ran = [name for name, _ in _lib.trace_end()]
+    assert all(k in ran for k in ("dibr_tile_fwd_kernel", "soft_fwd_kernel", "soft_tiles_fwd_kernel<leftovers>",
+                                  "soft_bwd_runs_kernel", "dibr_tile_soft_bwd_kernel<leftovers>")), ran
     assert g_ff.dtype == torch.float32 and torch.equal(feat2, feat)
     assert rel_vs_reference(r, "grad_ff", g_ff) <= GRAD_REL_REF
     assert rel_vs_reference(r, "grad_fvi", g_fvi) <= GRAD_REL_REF
@@ -376,8 +381,12 @@ def test_simple_scene_golden(golden_dir, sigmainv, boxlen, multiplier, knum):
     pmin = torch.min(fvi_m, dim=-2)[0]
     pmax = torch.max(fvi_m, dim=-2)[0]
     bb = torch.cat([pmin - boxlen * multiplier, pmax + boxlen * multiplier], dim=-1)
+    from kaolin_b200 import _lib
+    _lib.trace_begin()
     soft, prob, cidx, ctype = b200_C.render.mesh.dibr_soft_mask_forward_cuda(
         fvi_m, bb, face_idx, sigmainv, knum, multiplier)
+    ran = [name for name, _ in _lib.trace_end()]
+    assert "soft_tiles_fwd_kernel" in ran, ran      # the K-lists are written by the single-kernel path
     gt_soft = torch.from_numpy(g[key + "soft_mask"]).to(DEV)
     assert torch.allclose(soft, gt_soft, atol=1e-5, rtol=1e-5)
     assert torch.equal(cidx.cpu(), torch.from_numpy(g[key + "close_face_idx"][..., :knum].astype(np.int64)))
@@ -522,9 +531,15 @@ def test_soft_mask_dense_overflow_path():
     fnz = np.ones((1, F), np.float32)
     ff = synthetic.random_features(1, F, 1, seed=0)
     H = W = 64
+    from kaolin_b200 import _lib
     for knum in (30, 2000):
         t_fvi = T(fvi, True)
+        _lib.trace_begin()
         feat, soft, idx = dibr_rasterization(H, W, T(fvz), t_fvi, T(ff), T(fnz), boxlen=0.1, knum=knum)
+        ran = [name for name, _ in _lib.trace_end()]
+        # knum > 32: the single-kernel soft-mask path; otherwise the fused kernel and its leftovers
+        want = ["soft_tiles_fwd_kernel"] if knum > 32 else ["soft_fwd_kernel", "soft_tiles_fwd_kernel<leftovers>"]
+        assert all(k in ran for k in want), ran
         o_feat, o_soft, o_idx, o_w = oracle.dibr_rasterization(H, W, fvz, fvi, ff, fnz, boxlen=0.1,
                                                               knum=knum, return_weights=True)
         assert np.array_equal(N(idx), o_idx)
