@@ -12,6 +12,9 @@
  *
  * Return value: 0 on success; DIBR_B200_E* (<0) for argument errors detected on
  * the host; a positive cudaError_t if a launch failed (cudaGetLastError()).
+ * The fused entry points (dibr_b200_forward*, dibr_b200_backward*) check every
+ * argument before they enqueue anything: an argument error leaves the outputs
+ * untouched.
  *
  * The four "operator" entry points replace, one for one, the functions the
  * reference registers in kaolin/csrc/bindings.cpp:111-115; the two "fused"

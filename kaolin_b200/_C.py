@@ -45,7 +45,7 @@ def _check_all(func, named, float_dtype=torch.float32):
 def _fp64_via_fp32(op):
     """The reference's operators dispatch float and double (AT_DISPATCH_FLOATING_TYPES,
     rasterization_cuda.cu:218/427, dibr_soft_mask_cuda.cu:205/376).  The public API has a real
-    <double> instantiation (render/mesh/dibr.py:DibrRasterizationF64 -> dibr_b200_forward_f64); these
+    <double> instantiation (render/mesh/dibr.py:DibrRasterizationB200 -> dibr_b200_forward_f64); these
     packed operator shims serve double callers by casting: float64 inputs -> float32, the op,
     floating-point outputs -> float64 (fp32 rounding applies)."""
     import functools

@@ -2515,6 +2515,47 @@ int launch_raster_bwd_rows(const RasterBwdArgs& r, float* acc, int accumulate_xy
 
 #include "dibr_f64.cuh"
 
+// The argument checks of the fused forward (dibr_b200_forward, _bf16, _f64).  The float32/bf16
+// forward may leave output_weights NULL (nothing is written there then); the float64 one stores them.
+int check_forward(bool f64, int B, int F, int H, int W, int D, int mode, const void* fvz, const void* fvi,
+                  const void* ff, float multiplier, int knum, const void* out_feat, const int64_t* face_idx,
+                  const void* out_w, const void* soft_mask) {
+  const int rc = check_dims(B, (int64_t)B * F, H, W);
+  if (rc) return rc;
+  const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
+  if ((!raster && !soft) || F < 0 || D < 0 || !face_idx || (f64 && !(multiplier > 0.f))) return DIBR_B200_EINVAL;
+  if (F > 0 && !fvi) return DIBR_B200_EINVAL;
+  if (raster && ((f64 && !out_w) || (D > 0 && (!out_feat || (F > 0 && !ff))) || (F > 0 && !fvz)))
+    return DIBR_B200_EINVAL;
+  if (soft && (!soft_mask || knum <= 0)) return DIBR_B200_EINVAL;
+  return 0;
+}
+
+// The argument checks of the fused backward (dibr_b200_backward, _bf16, _views, _f64), all of them
+// made before anything is enqueued: a call that fails them writes no output.  On success `s` holds
+// the scene of the branches that need one (float32/bf16: the soft-mask branch; float64: either).
+int check_backward(bool f64, int B, int F, int H, int W, int D, const void* grad_features,
+                   const void* grad_soft_mask, const int64_t* face_idx, const void* output_weights,
+                   const void* soft_mask, const void* fvi, const void* ff, float multiplier, float boxlen_m,
+                   int knum, const void* g_fvi, const void* g_ff, void* ws, size_t ws_bytes, int view_begin,
+                   int view_end, Scene& s) {
+  const int64_t NF = (int64_t)B * F;
+  const int rc = check_dims(B, NF, H, W);
+  if (rc) return rc;
+  if (!face_idx || !g_fvi || F < 0 || D < 0 || (f64 && !(multiplier > 0.f))) return DIBR_B200_EINVAL;
+  if (F > 0 && !fvi) return DIBR_B200_EINVAL;
+  if (view_begin < 0 || view_end > B || view_begin >= view_end) return DIBR_B200_EINVAL;
+  const bool raster = grad_features && D > 0;
+  const bool soft_ok = !grad_soft_mask || (soft_mask && knum > 0);
+  if (f64 && !soft_ok) return DIBR_B200_EINVAL;     // the float64 backward refuses it even without faces
+  if (NF == 0) return 0;                            // no faces: the gradients are only zeroed
+  // without stored weights the float32/bf16 rasterize branch recomputes them with the multiplier
+  if (raster && (!ff || !g_ff || !(output_weights || (!f64 && multiplier > 0.f)))) return DIBR_B200_EINVAL;
+  if (!soft_ok) return DIBR_B200_EINVAL;
+  if (f64) return raster || grad_soft_mask ? f64_scene(s, B, F, H, W, multiplier, ws, ws_bytes) : 0;
+  return grad_soft_mask ? setup_scene(s, B, NF, F, H, W, multiplier, boxlen_m, knum, ws, ws_bytes) : 0;
+}
+
 }  // namespace
 
 // ===========================================================================
@@ -2531,20 +2572,15 @@ int dibr_b200_forward_f64(int batch, int num_faces, int height, int width, int f
                           float multiplier, float eps, int mode, float sigmainv, double boxlen_m, int knum,
                           double* interpolated_features, int64_t* face_idx, double* output_weights,
                           double* soft_mask, void* workspace, size_t workspace_bytes_, dibr_b200_stream_t stream) {
-  const int64_t NF = (int64_t)batch * num_faces;
-  int rc = check_dims(batch, NF, height, width);
+  int rc = check_forward(true, batch, num_faces, height, width, feat_dim, mode, face_vertices_z, face_vertices_image,
+                         face_features, multiplier, knum, interpolated_features, face_idx, output_weights, soft_mask);
   if (rc) return rc;
   const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
-  if ((!raster && !soft) || num_faces < 0 || feat_dim < 0 || !face_idx || !(multiplier > 0.f)) return DIBR_B200_EINVAL;
-  if (num_faces > 0 && !face_vertices_image) return DIBR_B200_EINVAL;
-  if (raster && (!output_weights || (feat_dim > 0 && (!interpolated_features || (num_faces > 0 && !face_features))) ||
-                 (num_faces > 0 && !face_vertices_z)))
-    return DIBR_B200_EINVAL;
-  if (soft && (!soft_mask || knum <= 0)) return DIBR_B200_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   F64Args a;
-  rc = f64_setup(a, batch, num_faces, height, width, face_vertices_image, face_normals_z, valid_faces, multiplier,
-                 boxlen_m, (raster ? 1 : 0) | (soft ? 2 : 0), true, workspace, workspace_bytes_, st);
+  rc = f64_scene(a.s, batch, num_faces, height, width, multiplier, workspace, workspace_bytes_);
+  if (rc) return rc;
+  rc = f64_bins(a.s, face_vertices_image, face_normals_z, valid_faces, boxlen_m, (raster ? 1 : 0) | (soft ? 2 : 0), st);
   if (rc) return rc;
   a.D = feat_dim; a.K = knum; a.mode = mode; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier;
   a.margin = boxlen_m; a.xy = face_vertices_image; a.z = face_vertices_z; a.feat = face_features;
@@ -2562,13 +2598,12 @@ int dibr_b200_backward_f64(int batch, int num_faces, int height, int width, int 
                            int knum, double* grad_face_vertices_image, double* grad_face_features, void* workspace,
                            size_t workspace_bytes_, int flags, dibr_b200_stream_t stream) {
   const int64_t NF = (int64_t)batch * num_faces;
-  int rc = check_dims(batch, NF, height, width);
+  F64Args a;
+  int rc = check_backward(true, batch, num_faces, height, width, feat_dim, grad_features, grad_soft_mask, face_idx,
+                          output_weights, soft_mask, face_vertices_image, face_features, multiplier, 0.f, knum,
+                          grad_face_vertices_image, grad_face_features, workspace, workspace_bytes_, 0, batch, a.s);
   if (rc) return rc;
-  if (!face_idx || !grad_face_vertices_image || num_faces < 0 || feat_dim < 0 || !(multiplier > 0.f)) return DIBR_B200_EINVAL;
-  if (num_faces > 0 && !face_vertices_image) return DIBR_B200_EINVAL;
   const bool run_raster = grad_features && feat_dim > 0;
-  if (run_raster && NF > 0 && (!output_weights || !face_features || !grad_face_features)) return DIBR_B200_EINVAL;
-  if (grad_soft_mask && (!soft_mask || knum <= 0)) return DIBR_B200_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(grad_face_vertices_image, 0, (size_t)NF * 6 * sizeof(double), st);
   if (e != cudaSuccess) return (int)e;
@@ -2577,11 +2612,11 @@ int dibr_b200_backward_f64(int batch, int num_faces, int height, int width, int 
     if (e != cudaSuccess) return (int)e;
   }
   if (NF == 0 || (!run_raster && !grad_soft_mask)) return 0;
-  F64Args a;
   // the soft-mask branch needs the enlarged bins: forward's (BINS_VALID) or rebuilt here
-  rc = f64_setup(a, batch, num_faces, height, width, face_vertices_image, nullptr, nullptr, multiplier, boxlen_m, 2,
-                 grad_soft_mask && !(flags & DIBR_B200_BINS_VALID), workspace, workspace_bytes_, st);
-  if (rc) return rc;
+  if (grad_soft_mask && !(flags & DIBR_B200_BINS_VALID)) {
+    rc = f64_bins(a.s, face_vertices_image, nullptr, nullptr, boxlen_m, 2, st);
+    if (rc) return rc;
+  }
   a.D = feat_dim; a.K = knum; a.mode = 0; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier;
   a.margin = boxlen_m; a.xy = face_vertices_image; a.z = nullptr; a.feat = face_features;
   a.out_feat = nullptr; a.idx = const_cast<int64_t*>(face_idx); a.out_w = const_cast<double*>(output_weights);
@@ -2646,15 +2681,10 @@ static int forward_impl(int batch, int num_faces, int height, int width, int fea
                         int64_t* face_idx, float* output_weights, float* soft_mask, void* workspace,
                         size_t workspace_bytes_, dibr_b200_stream_t stream, bool bf16) {
   const int64_t NF = (int64_t)batch * num_faces;
-  int rc = check_dims(batch, NF, height, width);
+  int rc = check_forward(false, batch, num_faces, height, width, feat_dim, mode, face_vertices_z, face_vertices_image,
+                         face_features, multiplier, knum, interpolated_features, face_idx, output_weights, soft_mask);
   if (rc) return rc;
   const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
-  if ((!raster && !soft) || num_faces < 0 || feat_dim < 0 || !face_idx) return DIBR_B200_EINVAL;
-  if (num_faces > 0 && !face_vertices_image) return DIBR_B200_EINVAL;
-  if (raster && ((feat_dim > 0 && (!interpolated_features || (num_faces > 0 && !face_features))) ||
-                 (num_faces > 0 && !face_vertices_z)))
-    return DIBR_B200_EINVAL;   // output_weights may be NULL: nothing is written there then
-  if (soft && (!soft_mask || knum <= 0)) return DIBR_B200_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   FwdArgs a;
   Scene& s = a.s;
@@ -2712,11 +2742,12 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
                          int view_begin, int view_end) {
   const int64_t NF = (int64_t)batch * num_faces;
   const bool bins_valid = (flags & DIBR_B200_BINS_VALID) != 0;
-  int rc = check_dims(batch, NF, height, width);
+  SoftBwdArgs sa;   // the soft-mask branch's arguments: check_backward sets up its scene
+  int rc = check_backward(false, batch, num_faces, height, width, feat_dim, grad_features, grad_soft_mask, face_idx,
+                          output_weights, soft_mask, face_vertices_image, face_features, multiplier, boxlen_m, knum,
+                          grad_face_vertices_image, grad_face_features, workspace, workspace_bytes_, view_begin,
+                          view_end, sa.s);
   if (rc) return rc;
-  if (!face_idx || !grad_face_vertices_image || num_faces < 0 || feat_dim < 0) return DIBR_B200_EINVAL;
-  if (num_faces > 0 && !face_vertices_image) return DIBR_B200_EINVAL;
-  if (view_begin < 0 || view_end > batch || view_begin >= view_end) return DIBR_B200_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaSuccess;
   const bool run_raster = grad_features && feat_dim > 0;
@@ -2740,8 +2771,6 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
   }
   if (NF == 0) return 0;
   if (run_raster) {
-    if (!face_features || !grad_face_features) return DIBR_B200_EINVAL;
-    if (!output_weights && !(multiplier > 0.f)) return DIBR_B200_EINVAL;
     RasterBwdArgs a;
     const size_t px0 = (size_t)view_begin * height * width;
     a.B = nv; a.H = height; a.W = width; a.F = num_faces; a.D = feat_dim;
@@ -2759,33 +2788,28 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
     if (rc) return rc;
   }
   if (grad_soft_mask) {
-    if (!soft_mask || knum <= 0) return DIBR_B200_EINVAL;
-    SoftBwdArgs a;
-    rc = setup_scene(a.s, batch, NF, num_faces, height, width, multiplier, boxlen_m, knum, workspace,
-                     workspace_bytes_);
-    if (rc) return rc;
-    Scene& s = a.s;
+    Scene& s = sa.s;
     s.xy = face_vertices_image;
-    a.sigmainv = sigmainv; a.K = knum; a.grad_soft = grad_soft_mask; a.soft = soft_mask;
-    a.idx = face_idx; a.grad_xy = grad_face_vertices_image;
-    a.view_begin = view_begin; a.view_end = view_end;
+    sa.sigmainv = sigmainv; sa.K = knum; sa.grad_soft = grad_soft_mask; sa.soft = soft_mask;
+    sa.idx = face_idx; sa.grad_xy = grad_face_vertices_image;
+    sa.view_begin = view_begin; sa.view_end = view_end;
     const unsigned persistent = persistent_grid(s, dibr_tile_soft_bwd_kernel);
     if (!bins_valid) {
       // no forward state: rebuild the large bins and recompute every tile
       rc = build_bins(s, 2, st);
       if (rc) return rc;
-      a.from_list = 0;
+      sa.from_list = 0;
       Span sp("dibr_tile_soft_bwd_kernel<all tiles>", st);
-      dibr_tile_soft_bwd_kernel<<<persistent, kThreads, 0, st>>>(a);
+      dibr_tile_soft_bwd_kernel<<<persistent, kThreads, 0, st>>>(sa);
     } else {
       // forward left the bins, the hit cache and the list of tiles it could not cache
-      a.from_list = 1;
+      sa.from_list = 1;
       if (s.pool_tiles > 0) {
         Span sp("soft_bwd_runs_kernel", st);
-        soft_bwd_runs_kernel<<<(unsigned)s.pool_tiles, kThreads, 0, st>>>(a);
+        soft_bwd_runs_kernel<<<(unsigned)s.pool_tiles, kThreads, 0, st>>>(sa);
       }
       Span sp("dibr_tile_soft_bwd_kernel<leftovers>", st);
-      dibr_tile_soft_bwd_kernel<<<persistent, kThreads, 0, st>>>(a);
+      dibr_tile_soft_bwd_kernel<<<persistent, kThreads, 0, st>>>(sa);
     }
     return (int)cudaGetLastError();
   }

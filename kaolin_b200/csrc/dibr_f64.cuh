@@ -203,26 +203,28 @@ F64Layout f64_layout(int B, int64_t NF, int H, int W) {
   return L;
 }
 
-// Prepares the float scene (conservative bboxes) + bins for a double call.
-int f64_setup(F64Args& a, int B, int F, int H, int W, const double* fvi, const double* fnz, const uint8_t* valid,
-              float multiplier, double margin, int sets, bool rebuild, void* ws, size_t ws_bytes, cudaStream_t st) {
+// Lays out the float scene of a double call (scaled vertices, conservative bboxes, validity) in the
+// workspace.  Host only: nothing is enqueued.
+int f64_scene(Scene& s, int B, int F, int H, int W, float multiplier, void* ws, size_t ws_bytes) {
   const int64_t NF = (int64_t)B * F;
   const F64Layout L = f64_layout(B, NF, H, W);
   char* p = (char*)align_up((size_t)ws, 256);
   if (!ws || ws_bytes < L.total || p + L.total - 256 > (char*)ws + ws_bytes) return DIBR_B200_EWORKSPACE;
-  int rc = setup_scene(a.s, B, NF, F, H, W, multiplier, 0.f, 0, p, L.base);
+  int rc = setup_scene(s, B, NF, F, H, W, multiplier, 0.f, 0, p, L.base);
   if (rc) return rc;
-  float* xyf = (float*)(p + L.base);
-  float* bt = (float*)(p + L.base + L.xyf);
-  float* bl = (float*)(p + L.base + L.xyf + L.bt);
-  uint8_t* vb = (uint8_t*)(p + L.base + L.xyf + L.bt + L.bl);
-  Scene& s = a.s;
-  s.xy = xyf; s.premultiplied = 1; s.valid = vb; s.bbox_tight = bt; s.bbox_large = bl;
-  if (rebuild) {
-    if (NF > 0)
-      f64_prep_kernel<<<(unsigned)((NF + 255) / 256), 256, 0, st>>>(NF, fvi, fnz, valid, multiplier, margin, xyf, bt, bl, vb);
-    rc = build_bins(s, sets, st);     // with no faces: zeroed counters, every pixel takes the empty path
-    if (rc) return rc;
-  }
+  s.xy = (float*)(p + L.base); s.premultiplied = 1;
+  s.bbox_tight = (float*)(p + L.base + L.xyf);
+  s.bbox_large = (float*)(p + L.base + L.xyf + L.bt);
+  s.valid = (uint8_t*)(p + L.base + L.xyf + L.bt + L.bl);
   return 0;
+}
+
+// Fills the float scene laid out by f64_scene from the double inputs and bins it.
+int f64_bins(const Scene& s, const double* fvi, const double* fnz, const uint8_t* valid, double margin, int sets,
+             cudaStream_t st) {
+  if (s.NF > 0)
+    f64_prep_kernel<<<(unsigned)((s.NF + 255) / 256), 256, 0, st>>>(
+        s.NF, fvi, fnz, valid, s.multiplier, margin, const_cast<float*>(s.xy), const_cast<float*>(s.bbox_tight),
+        const_cast<float*>(s.bbox_large), const_cast<uint8_t*>(s.valid));
+  return build_bins(s, sets, st);     // with no faces: zeroed counters, every pixel takes the empty path
 }

@@ -419,12 +419,12 @@ class PeerGradAllGather:
         return full_fvi, full_ff
 
 
-_DIBR_NODES = ("DibrRasterizationB200", "DibrRasterizationF64")     # render/mesh/dibr.py: fp32 / float64 node
+_DIBR_NODE = "DibrRasterizationB200"     # render/mesh/dibr.py: the node of every dtype
 
 
 def _dibr_node(output):
     """The autograd node of the ``dibr_rasterization`` call (fp32 or float64) that produced ``output``."""
-    is_dibr = lambda n: type(n).__name__.startswith(_DIBR_NODES)
+    is_dibr = lambda n: type(n).__name__.startswith(_DIBR_NODE)
     node = getattr(output, "grad_fn", None)
     seen = 0
     while node is not None and not is_dibr(node) and seen < 4:

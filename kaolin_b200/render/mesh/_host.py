@@ -51,6 +51,27 @@ def check_size(func, name, t, shape):
         raise RuntimeError(f"{func}: expected {name} of size {list(shape)}, got {list(t.shape)}")
 
 
+def any_double(*tensors):
+    """Whether a float64 tensor is among the inputs: such calls run the float64 instantiation."""
+    return any(isinstance(t, torch.Tensor) and t.dtype == torch.float64 for t in tensors)
+
+
+def join_features(face_features):
+    """-> (face_features as one tensor, split).  A list/tuple of (..., D_i) feature tensors is
+    concatenated along the last dimension, and ``split(out)`` cuts an output interpolated from it
+    back into a tuple of (..., D_i) views; a single tensor passes through both unchanged."""
+    if not isinstance(face_features, (list, tuple)):
+        return face_features, lambda out: out
+
+    def split(out):
+        outs, cur = [], 0
+        for f in face_features:
+            outs.append(out[..., cur:cur + f.shape[-1]])
+            cur += f.shape[-1]
+        return tuple(outs)
+    return torch.cat(face_features, dim=-1), split
+
+
 # Screen tiles that get a soft-mask hit-cache block (forward scratch of the enumerate / evaluate
 # kernels AND the backward's input).  Every tile when that fits in CACHE_MAX_BYTES - at 256^2 a third
 # of the 16x16 tiles touch the silhouette, at 1024^2 a tenth, and the host cannot know the number
@@ -70,14 +91,16 @@ def cache_tiles_for(batch, height, width, knum):
     return min(tiles, want, max(1, CACHE_MAX_BYTES // (3072 * knum + 16)))
 
 
-_ws_bytes = {}     # (batch, faces, H, W, knum, cache policy) -> bytes: a pure function of the shape
+_ws_bytes = {}     # (batch, faces, H, W, knum, cache policy, f64) -> bytes: a pure function of the shape
 
 
-def workspace(batch, total_faces, height, width, device, knum=0):
-    key = (batch, total_faces, height, width, knum, CACHE_TILE_FRACTION, CACHE_MAX_BYTES)
+def workspace(batch, total_faces, height, width, device, knum=0, f64=False):
+    key = (batch, total_faces, height, width, knum, CACHE_TILE_FRACTION, CACHE_MAX_BYTES, f64)
     n = _ws_bytes.get(key)
     if n is None:
-        if knum > 0:
+        if f64:         # the float64 kernels keep no hit cache
+            n = _lib.lib().dibr_b200_workspace_bytes_f64(batch, total_faces, height, width)
+        elif knum > 0:
             want = cache_tiles_for(batch, height, width, knum)
             n = _lib.lib().dibr_b200_workspace_bytes_cached(batch, total_faces, height, width, knum, want)
         else:
@@ -92,31 +115,36 @@ def workspace(batch, total_faces, height, width, device, knum=0):
 
 def forward(mode, height, width, fvz, fvi, ff, fnz, valid_u8, multiplier, eps,
             sigmainv, boxlen_m, knum, face_idx_in=None):
-    """Calls dibr_b200_forward; returns (feat, face_idx, None, soft, workspace).
+    """Calls dibr_b200_forward, _bf16 or _f64 (from the dtypes of fvi and ff); returns
+    (feat, face_idx, weights, soft, workspace).
 
-    The barycentric weights are not stored (the third slot is always None): the backward
-    recomputes them bit for bit from face_idx, the vertices and the same multiplier and eps."""
+    float32 / bf16: the barycentric weights are not stored (the third slot is None): the backward
+    recomputes them bit for bit from face_idx, the vertices and the same multiplier and eps.
+    float64: they are, as (B,H,W,3) doubles for the backward to read; boxlen_m stays a double."""
     dev = fvi.device
     B, F = fvi.shape[0], fvi.shape[1]
     D = 0 if ff is None else ff.shape[-1]
     raster = bool(mode & _lib.RASTER)
     soft_on = bool(mode & _lib.SOFT_MASK)
+    f64 = fvi.dtype == torch.float64
     bf16 = ff is not None and ff.dtype == torch.bfloat16
-    feat = torch.empty((B, height, width, D), dtype=torch.bfloat16 if bf16 else torch.float32,
+    real = torch.float64 if f64 else torch.float32
+    feat = torch.empty((B, height, width, D), dtype=torch.bfloat16 if bf16 else real,
                        device=dev) if raster else None
+    wts = torch.empty((B, height, width, 3), dtype=real, device=dev) if raster and f64 else None
     idx = torch.empty((B, height, width), dtype=torch.int64, device=dev) if raster else face_idx_in
-    soft = torch.empty((B, height, width), dtype=torch.float32, device=dev) if soft_on else None
+    soft = torch.empty((B, height, width), dtype=real, device=dev) if soft_on else None
     if B == 0:       # an empty view shard (batch < world size): empty images, nothing to launch
-        return feat, idx, None, soft, None
-    ws = workspace(B, B * F, height, width, dev, knum if soft_on else 0)
+        return feat, idx, wts, soft, None
+    ws = workspace(B, B * F, height, width, dev, knum if soft_on else 0, f64)
+    name = "dibr_b200_forward_f64" if f64 else "dibr_b200_forward"
     with torch.cuda.device(dev):
-        fn = _lib.lib().dibr_b200_forward_bf16 if bf16 else _lib.lib().dibr_b200_forward
-        st = fn(
+        st = getattr(_lib.lib(), name + "_bf16" if bf16 else name)(
             B, F, height, width, D, ptr(fvz), ptr(fvi), ptr(ff), ptr(fnz), ptr(valid_u8),
             float(multiplier), float(eps), mode, float(sigmainv), float(boxlen_m), int(knum),
-            ptr(feat), ptr(idx), None, ptr(soft), ptr(ws), ws.numel(), stream_ptr(dev))
-    _lib.check(st, "dibr_b200_forward")
-    return feat, idx, None, soft, ws
+            ptr(feat), ptr(idx), ptr(wts), ptr(soft), ptr(ws), ws.numel(), stream_ptr(dev))
+    _lib.check(st, name)
+    return feat, idx, wts, soft, ws
 
 
 
@@ -134,52 +162,61 @@ def _backward_call(B, F, height, width, D, g_feat, g_soft, face_idx, wts, soft, 
                 stream_ptr(dev))
         _lib.check(st, "dibr_b200_backward_views")
         return
+    name = "dibr_b200_backward_f64" if fvi.dtype == torch.float64 else "dibr_b200_backward"
     with torch.cuda.device(dev):
-        fn = _lib.lib().dibr_b200_backward_bf16 if bf16 else _lib.lib().dibr_b200_backward
-        st = fn(
+        st = getattr(_lib.lib(), name + "_bf16" if bf16 else name)(
             B, F, height, width, D, ptr(g_feat), ptr(g_soft), ptr(face_idx), ptr(wts), ptr(soft),
             ptr(fvi), ptr(ff), float(multiplier), float(eps), float(sigmainv), float(boxlen_m),
             int(knum), ptr(g_fvi), ptr(g_ff), ptr(ws), ws_bytes, int(flags), stream_ptr(dev))
-    _lib.check(st, "dibr_b200_backward")
+    _lib.check(st, name)
 
 
 def backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multiplier, eps,
              sigmainv, boxlen_m, knum, ws, bins_valid, feature_grad_hook=None, views=None, out=None):
-    """Calls dibr_b200_backward; returns (grad_face_vertices_image, grad_face_features fp32).
+    """Calls dibr_b200_backward, _bf16 or _f64 (from the dtypes of fvi and ff); returns
+    (grad_face_vertices_image, grad_face_features in the precision of fvi).
 
-    ``wts`` is None after ``forward`` (the kernels recompute the weights; ``multiplier`` and ``eps``
-    must then be the forward's) or the (B,H,W,3) weights of the same forward, which are read.
+    ``wts`` is None after a float32 / bf16 ``forward`` (the kernels recompute the weights;
+    ``multiplier`` and ``eps`` must then be the forward's) or the (B,H,W,3) weights of the same
+    forward, which are read (always so in float64).
 
     ``views=(v0, v1)`` restricts the call to those views of the batch (dibr_b200_backward_views: all
     tensors stay the full-batch ones, only rows v0..v1-1 of the gradients are written) and ``out=
     (g_fvi, g_ff)`` supplies the full-batch gradient buffers to write into - together they let a
-    caller pipeline view chunks (kaolin_b200.multi_gpu.pipelined_backward_all_gather).
+    caller pipeline view chunks (kaolin_b200.multi_gpu.pipelined_backward_all_gather).  Both serve
+    float32 / bf16 only.
 
     ``feature_grad_hook`` (per call — there is no process-global state): called as
     ``hook(g_ff)`` between the two branches of a fused backward.  grad_face_features is
     final after the rasterize branch, so e.g. its all-gather can travel while the
-    soft-mask branch runs (kaolin_b200.multi_gpu.OverlappedGradAllGather)."""
+    soft-mask branch runs (kaolin_b200.multi_gpu.OverlappedGradAllGather).  The float64
+    backward is one kernel: it calls the hook once, at the end."""
     dev = fvi.device
     B, F = fvi.shape[0], fvi.shape[1]
     D = 0 if ff is None else ff.shape[-1]
+    f64 = fvi.dtype == torch.float64
+    if f64 and (views is not None or out is not None):
+        raise ValueError("kaolin_b200: views= and out= serve the float32 / bfloat16 backward only")
+    # grad_face_features is accumulated (atomics) in the precision of the vertices whatever the
+    # storage type of the features: fp32 for fp32 / bf16
     if B * F == 0 and out is None:       # empty mesh: empty gradients, nothing to launch
-        return torch.zeros_like(fvi), (torch.zeros(ff.shape, dtype=torch.float32, device=dev) if ff is not None else None)
+        return torch.zeros_like(fvi), (torch.zeros(ff.shape, dtype=fvi.dtype, device=dev) if ff is not None else None)
     if out is not None:
         g_fvi, g_ff = out
     else:
         g_fvi = torch.empty_like(fvi)
-        # grad_face_features is accumulated (atomics) in fp32 whatever the storage type
-        g_ff = torch.empty(ff.shape, dtype=torch.float32, device=dev) if ff is not None else None
+        g_ff = torch.empty(ff.shape, dtype=fvi.dtype, device=dev) if ff is not None else None
     # The workspace carries forward's bins / hit cache (soft-mask branch, bins_valid) and the
     # per-face records of the row-walk rasterize backward; without forward state a fresh
     # minimum-size one serves both.
     if ws is None:
-        ws = workspace(B, B * F, height, width, dev)
+        ws = workspace(B, B * F, height, width, dev, f64=f64)
         bins_valid = False
     ws_bytes = ws.numel()
     flags = _lib.BINS_VALID if bins_valid else 0
     hook = feature_grad_hook
-    if hook is not None and g_feat is not None and g_soft is not None and D > 0:
+    both = hook is not None and g_feat is not None and g_soft is not None
+    if both and D > 0 and not f64:
         # two calls: rasterize branch (g_ff final -> hook), then the soft-mask branch added on top
         _backward_call(B, F, height, width, D, g_feat, None, face_idx, wts, None, fvi, ff, multiplier, eps,
                        sigmainv, boxlen_m, knum, g_fvi, g_ff, ws, ws_bytes, 0, dev, views)
@@ -189,55 +226,6 @@ def backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multip
     else:
         _backward_call(B, F, height, width, D, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multiplier, eps,
                        sigmainv, boxlen_m, knum, g_fvi, g_ff, ws, ws_bytes, flags, dev, views)
-    return g_fvi, g_ff
-
-
-# ---------------------------------------------------------------------------
-# float64 instantiation (dibr_b200_forward_f64 / dibr_b200_backward_f64)
-def forward_f64(mode, height, width, fvz, fvi, ff, fnz, valid_u8, multiplier, eps, sigmainv, boxlen_m, knum,
-                face_idx_in=None):
-    """-> (feat f64, face_idx, weights f64, soft f64, workspace); boxlen_m is a Python float (double)."""
-    dev = fvi.device
-    B, F = fvi.shape[0], fvi.shape[1]
-    D = 0 if ff is None else ff.shape[-1]
-    raster = bool(mode & _lib.RASTER)
-    soft_on = bool(mode & _lib.SOFT_MASK)
-    f64 = torch.float64
-    feat = torch.empty((B, height, width, D), dtype=f64, device=dev) if raster else None
-    wts = torch.empty((B, height, width, 3), dtype=f64, device=dev) if raster else None
-    idx = torch.empty((B, height, width), dtype=torch.int64, device=dev) if raster else face_idx_in
-    soft = torch.empty((B, height, width), dtype=f64, device=dev) if soft_on else None
-    if B == 0:
-        return feat, idx, wts, soft, None
-    n = _lib.lib().dibr_b200_workspace_bytes_f64(B, B * F, height, width)
-    if n == 0:
-        raise RuntimeError("kaolin_b200: unsupported problem size")
-    ws = torch.empty(n, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_forward_f64(
-            B, F, height, width, D, ptr(fvz), ptr(fvi), ptr(ff), ptr(fnz), ptr(valid_u8), float(multiplier),
-            float(eps), mode, float(sigmainv), float(boxlen_m), int(knum), ptr(feat), ptr(idx), ptr(wts), ptr(soft),
-            ptr(ws), ws.numel(), stream_ptr(dev))
-    _lib.check(st, "dibr_b200_forward_f64")
-    return feat, idx, wts, soft, ws
-
-
-def backward_f64(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multiplier, eps, sigmainv, boxlen_m,
-                 knum, ws):
-    dev = fvi.device
-    B, F = fvi.shape[0], fvi.shape[1]
-    D = 0 if ff is None else ff.shape[-1]
-    if B * F == 0:
-        return torch.zeros_like(fvi), (torch.zeros_like(ff) if ff is not None else None)
-    g_fvi = torch.empty_like(fvi)
-    g_ff = torch.empty_like(ff) if ff is not None else None
-    flags = _lib.BINS_VALID if ws is not None else 0
-    if ws is None:
-        ws = torch.empty(_lib.lib().dibr_b200_workspace_bytes_f64(B, B * F, height, width), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_backward_f64(
-            B, F, height, width, D, ptr(g_feat), ptr(g_soft), ptr(face_idx), ptr(wts), ptr(soft), ptr(fvi), ptr(ff),
-            float(multiplier), float(eps), float(sigmainv), float(boxlen_m), int(knum), ptr(g_fvi), ptr(g_ff),
-            ptr(ws), ws.numel(), int(flags), stream_ptr(dev))
-    _lib.check(st, "dibr_b200_backward_f64")
+        if both and f64:
+            hook(g_ff)
     return g_fvi, g_ff

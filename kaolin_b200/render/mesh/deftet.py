@@ -11,6 +11,7 @@ import torch
 from torch.autograd import Function
 
 from ... import _C
+from . import _host
 
 __all__ = ["deftet_sparse_render"]
 
@@ -61,13 +62,7 @@ def deftet_sparse_render(pixel_coords, render_ranges, face_vertices_z, face_vert
     Returns:
         (rendered features (B, num_pixels, knum, D) or a tuple of them, face_idx (B, num_pixels, knum), -1 = void)
     """
-    _face_features = torch.cat(face_features, dim=-1) if isinstance(face_features, (list, tuple)) else face_features
+    _face_features, split = _host.join_features(face_features)
     image_features, face_idx = DeftetSparseRendererB200.apply(
         pixel_coords, render_ranges, face_vertices_z, face_vertices_image, _face_features, knum, eps)
-    if isinstance(face_features, (list, tuple)):
-        outs, cur = [], 0
-        for f in face_features:
-            outs.append(image_features[..., cur:cur + f.shape[-1]])
-            cur += f.shape[-1]
-        image_features = tuple(outs)
-    return image_features, face_idx
+    return split(image_features), face_idx

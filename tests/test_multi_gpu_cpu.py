@@ -207,11 +207,6 @@ def test_attach_finds_the_dibr_node_through_a_slice():
     g.hook = lambda t: None
     assert g.attach(out) is g
     assert out.grad_fn.feature_grad_hook is g.hook and not hasattr(other.grad_fn, "feature_grad_hook")
-    class DibrRasterizationF64(DibrRasterizationB200):         # the float64 node is recognised as well
-        pass
-
-    out64 = DibrRasterizationF64.apply(x)
-    assert multi_gpu._dibr_node(out64) is out64.grad_fn
     with pytest.raises(ValueError):
         multi_gpu._dibr_node(x * 3.0)
     with pytest.raises(ValueError):
