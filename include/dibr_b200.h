@@ -450,6 +450,47 @@ int dibr_b200_specular_backward(
     float* grad_light_sharpness, void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
 
 /*
+ * Deferred shading (kaolin/render/easy_render/mesh.py:427-464 sg_shade; kaolin_b200/csrc/lighting.cu):
+ * the diffuse and specular terms above for every pixel of a (B, H, W) G-buffer, in one pass per
+ * pixel.  Per view b (camera, B x 16 floats): R (3x3 row-major, world to camera), tan_x =
+ * (camera width / 2) / focal_x, tan_y likewise, x0, y0, camera width, camera height, one unused float.
+ * Per pixel (i, j): face_idx (B,H,W) int64; albedo, spec_albedo, normals (B,H,W,3); roughness (B,H,W).
+ *   face_idx < 0 (background): diffuse = specular = img = 0, every per-pixel gradient 0, and the
+ *     pixel adds nothing to the light gradients;
+ *   n = normals / max(|normals|, 1e-12)                                (F.normalize)
+ *   pixel = ((j + 1/2) cw / W - x0, (i + 1/2) ch / H + y0), ndc = 2 pixel / (cw, ch) - 1,
+ *   d = (ndc_x tan_x, -ndc_y tan_y, -1), v = -R^T d / |R^T d|          (kaolin/render/camera/raygen.py,
+ *     the custom-resolution pixel grid; fp32, in the reference's order of operations)
+ *   diffuse  = dibr_b200_diffuse_forward(SG_INNER_PRODUCT) of (n, albedo)
+ *   specular = dibr_b200_specular_forward of (n, roughness, v, spec_albedo)
+ *   img      = diffuse + specular                                       all (B,H,W,3) float32
+ * Every output element is written.  The backward takes any subset of grad_diffuse, grad_specular and
+ * grad_img (NULL counts as zero); the diffuse term sees grad_diffuse + grad_img and the specular term
+ * grad_specular + grad_img.  It writes any subset of grad_albedo, grad_spec_albedo, grad_roughness,
+ * grad_normals (through the normalisation) and the light gradients; a NULL gradient is not
+ * computed, and with only light gradients requested nothing is written per pixel.  The camera gets
+ * no gradient.  Light gradients need workspace >= dibr_b200_sg_shade_workspace_bytes(L) = 7.4 KB per
+ * light, independent of the pixel count, and are bit-reproducible.  H or W above 16384 gives
+ * DIBR_B200_ESIZE; negative sizes or a NULL input that is read give DIBR_B200_EINVAL, before any
+ * CUDA call.  Unspecified, where the reference itself gives inf or NaN: a covered pixel of roughness 0,
+ * or whose unit normal is exactly perpendicular to its view (w + v = 0).
+ */
+size_t dibr_b200_sg_shade_workspace_bytes(int num_lights);
+int dibr_b200_sg_shade_forward(
+    int batch, int height, int width, int num_lights, const float* camera, const int64_t* face_idx,
+    const float* albedo, const float* spec_albedo, const float* roughness, const float* normals,
+    const float* light_amplitude, const float* light_direction, const float* light_sharpness, float* diffuse,
+    float* specular, float* img, dibr_b200_stream_t stream);
+int dibr_b200_sg_shade_backward(
+    int batch, int height, int width, int num_lights, const float* camera, const int64_t* face_idx,
+    const float* albedo, const float* spec_albedo, const float* roughness, const float* normals,
+    const float* light_amplitude, const float* light_direction, const float* light_sharpness,
+    const float* grad_diffuse, const float* grad_specular, const float* grad_img, float* grad_albedo,
+    float* grad_spec_albedo, float* grad_roughness, float* grad_normals, float* grad_light_amplitude,
+    float* grad_light_direction, float* grad_light_sharpness, void* workspace, size_t workspace_bytes,
+    dibr_b200_stream_t stream);
+
+/*
  * Exchange step of the view-sharded path (SURVEY.md 8e; kaolin_b200/csrc/peer_push.cu): the
  * reference has no multi-GPU code - its callers all-gather the per-view gradients with
  * torch.distributed.  All-gather by STORES over NVLink: copies `bytes` (multiple of 16) from the

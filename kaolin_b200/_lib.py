@@ -95,6 +95,10 @@ SIGNATURES = {
     "dibr_b200_specular_forward": (_i, [_i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dibr_b200_specular_backward": (_i, [_i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                          _vp, _vp, _vp, _vp, _sz, _vp]),
+    # deferred shading of a G-buffer: both terms above in one pass per pixel (easy_render sg_shade)
+    "dibr_b200_sg_shade_workspace_bytes": (_sz, [_i]),
+    "dibr_b200_sg_shade_forward": (_i, [_i, _i, _i, _i] + [_vp] * 12 + [_vp]),
+    "dibr_b200_sg_shade_backward": (_i, [_i, _i, _i, _i] + [_vp] * 19 + [_vp, _sz, _vp]),
 }
 
 

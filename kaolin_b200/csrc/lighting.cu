@@ -41,15 +41,20 @@ constexpr int kBwdCtas = kSms * 2;          // 2 resident CTAs per SM (__launch_
 constexpr float kPi = 3.14159265358979323846f;
 constexpr float kTwoPi = 6.28318530717958647692f;
 
-enum Kind { GENERAL = 0, LOBE = 1, FITTED = 2, SH9 = 3, SPECULAR = 4 };
+enum Kind { GENERAL = 0, LOBE = 1, FITTED = 2, SH9 = 3, SPECULAR = 4, SHADE = 5 };
 
 template <int K> struct Cfg {
-  // per-point floats in registers (SPECULAR: the warped lobe a, w, ws, then V(ndl) V(ndv), (1-ldh)^5, ndl)
-  static constexpr int kIn = K == GENERAL ? 7 : K == SPECULAR ? 8 : 3;
-  static constexpr int kRec = (K == GENERAL || K == LOBE || K == SPECULAR) ? 8 : 16;  // floats per staged light
+  // per-point floats in registers (SPECULAR: the warped lobe a, w, ws, then V(ndl) V(ndv), (1-ldh)^5, ndl;
+  // SHADE: unit normal, roughness, view, and SPECULAR's 8 besides)
+  static constexpr int kIn = K == GENERAL ? 7 : K == SPECULAR ? 8 : K == SHADE ? 7 : 3;
+  static constexpr int kRec = (K == GENERAL || K == LOBE || K == SPECULAR || K == SHADE) ? 8 : 16;  // floats per staged light
   static constexpr int kAcc = K == SH9 ? 9 : 7;                      // per-light gradient partials
-  // resident forward CTAs per SM: the SPECULAR prologue needs more than 64 registers
-  static constexpr int kFwdBlocks = K == SPECULAR ? 3 : 4;
+  // resident forward CTAs per SM: the SPECULAR prologue needs more than 64 registers, and SHADE holds
+  // both lobes' state (normal, warped lobe and epilogue factors, two sums) for each of its points
+  static constexpr int kFwdBlocks = K == SPECULAR ? 3 : K == SHADE ? 2 : 4;
+  // points per thread: kPts, except in SHADE's backward, whose per-point state (both lobes' sums,
+  // their gradients and the normal's) does not fit 128 registers at 4 points
+  static constexpr int pts(bool bwd) { return bwd && K == SHADE ? 2 : kPts; }
 };
 
 struct Args {
@@ -73,13 +78,14 @@ struct Args {
 };                                  // SPECULAR: albedo = spec_albedo, g_albedo = grad_spec_albedo
 
 // ---------------------------------------------------------------------------------------------
-// 4-point row loads / stores: three (C = 3) or one (C = 1) 16-byte accesses when aligned.
-template <int C>
-__device__ __forceinline__ void load_rows(const float* __restrict__ base, int64_t p0, int64_t n, float (&v)[kPts][C]) {
+// P-point row loads / stores (P = kPts except in SHADE's backward): P C / 4 16-byte accesses when
+// aligned and P C is a multiple of 4, scalar accesses otherwise.
+template <int C, int P>
+__device__ __forceinline__ void load_rows(const float* __restrict__ base, int64_t p0, int64_t n, float (&v)[P][C]) {
   const float* src = base + p0 * C;
-  if (p0 + kPts <= n && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
+  if ((P * C) % 4 == 0 && p0 + P <= n && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
 #pragma unroll
-    for (int q = 0; q < C; ++q) {
+    for (int q = 0; q < P * C / 4; ++q) {
       const float4 t = __ldg(reinterpret_cast<const float4*>(src) + q);
       v[(4 * q) / C][(4 * q) % C] = t.x;
       v[(4 * q + 1) / C][(4 * q + 1) % C] = t.y;
@@ -88,23 +94,23 @@ __device__ __forceinline__ void load_rows(const float* __restrict__ base, int64_
     }
   } else {
 #pragma unroll
-    for (int p = 0; p < kPts; ++p)
+    for (int p = 0; p < P; ++p)
 #pragma unroll
       for (int c = 0; c < C; ++c) v[p][c] = (p0 + p < n) ? __ldg(src + p * C + c) : 0.f;
   }
 }
 
-template <int C>
-__device__ __forceinline__ void store_rows(float* __restrict__ base, int64_t p0, int64_t n, const float (&v)[kPts][C]) {
+template <int C, int P>
+__device__ __forceinline__ void store_rows(float* __restrict__ base, int64_t p0, int64_t n, const float (&v)[P][C]) {
   float* dst = base + p0 * C;
-  if (p0 + kPts <= n && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+  if ((P * C) % 4 == 0 && p0 + P <= n && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
 #pragma unroll
-    for (int q = 0; q < C; ++q)
+    for (int q = 0; q < P * C / 4; ++q)
       reinterpret_cast<float4*>(dst)[q] = make_float4(v[(4 * q) / C][(4 * q) % C], v[(4 * q + 1) / C][(4 * q + 1) % C],
                                                       v[(4 * q + 2) / C][(4 * q + 2) % C], v[(4 * q + 3) / C][(4 * q + 3) % C]);
   } else {
 #pragma unroll
-    for (int p = 0; p < kPts; ++p)
+    for (int p = 0; p < P; ++p)
       if (p0 + p < n)
 #pragma unroll
         for (int c = 0; c < C; ++c) dst[p * C + c] = v[p][c];
@@ -704,6 +710,299 @@ int launch_bwd(const Args& a, cudaStream_t st) {
 
 size_t partial_bytes(int slots, int lights) { return (size_t)kBwdCtas * (size_t)lights * (size_t)slots * sizeof(float); }
 
+// ---------------------------------------------------------------------------------------------
+// SHADE (sg_shade of kaolin/render/easy_render/mesh.py): deferred shading of a (B, H, W) G-buffer, one
+// point per pixel.  A background pixel (face_idx < 0) gives exactly 0 and takes no part in the light
+// gradients; a covered one normalises its normal as F.normalize does, generates its view ray, and
+// evaluates the LOBE (diffuse) and SPECULAR pairs against each staged light, so each light is staged
+// and read once for both terms.  Both lobes' light partials go into the same 7-float slot: the
+// finalize step is linear in them.  A warp whose 32 pixels are all background skips the light loop.
+constexpr int kCam = 16;   // floats per view: R (row-major), tan_x, tan_y, x0, y0, camera width, height, 0
+
+struct ShadeArgs {
+  Args a;                  // a.n = B H W pixels; the lights, their gradients and the partial slots
+  int H, W;
+  const int64_t* face_idx;
+  const float* cam;
+  const float* normal; const float* albedo; const float* spec_albedo; const float* rough;
+  float* diffuse; float* specular; float* img;
+  const float* g_diffuse; const float* g_specular; const float* g_img;
+  float* g_normal; float* g_albedo; float* g_spec_albedo; float* g_rough;
+};
+
+// Which of a thread's P pixels are covered; whether any of its warp's are.
+template <int P>
+__device__ __forceinline__ bool shade_mask(const ShadeArgs& s, int64_t p0, bool (&cov)[P]) {
+  bool any = false;
+#pragma unroll
+  for (int q = 0; q < P; ++q) {
+    cov[q] = p0 + q < s.a.n && __ldg(s.face_idx + p0 + q) >= 0;
+    any |= cov[q];
+  }
+  return __any_sync(0xffffffffu, any);
+}
+
+// The view of pixel (i, j): -normalize(R^T d), d the pinhole ray of kaolin/render/camera/raygen.py
+// through the pixel centre of the custom-resolution grid (scale = camera size / G-buffer size), in the
+// reference's fp32 operations and their order.
+__device__ __forceinline__ void shade_view(const float* __restrict__ cam, int H, int W, int i, int j, float* v) {
+  const float cw = __ldg(cam + 13), ch = __ldg(cam + 14);
+  const float sx = __fdiv_rn(cw, (float)W), sy = __fdiv_rn(ch, (float)H);
+  const float px = __fsub_rn(__fadd_rn(__fmul_rn(sx, (float)j), __fmul_rn(sx, 0.5f)), __ldg(cam + 11));
+  const float py = __fadd_rn(__fadd_rn(__fmul_rn(sy, (float)i), __fmul_rn(sy, 0.5f)), __ldg(cam + 12));
+  const float d0 = __fmul_rn(__fsub_rn(__fmul_rn(2.f, __fdiv_rn(px, cw)), 1.f), __ldg(cam + 9));
+  const float d1 = __fmul_rn(-__fsub_rn(__fmul_rn(2.f, __fdiv_rn(py, ch)), 1.f), __ldg(cam + 10));
+  float w[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) w[k] = __ldg(cam + k) * d0 + __ldg(cam + 3 + k) * d1 - __ldg(cam + 6 + k);
+  const float len = sqrtf(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) v[k] = -(w[k] / len);
+}
+
+// Per pixel: x7 = (unit normal, roughness, view), the raw layout of spec_geom; dn = max(|normal|, 1e-12).
+template <int P>
+__device__ __forceinline__ void shade_points(const ShadeArgs& s, int64_t p0, float (&x7)[P][7], float (&dn)[P]) {
+  float x[P][3], r[P][1];
+  load_rows<3>(s.normal, p0, s.a.n, x);
+  load_rows<1>(s.rough, p0, s.a.n, r);
+  const int64_t hw = (int64_t)s.H * s.W;
+  int64_t b = p0 / hw;
+  const int rem = (int)(p0 - b * hw);
+  int i = rem / s.W, j = rem - i * s.W;
+#pragma unroll
+  for (int q = 0; q < P; ++q) {
+    const float len = sqrtf(x[q][0] * x[q][0] + x[q][1] * x[q][1] + x[q][2] * x[q][2]);
+    dn[q] = len < 1e-12f ? 1e-12f : len;       // clamp_min: NaN stays NaN
+#pragma unroll
+    for (int k = 0; k < 3; ++k) x7[q][k] = x[q][k] / dn[q];
+    x7[q][3] = r[q][0];
+    if (p0 + q < s.a.n) shade_view(s.cam + kCam * b, s.H, s.W, i, j, x7[q] + 4);
+    else x7[q][4] = x7[q][5] = x7[q][6] = 0.f;
+    if (++j == s.W) { j = 0; if (++i == s.H) { i = 0; ++b; } }
+  }
+}
+
+// SPECULAR's per-point record (load_points<SPECULAR>) from x7.
+__device__ __forceinline__ void shade_spec_in(const float* x7, float* in) {
+  const Spec g = spec_geom(x7);
+  in[0] = g.a; in[1] = g.w[0]; in[2] = g.w[1]; in[3] = g.w[2]; in[4] = g.ws;
+  in[5] = g.V1 * g.V2; in[6] = g.p5; in[7] = g.ndl;
+}
+
+template <int P>
+__device__ __forceinline__ void shade_pairs_fwd(const float* s_light, int cnt, const float (&x7)[P][7],
+                                                const float (&sp)[P][8], float (&accd)[P][3], float (&accs)[P][3]) {
+  constexpr int R = Cfg<SHADE>::kRec;
+  for (int m = 0; m < cnt; ++m) {
+    float r[R];
+#pragma unroll
+    for (int q = 0; q < R / 4; ++q) *reinterpret_cast<float4*>(r + 4 * q) = reinterpret_cast<const float4*>(s_light + m * R)[q];
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      pair_fwd<LOBE>(x7[p], r, accd[p]);
+      pair_fwd<SPECULAR>(sp[p], r, accs[p]);
+    }
+  }
+}
+
+template <int P>
+__global__ void __launch_bounds__(kThreads, Cfg<SHADE>::kFwdBlocks) shade_fwd_kernel(ShadeArgs s) {
+  constexpr int T = kThreads * P;
+  __shared__ __align__(16) float s_light[kChunk * Cfg<SHADE>::kRec];
+  const Args& a = s.a;
+  const int64_t tiles = (a.n + T - 1) / T;
+  const int nchunks = (a.L + kChunk - 1) / kChunk;
+  if (nchunks == 1) { stage_chunk<SHADE>(a, 0, a.L, s_light); __syncthreads(); }
+  for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int64_t p0 = tile * T + (int64_t)threadIdx.x * P;
+    bool cov[P];
+    const bool active = shade_mask(s, p0, cov);
+    float x7[P][Cfg<SHADE>::kIn] = {}, dn[P], sp[P][8] = {};
+    float accd[P][3] = {}, accs[P][3] = {}, al[P][3] = {}, sa[P][3] = {};
+    if (active) {
+      shade_points(s, p0, x7, dn);
+#pragma unroll
+      for (int p = 0; p < P; ++p) shade_spec_in(x7[p], sp[p]);
+    }
+    for (int c = 0; c < nchunks; ++c) {
+      const int cnt = min(kChunk, a.L - c * kChunk);
+      if (nchunks > 1) { __syncthreads(); stage_chunk<SHADE>(a, c * kChunk, cnt, s_light); __syncthreads(); }
+      if (active) shade_pairs_fwd(s_light, cnt, x7, sp, accd, accs);
+    }
+    if (active) {
+      load_rows<3>(s.albedo, p0, a.n, al);
+      load_rows<3>(s.spec_albedo, p0, a.n, sa);
+    }
+    float od[P][3], os[P][3], oi[P][3];
+#pragma unroll
+    for (int p = 0; p < P; ++p)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const float d = clamp0(accd[p][k]) * (al[p][k] / kPi);
+        const float e = clamp0(((accs[p][k] * sp[p][5]) * (sa[p][k] + (1.f - sa[p][k]) * sp[p][6])) * sp[p][7]);
+        od[p][k] = cov[p] ? d : 0.f;
+        os[p][k] = cov[p] ? e : 0.f;
+        oi[p][k] = cov[p] ? d + e : 0.f;
+      }
+    store_rows<3>(s.diffuse, p0, a.n, od);
+    store_rows<3>(s.specular, p0, a.n, os);
+    store_rows<3>(s.img, p0, a.n, oi);
+  }
+}
+
+// d loss / d diffuse and d loss / d specular of each pixel: each output's gradient plus img's.
+template <int P>
+__device__ __forceinline__ void shade_grads(const ShadeArgs& s, int64_t p0, float (&gd)[P][3], float (&gs)[P][3]) {
+  if (s.g_diffuse) load_rows<3>(s.g_diffuse, p0, s.a.n, gd);
+  if (s.g_specular) load_rows<3>(s.g_specular, p0, s.a.n, gs);
+  if (s.g_img) {
+    float gi[P][3];
+    load_rows<3>(s.g_img, p0, s.a.n, gi);
+#pragma unroll
+    for (int p = 0; p < P; ++p)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { gd[p][k] += gi[p][k]; gs[p][k] += gi[p][k]; }
+  }
+}
+
+template <int P>
+__global__ void __launch_bounds__(kThreads, 2) shade_bwd_kernel(ShadeArgs s) {
+  constexpr int R = Cfg<SHADE>::kRec, A = Cfg<SHADE>::kAcc, T = kThreads * P;
+  __shared__ __align__(16) float s_light[kChunk * R];
+  __shared__ float s_red[kWarps][kChunk][A];
+  const Args& a = s.a;
+  const int64_t tiles = (a.n + T - 1) / T;
+  const int nchunks = (a.L + kChunk - 1) / kChunk;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const bool want_light = a.partial != nullptr;
+  const bool want_point = s.g_normal || s.g_rough;
+  float* part = want_light ? a.partial + (size_t)blockIdx.x * a.L * A : nullptr;
+  if (want_light)
+    for (int i = threadIdx.x; i < a.L * A; i += kThreads) part[i] = 0.f;
+  if (nchunks == 1) { stage_chunk<SHADE>(a, 0, a.L, s_light); }
+  __syncthreads();
+  for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int64_t p0 = tile * T + (int64_t)threadIdx.x * P;
+    bool cov[P];
+    const bool active = shade_mask(s, p0, cov);
+    float x7[P][7] = {}, dn[P] = {}, sp[P][8] = {};
+    float gd[P][3] = {}, gs[P][3] = {}, al[P][3] = {}, sa[P][3] = {};
+    if (active) {
+      shade_points(s, p0, x7, dn);
+#pragma unroll
+      for (int p = 0; p < P; ++p) shade_spec_in(x7[p], sp[p]);
+      shade_grads(s, p0, gd, gs);
+      load_rows<3>(s.albedo, p0, a.n, al);
+      load_rows<3>(s.spec_albedo, p0, a.n, sa);
+    }
+    // phase 1: both lobes' sums, for the clamp masks and the epilogues
+    float pred[P][3] = {}, pres[P][3] = {};
+    for (int c = 0; c < nchunks; ++c) {
+      const int cnt = min(kChunk, a.L - c * kChunk);
+      if (nchunks > 1) { __syncthreads(); stage_chunk<SHADE>(a, c * kChunk, cnt, s_light); __syncthreads(); }
+      if (active) shade_pairs_fwd(s_light, cnt, x7, sp, pred, pres);
+    }
+    // epilogue backward: the LOBE epilogue of the diffuse term, spec_epilogue_bwd of the specular one
+    float gpd[P][3], gps[P][3], ga[P][3], gsa[P][3], eg[P][4] = {};
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      if (cov[p]) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          gpd[p][k] = pred[p][k] >= 0.f ? gd[p][k] * (al[p][k] / kPi) : 0.f;
+          ga[p][k] = gd[p][k] * clamp0(pred[p][k]) / kPi;
+        }
+        spec_epilogue_bwd(spec_geom(x7[p]), pres[p], gs[p], sa[p], gps[p], gsa[p], eg[p]);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gpd[p][k] = gps[p][k] = ga[p][k] = gsa[p][k] = 0.f;
+      }
+    }
+    if (s.g_albedo) store_rows<3>(s.g_albedo, p0, a.n, ga);
+    if (s.g_spec_albedo) store_rows<3>(s.g_spec_albedo, p0, a.n, gsa);
+    // phase 2: light partials of both lobes into one slot, and the per-pixel gradients
+    float pgd[P][3] = {}, pgs[P][5] = {};
+    if (want_light || want_point) {
+      for (int c = 0; c < nchunks; ++c) {
+        const int cnt = min(kChunk, a.L - c * kChunk);
+        if (nchunks > 1) { __syncthreads(); stage_chunk<SHADE>(a, c * kChunk, cnt, s_light); __syncthreads(); }
+        for (int m = 0; m < cnt; ++m) {
+          float la[A] = {};
+          if (active) {
+            float r[R];
+#pragma unroll
+            for (int q = 0; q < R / 4; ++q) *reinterpret_cast<float4*>(r + 4 * q) = reinterpret_cast<const float4*>(s_light + m * R)[q];
+#pragma unroll
+            for (int p = 0; p < P; ++p)
+              if (cov[p]) {
+                pair_bwd<LOBE>(x7[p], gpd[p], r, la, pgd[p], want_point);
+                pair_bwd<SPECULAR>(sp[p], gps[p], r, la, pgs[p], want_point);
+              }
+            if (want_light) {
+#pragma unroll
+              for (int j = 0; j < A; ++j) {
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) la[j] += __shfl_xor_sync(0xffffffffu, la[j], o);
+              }
+            }
+          }
+          if (want_light && lane == 0)
+#pragma unroll
+            for (int j = 0; j < A; ++j) s_red[warp][m][j] = la[j];
+        }
+        if (want_light) {
+          __syncthreads();
+          for (int i = threadIdx.x; i < cnt * A; i += kThreads) {
+            const int m = i / A, j = i - m * A;
+            float sum = 0.f;
+#pragma unroll
+            for (int w = 0; w < kWarps; ++w) sum += s_red[w][m][j];
+            part[(size_t)(c * kChunk + m) * A + j] += sum;
+          }
+          __syncthreads();
+        }
+      }
+    }
+    if (want_point) {
+      float on[P][3] = {}, orr[P][1] = {};
+#pragma unroll
+      for (int p = 0; p < P; ++p) {
+        if (!cov[p]) continue;
+        float gn[3], gv[3];
+        spec_point_bwd(x7[p], spec_geom(x7[p]), pgs[p], eg[p], gn, orr[p][0], gv);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gn[k] += 2.133f * pgd[p][k];
+        // n = x / max(|x|, eps): (g - n (n.g)) / |x| where |x| >= eps, g / eps below
+        const float* n = x7[p];
+        const float ng = dn[p] > 1e-12f ? n[0] * gn[0] + n[1] * gn[1] + n[2] * gn[2] : 0.f;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) on[p][k] = (gn[k] - n[k] * ng) / dn[p];
+      }
+      if (s.g_normal) store_rows<3>(s.g_normal, p0, a.n, on);
+      if (s.g_rough) store_rows<1>(s.g_rough, p0, a.n, orr);
+    }
+  }
+}
+
+int launch_shade_fwd(const ShadeArgs& s, cudaStream_t st) {
+  constexpr int P = Cfg<SHADE>::pts(false);
+  const int64_t tiles = (s.a.n + kThreads * P - 1) / (kThreads * P);
+  if (tiles == 0) return 0;
+  const int64_t ctas = (int64_t)kSms * Cfg<SHADE>::kFwdBlocks;
+  shade_fwd_kernel<P><<<(unsigned)(tiles < ctas ? tiles : ctas), kThreads, 0, st>>>(s);
+  return (int)cudaGetLastError();
+}
+
+int launch_shade_bwd(const ShadeArgs& s, cudaStream_t st) {
+  constexpr int P = Cfg<SHADE>::pts(true);
+  const int64_t tiles = (s.a.n + kThreads * P - 1) / (kThreads * P);
+  const int ctas = (int)(tiles < kBwdCtas ? tiles : kBwdCtas);
+  if (ctas > 0) shade_bwd_kernel<P><<<ctas, kThreads, 0, st>>>(s);
+  if (s.a.partial && s.a.L > 0) lighting_finalize_kernel<SHADE><<<(s.a.L + 127) / 128, 128, 0, st>>>(s.a, ctas);
+  return (int)cudaGetLastError();
+}
+
 }  // namespace
 
 extern "C" {
@@ -902,6 +1201,68 @@ int dibr_b200_specular_backward(int64_t num_points, int num_lights, const float*
     return 0;
   }
   return launch_bwd<SPECULAR>(a, st);
+}
+
+size_t dibr_b200_sg_shade_workspace_bytes(int num_lights) {
+  return num_lights < 0 ? 0 : partial_bytes(Cfg<SHADE>::kAcc, num_lights);
+}
+
+static int shade_args(ShadeArgs& s, int batch, int height, int width, int num_lights, const float* camera,
+                      const int64_t* face_idx, const float* albedo, const float* spec_albedo, const float* roughness,
+                      const float* normals, const float* light_amplitude, const float* light_direction,
+                      const float* light_sharpness) {
+  if (batch < 0 || height < 0 || width < 0 || num_lights < 0) return DIBR_B200_EINVAL;
+  if (height > 16384 || width > 16384) return DIBR_B200_ESIZE;
+  if (num_lights > 0 && (!light_amplitude || !light_direction || !light_sharpness)) return DIBR_B200_EINVAL;
+  const int64_t n = (int64_t)batch * height * width;
+  if (n > 0 && (!camera || !face_idx || !albedo || !spec_albedo || !roughness || !normals)) return DIBR_B200_EINVAL;
+  s = ShadeArgs{};
+  s.a.n = n; s.a.L = num_lights;
+  s.a.l_amp = light_amplitude; s.a.l_dir = light_direction; s.a.l_sharp = light_sharpness;
+  s.H = height; s.W = width;
+  s.face_idx = face_idx; s.cam = camera;
+  s.normal = normals; s.albedo = albedo; s.spec_albedo = spec_albedo; s.rough = roughness;
+  return 0;
+}
+
+int dibr_b200_sg_shade_forward(int batch, int height, int width, int num_lights, const float* camera,
+                               const int64_t* face_idx, const float* albedo, const float* spec_albedo,
+                               const float* roughness, const float* normals, const float* light_amplitude,
+                               const float* light_direction, const float* light_sharpness, float* diffuse,
+                               float* specular, float* img, dibr_b200_stream_t stream) {
+  ShadeArgs s;
+  const int rc = shade_args(s, batch, height, width, num_lights, camera, face_idx, albedo, spec_albedo, roughness,
+                            normals, light_amplitude, light_direction, light_sharpness);
+  if (rc) return rc;
+  if (s.a.n > 0 && (!diffuse || !specular || !img)) return DIBR_B200_EINVAL;
+  s.diffuse = diffuse; s.specular = specular; s.img = img;
+  return launch_shade_fwd(s, (cudaStream_t)stream);
+}
+
+int dibr_b200_sg_shade_backward(int batch, int height, int width, int num_lights, const float* camera,
+                                const int64_t* face_idx, const float* albedo, const float* spec_albedo,
+                                const float* roughness, const float* normals, const float* light_amplitude,
+                                const float* light_direction, const float* light_sharpness,
+                                const float* grad_diffuse, const float* grad_specular, const float* grad_img,
+                                float* grad_albedo, float* grad_spec_albedo, float* grad_roughness,
+                                float* grad_normals, float* grad_light_amplitude, float* grad_light_direction,
+                                float* grad_light_sharpness, void* workspace, size_t workspace_bytes,
+                                dibr_b200_stream_t stream) {
+  ShadeArgs s;
+  const int rc = shade_args(s, batch, height, width, num_lights, camera, face_idx, albedo, spec_albedo, roughness,
+                            normals, light_amplitude, light_direction, light_sharpness);
+  if (rc) return rc;
+  s.g_diffuse = grad_diffuse; s.g_specular = grad_specular; s.g_img = grad_img;
+  s.g_albedo = grad_albedo; s.g_spec_albedo = grad_spec_albedo; s.g_rough = grad_roughness; s.g_normal = grad_normals;
+  s.a.gl_amp = grad_light_amplitude; s.a.gl_dir = grad_light_direction; s.a.gl_sharp = grad_light_sharpness;
+  const bool want_light = num_lights > 0 && (s.a.gl_amp || s.a.gl_dir || s.a.gl_sharp);
+  if (want_light) {
+    if (!workspace) return DIBR_B200_EINVAL;
+    if (workspace_bytes < dibr_b200_sg_shade_workspace_bytes(num_lights)) return DIBR_B200_EWORKSPACE;
+    s.a.partial = (float*)workspace;
+  }
+  if (!want_light && !grad_albedo && !grad_spec_albedo && !grad_roughness && !grad_normals) return 0;
+  return launch_shade_bwd(s, (cudaStream_t)stream);
 }
 
 }  // extern "C"

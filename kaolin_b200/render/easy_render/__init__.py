@@ -1,3 +1,4 @@
-from .mesh import mesh_rasterize_interpolate_cuda  # noqa: F401
+from .mesh import (RenderPass, render_mesh, mesh_rasterize_interpolate_cuda,  # noqa: F401
+                   texture_sample_materials, sg_shade)
 
-__all__ = ["mesh_rasterize_interpolate_cuda"]
+__all__ = ["RenderPass", "render_mesh", "mesh_rasterize_interpolate_cuda", "texture_sample_materials", "sg_shade"]
