@@ -16,6 +16,13 @@
  * argument before they enqueue anything: an argument error leaves the outputs
  * untouched.
  *
+ * Alignment: every non-NULL tensor pointer passed to dibr_b200_forward, _bf16,
+ * _f64, dibr_b200_backward, _bf16, _views, _f64 (and so dibr_b200_rasterize_backward,
+ * which calls dibr_b200_backward) must be 16-byte aligned; otherwise the call
+ * returns DIBR_B200_EINVAL.  The kernels make 16-byte vector accesses on them.
+ * A fresh allocation is aligned; a contiguous view at an element offset may not be
+ * (the Python layer copies such inputs).  The workspace needs no alignment.
+ *
  * The four "operator" entry points replace, one for one, the functions the
  * reference registers in kaolin/csrc/bindings.cpp:111-115; the two "fused"
  * entry points implement the same mathematics directly on the public-API

@@ -128,6 +128,10 @@ def rasterize_backward_cuda(grad_interpolated_features, interpolated_features, s
     _check_size(fn, "face_features", face_features, (B, F, 3, D))
     g_xy = torch.empty_like(face_vertices_image)
     g_ff = torch.empty_like(face_features)
+    # dibr_b200_rasterize_backward shares the fused backward's 16-byte pointer alignment requirement
+    from .render.mesh._host import aligned
+    (grad_interpolated_features, selected_face_idx, output_weights, face_vertices_image, face_features) = map(
+        aligned, (grad_interpolated_features, selected_face_idx, output_weights, face_vertices_image, face_features))
     with torch.cuda.device(dev):
         st = _lib.lib().dibr_b200_rasterize_backward(
             B, F, H, W, D, _ptr(grad_interpolated_features), _ptr(selected_face_idx),

@@ -32,6 +32,7 @@
 // recomputed (dibr_tile_soft_bwd_kernel).
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <initializer_list>
 #include <type_traits>
 #include <vector>
 #include <string>
@@ -2515,13 +2516,23 @@ int launch_raster_bwd_rows(const RasterBwdArgs& r, float* acc, int accumulate_xy
 
 #include "dibr_f64.cuh"
 
+// Whether every non-null tensor pointer starts on a 16-byte boundary.  The kernels read and write
+// the caller's tensors with float2 / float4 / int4 accesses and 16-byte cp.async copies at offsets
+// that are multiples of the vector size from the tensor's start, so only the start is checked.
+bool aligned16(std::initializer_list<const void*> ptrs) {
+  for (const void* p : ptrs)
+    if (reinterpret_cast<uintptr_t>(p) & 15) return false;
+  return true;
+}
+
 // The argument checks of the fused forward (dibr_b200_forward, _bf16, _f64).  The float32/bf16
 // forward may leave output_weights NULL (nothing is written there then); the float64 one stores them.
 int check_forward(bool f64, int B, int F, int H, int W, int D, int mode, const void* fvz, const void* fvi,
-                  const void* ff, float multiplier, int knum, const void* out_feat, const int64_t* face_idx,
-                  const void* out_w, const void* soft_mask) {
+                  const void* ff, const void* fnz, const void* valid, float multiplier, int knum,
+                  const void* out_feat, const int64_t* face_idx, const void* out_w, const void* soft_mask) {
   const int rc = check_dims(B, (int64_t)B * F, H, W);
   if (rc) return rc;
+  if (!aligned16({fvz, fvi, ff, fnz, valid, out_feat, face_idx, out_w, soft_mask})) return DIBR_B200_EINVAL;
   const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
   if ((!raster && !soft) || F < 0 || D < 0 || !face_idx || (f64 && !(multiplier > 0.f))) return DIBR_B200_EINVAL;
   if (F > 0 && !fvi) return DIBR_B200_EINVAL;
@@ -2542,6 +2553,8 @@ int check_backward(bool f64, int B, int F, int H, int W, int D, const void* grad
   const int64_t NF = (int64_t)B * F;
   const int rc = check_dims(B, NF, H, W);
   if (rc) return rc;
+  if (!aligned16({grad_features, grad_soft_mask, face_idx, output_weights, soft_mask, fvi, ff, g_fvi, g_ff}))
+    return DIBR_B200_EINVAL;
   if (!face_idx || !g_fvi || F < 0 || D < 0 || (f64 && !(multiplier > 0.f))) return DIBR_B200_EINVAL;
   if (F > 0 && !fvi) return DIBR_B200_EINVAL;
   if (view_begin < 0 || view_end > B || view_begin >= view_end) return DIBR_B200_EINVAL;
@@ -2573,7 +2586,8 @@ int dibr_b200_forward_f64(int batch, int num_faces, int height, int width, int f
                           double* interpolated_features, int64_t* face_idx, double* output_weights,
                           double* soft_mask, void* workspace, size_t workspace_bytes_, dibr_b200_stream_t stream) {
   int rc = check_forward(true, batch, num_faces, height, width, feat_dim, mode, face_vertices_z, face_vertices_image,
-                         face_features, multiplier, knum, interpolated_features, face_idx, output_weights, soft_mask);
+                         face_features, face_normals_z, valid_faces, multiplier, knum, interpolated_features, face_idx,
+                         output_weights, soft_mask);
   if (rc) return rc;
   const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
   cudaStream_t st = (cudaStream_t)stream;
@@ -2682,7 +2696,8 @@ static int forward_impl(int batch, int num_faces, int height, int width, int fea
                         size_t workspace_bytes_, dibr_b200_stream_t stream, bool bf16) {
   const int64_t NF = (int64_t)batch * num_faces;
   int rc = check_forward(false, batch, num_faces, height, width, feat_dim, mode, face_vertices_z, face_vertices_image,
-                         face_features, multiplier, knum, interpolated_features, face_idx, output_weights, soft_mask);
+                         face_features, face_normals_z, valid_faces, multiplier, knum, interpolated_features, face_idx,
+                         output_weights, soft_mask);
   if (rc) return rc;
   const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
   cudaStream_t st = (cudaStream_t)stream;

@@ -16,6 +16,13 @@ def stream_ptr(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def aligned(t):
+    """``t``, or a fresh copy of it if its data does not start on a 16-byte boundary.  The fused
+    entry points reject such pointers (their kernels make 16-byte vector accesses); a contiguous
+    view at an element offset, e.g. ``buf[1:].view(B, F, 3, 2)``, is still legal input."""
+    return t if t is None or t.data_ptr() % 16 == 0 else t.clone()
+
+
 FEATURE_DTYPES = (torch.float32, torch.bfloat16)   # storage of face_features / interpolated features
 
 
@@ -116,7 +123,8 @@ def workspace(batch, total_faces, height, width, device, knum=0, f64=False):
 def forward(mode, height, width, fvz, fvi, ff, fnz, valid_u8, multiplier, eps,
             sigmainv, boxlen_m, knum, face_idx_in=None):
     """Calls dibr_b200_forward, _bf16 or _f64 (from the dtypes of fvi and ff); returns
-    (feat, face_idx, weights, soft, workspace).
+    (feat, face_idx, weights, soft, workspace).  Inputs that do not start on a 16-byte boundary are
+    copied first (``aligned``).
 
     float32 / bf16: the barycentric weights are not stored (the third slot is None): the backward
     recomputes them bit for bit from face_idx, the vertices and the same multiplier and eps.
@@ -124,6 +132,7 @@ def forward(mode, height, width, fvz, fvi, ff, fnz, valid_u8, multiplier, eps,
     dev = fvi.device
     B, F = fvi.shape[0], fvi.shape[1]
     D = 0 if ff is None else ff.shape[-1]
+    fvz, fvi, ff, fnz, valid_u8, face_idx_in = map(aligned, (fvz, fvi, ff, fnz, valid_u8, face_idx_in))
     raster = bool(mode & _lib.RASTER)
     soft_on = bool(mode & _lib.SOFT_MASK)
     f64 = fvi.dtype == torch.float64
@@ -184,7 +193,8 @@ def backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multip
     tensors stay the full-batch ones, only rows v0..v1-1 of the gradients are written) and ``out=
     (g_fvi, g_ff)`` supplies the full-batch gradient buffers to write into - together they let a
     caller pipeline view chunks (kaolin_b200.multi_gpu.pipelined_backward_all_gather).  Both serve
-    float32 / bf16 only.
+    float32 / bf16 only.  Inputs that do not start on a 16-byte boundary are copied first
+    (``aligned``); an ``out=`` buffer that does not raises ValueError.
 
     ``feature_grad_hook`` (per call — there is no process-global state): called as
     ``hook(g_ff)`` between the two branches of a fused backward.  grad_face_features is
@@ -197,6 +207,9 @@ def backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multip
     f64 = fvi.dtype == torch.float64
     if f64 and (views is not None or out is not None):
         raise ValueError("kaolin_b200: views= and out= serve the float32 / bfloat16 backward only")
+    if out is not None and any(t is not None and t.data_ptr() % 16 for t in out):
+        raise ValueError("kaolin_b200: the out= gradient buffers must start on a 16-byte boundary")
+    g_feat, g_soft, face_idx, wts, soft, fvi, ff = map(aligned, (g_feat, g_soft, face_idx, wts, soft, fvi, ff))
     # grad_face_features is accumulated (atomics) in the precision of the vertices whatever the
     # storage type of the features: fp32 for fp32 / bf16
     if B * F == 0 and out is None:       # empty mesh: empty gradients, nothing to launch

@@ -74,6 +74,39 @@ def test_workspace_query_and_host_side_errors():
     assert lib.dibr_b200_peer_push_multicast(ctypes.c_void_p(4096), 32, ctypes.c_void_p(4104), 0, 0, None) == _lib.EINVAL
 
 
+def test_misaligned_pointers_are_rejected_on_the_host():
+    """The fused entry points require 16-byte aligned tensor pointers and say so before any CUDA
+    call: fake device addresses that are all aligned but one give EINVAL without a GPU."""
+    lib = _lib.lib()
+    B, F, H, W, D = 1, 4, 8, 8, 3
+    ok, off = ctypes.c_void_p(1 << 20), ctypes.c_void_p((1 << 20) + 4)    # off: one fp32 element in
+
+    def forward(entry, **bad):
+        p = dict(fvz=ok, fvi=ok, ff=ok, fnz=ok, valid=None, feat=ok, idx=ok, w=None, soft=ok)
+        p.update(bad)
+        return getattr(lib, entry)(B, F, H, W, D, p["fvz"], p["fvi"], p["ff"], p["fnz"], p["valid"], 1000.0, 1e-8,
+                                   3, 7000.0, 20.0, 30, p["feat"], p["idx"], p["w"], p["soft"], ok, 1 << 20, None)
+
+    def backward(entry, **bad):
+        p = dict(g=ok, gs=ok, idx=ok, w=ok, soft=ok, fvi=ok, ff=ok, gfvi=ok, gff=ok)
+        p.update(bad)
+        return getattr(lib, entry)(B, F, H, W, D, p["g"], p["gs"], p["idx"], p["w"], p["soft"], p["fvi"], p["ff"],
+                                   1000.0, 1e-8, 7000.0, 20.0, 30, p["gfvi"], p["gff"], ok, 1 << 20, 0, None)
+
+    for entry in ("dibr_b200_forward", "dibr_b200_forward_bf16"):
+        for name in ("fvz", "fvi", "ff", "fnz", "valid", "feat", "idx", "w", "soft"):
+            assert forward(entry, **{name: off}) == _lib.EINVAL, (entry, name)
+    assert forward("dibr_b200_forward_f64", w=ok, fvi=off) == _lib.EINVAL
+    for entry in ("dibr_b200_backward", "dibr_b200_backward_bf16", "dibr_b200_backward_f64"):
+        for name in ("g", "gs", "idx", "w", "soft", "fvi", "ff", "gfvi", "gff"):
+            assert backward(entry, **{name: off}) == _lib.EINVAL, (entry, name)
+    st = lib.dibr_b200_backward_views(B, F, H, W, D, off, ok, ok, None, ok, ok, ok, 0, 1000.0, 1e-8, 7000.0, 20.0,
+                                      30, ok, ok, ok, 1 << 20, 0, 0, 1, None)
+    assert st == _lib.EINVAL
+    st = lib.dibr_b200_rasterize_backward(B, F, H, W, D, off, ok, ok, ok, ok, 1e-8, ok, ok, None)
+    assert st == _lib.EINVAL
+
+
 def test_python_signatures_match_reference():
     """rasterization.py:373-381, dibr.py:75-76,119-122."""
     sig = inspect.signature(rasterize)

@@ -1,7 +1,8 @@
 """Argument errors are reported before any work is enqueued.
 
 The fused backward entry points (dibr_b200_backward, _bf16, _views, _f64) get correctly sized device
-buffers with one argument wrong at a time; the gradient outputs hold a NaN sentinel.  A rejected call
+buffers with one argument wrong at a time (including a tensor pointer that is not 16-byte aligned); the gradient outputs
+hold a NaN sentinel.  A rejected call
 returns its error code, launches no kernel (the per-kernel trace is empty) and leaves the outputs as
 they were (checked after a synchronise, so a memset would show too).  The same buffers with every
 argument right run the backward and overwrite the sentinel.
@@ -90,6 +91,7 @@ REJECTED = [  # (id, the one wrong argument, expected status)
     ("face_features_null", dict(ff=None), _lib.EINVAL),
     ("grad_face_features_null", dict(g_ff=None), _lib.EINVAL),
     ("multiplier_zero", dict(mult=0.), _lib.EINVAL),
+    ("grad_features_misaligned", dict(g_feat="offset"), _lib.EINVAL),
 ]
 
 
@@ -101,6 +103,12 @@ def test_rejected_backward_enqueues_nothing(entry, case):
     outputs = (a["g_fvi"], a["g_ff"])
     if wrong.get("ws") == "short":      # a real allocation one byte smaller than the minimum
         wrong = dict(ws=torch.empty(a["ws"].numel() - 1, dtype=torch.uint8, device=DEV))
+    if wrong.get("g_feat") == "offset":  # the same values one element into a valid buffer
+        g = a["g_feat"]
+        buf = torch.empty(g.numel() + 1, dtype=g.dtype, device=DEV)
+        buf[1:].copy_(g.reshape(-1))
+        wrong = dict(g_feat=buf[1:].view(g.shape))
+        assert wrong["g_feat"].data_ptr() % 16 != 0
     a.update(wrong)
     st, ran = _traced_call(entry, a, outputs)
     assert st == code, st
