@@ -498,6 +498,72 @@ int dibr_b200_sg_shade_backward(
     dibr_b200_stream_t stream);
 
 /*
+ * Mesh topology, uniform Laplacian and vertex averaging (kaolin_b200/csrc/mesh_topology.cu) for one
+ * mesh of V vertices and F faces of S >= 3 vertices, `faces` (F, S) int64.  The reference builds dense
+ * V x V matrices; these entry points work on two CSR structures built once by
+ * dibr_b200_mesh_topology_build, in caller-owned int32 buffers:
+ *   corner_ptr (V+1), corners (F*S)  for vertex i, the corners f*S + k with faces[f, k] == i, in the
+ *                                    order of the key k*F + f (that of the reference's per-corner
+ *                                    scatter_add_ loop, kaolin/ops/mesh/mesh.py:202-204)
+ *   adj_ptr (V+1), adj (2*F*S)       for vertex i, its unique neighbours faces[f, (k +- 1) mod S] in
+ *                                    ascending order (the unique `roll` pairs of mesh.py:100-103); the
+ *                                    first adj_ptr[V] entries are used.  A degenerate face gives a
+ *                                    self-loop i -> i.  Quads give their four cyclic edges.
+ *   degree (V) int32, weight (V) f32 the number of neighbours (self-loop included) and 1.0f / degree
+ *                                    as an IEEE division (0 for degree 0)
+ *   status (2) int32                 {adj_ptr[V], error}: error is non-zero when a face index lies
+ *                                    outside [0, V).  Such a corner is counted and written nowhere;
+ *                                    the topology is then not usable.  (Deliberate deviation: the
+ *                                    reference does not check; on the CPU it drops an index >= V from
+ *                                    its sparse matrix, and a negative index writes out of bounds.)
+ * The build needs V < 2^31 - 1 and 2*F*S < 2^31 (else DIBR_B200_ESIZE) and workspace >=
+ * dibr_b200_mesh_topology_workspace_bytes(); it is deterministic and never needs O(V^2) memory.
+ * Read status to know the edge count; nothing else has to come back to the host.
+ */
+size_t dibr_b200_mesh_topology_workspace_bytes(int num_vertices, int64_t num_faces, int face_size);
+int dibr_b200_mesh_topology_build(int num_vertices, int64_t num_faces, int face_size, const int64_t* faces,
+                                  int32_t* corner_ptr, int32_t* corners, int32_t* adj_ptr, int32_t* adj,
+                                  int32_t* degree, float* weight, int32_t* status, void* workspace,
+                                  size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
+ * uniform_laplacian (kaolin/ops/mesh/mesh.py:116-151) applied without the matrix: L[i, i] = -1,
+ * L[i, j] = weight[i] for the neighbours j != i, 0 elsewhere; x and y (batch, V, channels) f32.
+ *   transpose = 0: y = L x      y_i = weight_i sum_{j in N(i), j != i} x_j - x_i
+ *   transpose = 1: y = L^T x    y_j = sum_{i in N(j), i != j} weight_i x_i - x_j   (the backward)
+ *   smooth = 1:    without the -x term, i.e. (L + I) x: uniform_laplacian_smoothing
+ *                  (kaolin/metrics/trianglemesh.py:318-350)
+ * A gather per output element (no atomics: bit-reproducible), sums in adjacency order, in fp32.
+ */
+int dibr_b200_laplacian_apply(int batch, int num_vertices, int channels, const int32_t* adj_ptr, const int32_t* adj,
+                              const float* weight, const float* x, int transpose, int smooth, float* y,
+                              dibr_b200_stream_t stream);
+
+/*
+ * average_face_vertex_features / compute_vertex_normals (kaolin/ops/mesh/mesh.py:154-208):
+ * face_features (batch, F, S, channels) f32 -> out (batch, V, channels): per vertex the sum over its
+ * corners in key order, divided by max(count, 1).  Backward: grad_face_features[b, f, k, c] =
+ * grad_out[b, faces[f, k], c] / max(count, 1).
+ */
+int dibr_b200_vertex_average_forward(int batch, int num_vertices, int64_t num_faces, int face_size, int channels,
+                                     const int32_t* corner_ptr, const int32_t* corners, const float* face_features,
+                                     float* out, dibr_b200_stream_t stream);
+int dibr_b200_vertex_average_backward(int batch, int num_vertices, int64_t num_faces, int face_size, int channels,
+                                      const int64_t* faces, const int32_t* corner_ptr, const float* grad_out,
+                                      float* grad_face_features, dibr_b200_stream_t stream);
+
+/*
+ * Dense (V, V) f32 from the adjacency CSR, every element written: laplacian = 1 gives
+ * uniform_laplacian (mesh.py:116-151), laplacian = 0 adjacency_matrix(sparse=False) (mesh.py:78-114).
+ * dibr_b200_adjacency_coo writes the (2, num_edges) int64 indices of adjacency_matrix(sparse=True):
+ * rows and columns in CSR (lexicographic) order, which is the order of the reference's unique(dim=0).
+ */
+int dibr_b200_mesh_dense(int num_vertices, int laplacian, const int32_t* adj_ptr, const int32_t* adj,
+                         const float* weight, float* out, dibr_b200_stream_t stream);
+int dibr_b200_adjacency_coo(int num_vertices, int64_t num_edges, const int32_t* adj_ptr, const int32_t* adj,
+                            int64_t* indices, dibr_b200_stream_t stream);
+
+/*
  * Exchange step of the view-sharded path (SURVEY.md 8e; kaolin_b200/csrc/peer_push.cu): the
  * reference has no multi-GPU code - its callers all-gather the per-view gradients with
  * torch.distributed.  All-gather by STORES over NVLink: copies `bytes` (multiple of 16) from the

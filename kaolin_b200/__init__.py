@@ -3,7 +3,12 @@
 Provided: ``kaolin.render.mesh.{rasterize, dibr_soft_mask, dibr_rasterization}``
 (forward + backward), the four ``kaolin._C.render.mesh.*`` operators, and the steps
 either side of the rasterizer in the DIB-R loop (``render.mesh.prepare_vertices``,
-``render.mesh.texture_mapping``, ``metrics.render.mask_iou``); see DESIGN.md for scope.  There is no CPU fallback: every entry point
+``render.mesh.texture_mapping``, ``metrics.render.mask_iou``), lighting and deferred shading
+(``render.lighting``, ``render.easy_render``), and the mesh Laplacian regulariser of the loss
+(``ops.mesh.{adjacency_matrix, uniform_laplacian, average_face_vertex_features,
+compute_vertex_normals}``, ``metrics.trianglemesh.uniform_laplacian_smoothing``, and
+``ops.mesh.UniformLaplacian``, which applies the Laplacian without its V x V matrix); see DESIGN.md
+for scope.  There is no CPU fallback: every entry point
 raises if the CUDA library (kaolin_b200/csrc, built in-tree) is missing or the
 tensors are not on a CUDA device.
 """
@@ -11,4 +16,5 @@ __version__ = "0.1.0"
 
 from . import render   # noqa: E402,F401
 from . import metrics  # noqa: E402,F401
+from . import ops      # noqa: E402,F401
 from . import _C       # noqa: E402,F401

@@ -14,7 +14,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libdibr_b200.so")
 SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline.cu"),
            os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
-           os.path.join(CSRC, "lighting.cu")]
+           os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"),
            os.path.join(_HERE, "..", "include", "dibr_b200.h")]
@@ -99,6 +99,14 @@ SIGNATURES = {
     "dibr_b200_sg_shade_workspace_bytes": (_sz, [_i]),
     "dibr_b200_sg_shade_forward": (_i, [_i, _i, _i, _i] + [_vp] * 12 + [_vp]),
     "dibr_b200_sg_shade_backward": (_i, [_i, _i, _i, _i] + [_vp] * 19 + [_vp, _sz, _vp]),
+    # mesh topology, Laplacian and vertex averaging (ops.mesh, metrics.trianglemesh; csrc/mesh_topology.cu)
+    "dibr_b200_mesh_topology_workspace_bytes": (_sz, [_i, _i64, _i]),
+    "dibr_b200_mesh_topology_build": (_i, [_i, _i64, _i] + [_vp] * 8 + [_vp, _sz, _vp]),
+    "dibr_b200_laplacian_apply": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
+    "dibr_b200_vertex_average_forward": (_i, [_i, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dibr_b200_vertex_average_backward": (_i, [_i, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dibr_b200_mesh_dense": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dibr_b200_adjacency_coo": (_i, [_i, _i64, _vp, _vp, _vp, _vp]),
 }
 
 

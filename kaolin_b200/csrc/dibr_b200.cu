@@ -2571,6 +2571,20 @@ int check_backward(bool f64, int B, int F, int H, int W, int D, const void* grad
 
 }  // namespace
 
+// The launch trace for the library's other sources (mesh_topology.cu): the same events as Span.
+namespace dibr_b200_detail {
+bool span_open(const char* name, cudaStream_t st) {
+  Span s(name, st);        // records the opening event when a trace is open
+  const bool on = s.on;
+  s.on = false;            // span_close records the closing one
+  return on;
+}
+void span_close(cudaStream_t st) {
+  cudaEventRecord(g_trace.pool[g_trace.used + 1], st);
+  g_trace.used += 2;
+}
+}  // namespace dibr_b200_detail
+
 // ===========================================================================
 extern "C" {
 

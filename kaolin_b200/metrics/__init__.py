@@ -1,1 +1,2 @@
 from . import render  # noqa: F401
+from . import trianglemesh  # noqa: F401

@@ -1,0 +1,192 @@
+"""kaolin.ops.mesh drop-ins on sm_90a kernels (csrc/mesh_topology.cu): ``adjacency_matrix``,
+``uniform_laplacian``, ``average_face_vertex_features`` and ``compute_vertex_normals`` with the
+reference's signatures, and ``UniformLaplacian``, the Laplacian without its V x V matrix.
+
+The reference builds a dense V x V matrix (mesh.py:78-151), which does not fit in memory beyond a few
+ten thousand vertices.  Here the topology of ``faces`` is built once into two CSR structures (the
+corners of each vertex, and its unique neighbours) and every product is a gather over them.  The
+functional forms rebuild it on every call, as the reference rebuilds its matrix; ``UniformLaplacian``
+builds it once::
+
+    L = UniformLaplacian(V, faces)            # instead of L = uniform_laplacian(V, faces)
+    loss = (L @ (vertices - vertices_init)).pow(2).mean()
+
+Deliberate deviation: a face index outside [0, V) raises ``IndexError`` (the reference does not check).
+"""
+import torch
+
+from .. import _lib
+from ..render.mesh import _host
+
+__all__ = ["adjacency_matrix", "uniform_laplacian", "compute_vertex_normals", "average_face_vertex_features",
+           "UniformLaplacian"]
+
+
+def _check(func, typed):
+    """(name, tensor, dtype) triples: CUDA tensors on one device, each of its dtype; no CPU path."""
+    dev = _host.check_tensors(func, [(name, t) for name, t, _ in typed], dtype=None)
+    for name, t, dtype in typed:
+        if t.dtype != dtype:
+            raise RuntimeError(f"\"{func}\" not implemented for '{str(t.dtype).replace('torch.', '')}' "
+                               f"(kaolin_b200 takes {name} as {str(dtype).replace('torch.', '')})")
+    return dev
+
+
+class _Topology:
+    """The corner and adjacency CSRs of one mesh (see include/dibr_b200.h)."""
+
+    def __init__(self, func, num_vertices, faces):
+        _check(func, [("faces", faces, torch.int64)])
+        if faces.dim() != 2 or faces.shape[1] < 3:
+            raise RuntimeError(f"{func}: expected faces of shape (num_faces, face_size >= 3), got {list(faces.shape)}")
+        V, (F, S) = int(num_vertices), faces.shape
+        if V < 0:
+            raise ValueError(f"{func}: num_vertices must be >= 0, got {V}")
+        lib = _lib.lib()
+        nbytes = lib.dibr_b200_mesh_topology_workspace_bytes(V, F, S)
+        if nbytes == 0:
+            raise RuntimeError(f"{func}: {V} vertices or {F} faces of size {S} do not fit 32-bit indices")
+        dev = faces.device
+        faces = faces.contiguous()
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.num_vertices, self.faces = V, faces
+        self.corner_ptr = torch.empty(V + 1, **i32)
+        self.corners = torch.empty(max(F * S, 1), **i32)      # never empty: the ABI takes no NULL buffers
+        self.adj_ptr = torch.empty(V + 1, **i32)
+        self._adj = torch.empty(max(2 * F * S, 1), **i32)
+        self.degree = torch.empty(V, **i32)
+        self.weight = torch.empty(V, dtype=torch.float32, device=dev)
+        status = torch.empty(2, **i32)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _lib.check(lib.dibr_b200_mesh_topology_build(
+            V, F, S, _host.ptr(faces), _host.ptr(self.corner_ptr), _host.ptr(self.corners), _host.ptr(self.adj_ptr),
+            _host.ptr(self._adj), _host.ptr(self.degree), _host.ptr(self.weight), _host.ptr(status), _host.ptr(ws), nbytes,
+            _host.stream_ptr(dev)), func)
+        edges, error = status.tolist()          # the build's one device-to-host read
+        if error:
+            raise IndexError(f"{func}: faces holds an index outside [0, {V})")
+        self.num_edges = edges
+        self.adj = self._adj[:edges]
+
+    def apply(self, x, transpose, smooth):
+        """(L or L^T, + I if smooth) applied to x (..., V, C) float32, on the current stream."""
+        y = torch.empty_like(x)
+        V, C = x.shape[-2], x.shape[-1]
+        batch = x.numel() // max(V * C, 1)
+        _lib.check(_lib.lib().dibr_b200_laplacian_apply(
+            batch, V, C, _host.ptr(self.adj_ptr), _host.ptr(self._adj), _host.ptr(self.weight), _host.ptr(x),
+            int(transpose), int(smooth), _host.ptr(y), _host.stream_ptr(x.device)), "laplacian_apply")
+        return y
+
+    def dense(self, laplacian):
+        V = self.num_vertices
+        out = torch.empty((V, V), dtype=torch.float32, device=self.faces.device)
+        _lib.check(_lib.lib().dibr_b200_mesh_dense(
+            V, int(laplacian), _host.ptr(self.adj_ptr), _host.ptr(self._adj), _host.ptr(self.weight), _host.ptr(out),
+            _host.stream_ptr(out.device)), "uniform_laplacian" if laplacian else "adjacency_matrix")
+        return out
+
+
+class _Apply(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, topo, smooth):
+        ctx.topo, ctx.smooth = topo, smooth
+        return topo.apply(x, False, smooth)
+
+    @staticmethod
+    def backward(ctx, grad):
+        return ctx.topo.apply(grad.contiguous(), True, ctx.smooth), None, None
+
+
+def _apply(func, topo, x, smooth):
+    _check(func, [("x", x, torch.float32), ("faces", topo.faces, torch.int64)])
+    if x.dim() not in (2, 3) or x.shape[-2] != topo.num_vertices:
+        raise RuntimeError(f"{func}: expected x of shape (V, k) or (B, V, k) with V = {topo.num_vertices}, "
+                           f"got {list(x.shape)}")
+    return _Apply.apply(x.contiguous(), topo, smooth)
+
+
+class UniformLaplacian:
+    r"""The uniform Laplacian of a mesh, built once, without its :math:`V \times V` matrix.
+
+    ``L @ x`` (or ``L.matmul(x)``) equals ``torch.matmul(uniform_laplacian(num_vertices, faces), x)``
+    for x of shape (V, k) or (B, V, k) float32, with autograd to x; ``L.to_dense()`` is
+    ``uniform_laplacian(num_vertices, faces)``.  Memory is O(F·S + V).
+    """
+
+    def __init__(self, num_vertices, faces):
+        self._topo = _Topology("UniformLaplacian", num_vertices, faces)
+
+    def matmul(self, x):
+        return _apply("UniformLaplacian.matmul", self._topo, x, False)
+
+    __matmul__ = matmul
+
+    def to_dense(self):
+        return self._topo.dense(True)
+
+
+def adjacency_matrix(num_vertices, faces, sparse=True):
+    r"""kaolin.ops.mesh.adjacency_matrix: the (V, V) 0/1 adjacency, as a sparse COO tensor (indices in
+    lexicographic order, not marked coalesced) or dense float32."""
+    topo = _Topology("adjacency_matrix", num_vertices, faces)
+    if not sparse:
+        return topo.dense(False)
+    E = topo.num_edges
+    indices = torch.empty((2, E), dtype=torch.int64, device=faces.device)
+    _lib.check(_lib.lib().dibr_b200_adjacency_coo(
+        topo.num_vertices, E, _host.ptr(topo.adj_ptr), _host.ptr(topo._adj), _host.ptr(indices),
+        _host.stream_ptr(faces.device)), "adjacency_matrix")
+    values = torch.ones(E, dtype=torch.float32, device=faces.device)
+    return torch.sparse_coo_tensor(indices, values, (topo.num_vertices, topo.num_vertices))
+
+
+def uniform_laplacian(num_vertices, faces):
+    r"""kaolin.ops.mesh.uniform_laplacian: the dense (V, V) float32 matrix, -1 on the diagonal and
+    1 / num_neighbours(i) at the neighbours of i."""
+    return _Topology("uniform_laplacian", num_vertices, faces).dense(True)
+
+
+class _Average(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, face_features, topo):
+        ctx.topo = topo
+        B, F, S, N = face_features.shape
+        V = topo.num_vertices
+        out = torch.empty((B, V, N), dtype=torch.float32, device=face_features.device)
+        _lib.check(_lib.lib().dibr_b200_vertex_average_forward(
+            B, V, F, S, N, _host.ptr(topo.corner_ptr), _host.ptr(topo.corners), _host.ptr(face_features),
+            _host.ptr(out), _host.stream_ptr(out.device)), "average_face_vertex_features")
+        ctx.shape = face_features.shape
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        topo = ctx.topo
+        B, F, S, N = ctx.shape
+        grad = grad.contiguous()
+        g_ff = torch.empty(ctx.shape, dtype=torch.float32, device=grad.device)
+        _lib.check(_lib.lib().dibr_b200_vertex_average_backward(
+            B, topo.num_vertices, F, S, N, _host.ptr(topo.faces), _host.ptr(topo.corner_ptr), _host.ptr(grad),
+            _host.ptr(g_ff), _host.stream_ptr(grad.device)), "average_face_vertex_features")
+        return g_ff, None
+
+
+def average_face_vertex_features(faces, face_features, num_vertices=None):
+    r"""kaolin.ops.mesh.average_face_vertex_features: per-vertex mean of ``face_features``
+    (B, F, S, N) float32 over the faces incident to each vertex -> (B, V, N); 0 where no face is."""
+    func = "average_face_vertex_features"
+    _check(func, [("face_features", face_features, torch.float32), ("faces", faces, torch.int64)])
+    if faces.dim() != 2 or face_features.dim() != 4 or tuple(face_features.shape[1:3]) != tuple(faces.shape):
+        raise RuntimeError(f"{func}: expected face_features of shape (B, {faces.shape[0]}, {faces.shape[-1]}, N), "
+                           f"got {list(face_features.shape)}")
+    if num_vertices is None:
+        num_vertices = int(faces.max()) + 1
+    topo = _Topology(func, num_vertices, faces)
+    return _Average.apply(face_features.contiguous(), topo)
+
+
+def compute_vertex_normals(faces, face_normals, num_vertices=None):
+    r"""kaolin.ops.mesh.compute_vertex_normals: ``average_face_vertex_features`` of the per-corner
+    normals (B, F, S, 3) -> (B, V, 3)."""
+    return average_face_vertex_features(faces, face_normals, num_vertices=num_vertices)
