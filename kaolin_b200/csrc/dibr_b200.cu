@@ -657,7 +657,9 @@ __device__ __forceinline__ int soft_collect(const Scene& s, const TileCtx& c, SM
 // Normally hi = INT_MAX takes everything; when more than kSoftCap faces remain
 // (sub-pixel triangles) a prefix window in index order is taken instead: its upper end
 // is guessed from the average index density and halved until it fits (1-3 counting
-// passes), the caller continues with lo = hi until every pixel has its knum faces.
+// passes), the caller continues with lo = hi until every pixel has its knum faces.  A
+// window that comes out empty (the candidates cluster at higher indices) is moved past, so
+// n = 0 always means that no candidate is left above lo.
 template <typename SM>
 __device__ __forceinline__ int soft_window(const Scene& s, const TileCtx& c, SM& sm, int lo, int maxf, int& hi) {
   hi = 0x7fffffff;
@@ -668,7 +670,9 @@ __device__ __forceinline__ int soft_window(const Scene& s, const TileCtx& c, SM&
     if (width < 1) width = 1;
     while (true) {
       hi = lo + width;
-      if (soft_collect<true>(s, c, sm, lo, hi) <= kSoftCap || width == 1) break;
+      const int in_window = soft_collect<true>(s, c, sm, lo, hi);
+      if (in_window == 0) { lo = hi; continue; }  // all n candidates lie above hi
+      if (in_window <= kSoftCap || width == 1) break;
       width = width > 1 ? width / 2 : 1;
     }
     n = soft_collect<false>(s, c, sm, lo, hi);
