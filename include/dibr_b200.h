@@ -159,12 +159,16 @@ int dibr_b200_backward_views(
 /*
  * float64 instantiation of the fused entry points (the reference dispatches float and double:
  * rasterization_cuda.cu:218/427, dibr_soft_mask_cuda.cu:205/376; its tests parametrise the dtype).
- * Same contract as dibr_b200_forward / dibr_b200_backward with double tensors (face_idx stays i64;
- * multiplier / eps / sigmainv are C floats exactly as in the reference kernels' signatures, the
- * enlarged-bbox margin boxlen * multiplier is a double as in dibr.py:33-39).  Every per-pixel decision
- * is taken with the reference's <double> arithmetic (pixel centres computed in float and widened);
- * built for exactness, not speed (one thread per pixel walks its tile's bins; double atomics in the
- * backward).  workspace >= dibr_b200_workspace_bytes_f64(); pass it unchanged to the backward with
+ * Same contract as dibr_b200_forward / dibr_b200_backward with double tensors (face_idx stays i64).
+ * multiplier is a double: the vertices are scaled by it in double, as the reference's wrappers do in
+ * torch (rasterization.py:320, dibr.py:32); its float rounding is what the reference's kernels get, so
+ * it places the pixel centres and is the multiplier of 4*m*m, the probability and the gradient
+ * division.  eps / sigmainv are C floats as in the reference kernels' signatures; the enlarged-bbox
+ * margin boxlen * multiplier is a double as in dibr.py:33-39.  Every per-pixel decision is taken with
+ * the reference's <double> arithmetic, and face_idx, the weights, the features and the forward soft
+ * mask are bit-identical to the reference's <double> kernels (tests/test_f64_matrix_gpu.py); the
+ * gradients differ only in the order of the double atomics.  Built for exactness, not speed (one
+ * thread per pixel walks its tile's bins; double atomics in the backward).  workspace >= dibr_b200_workspace_bytes_f64(); pass it unchanged to the backward with
  * DIBR_B200_BINS_VALID to reuse the forward's bins.
  */
 size_t dibr_b200_workspace_bytes_f64(int batch, int64_t total_faces, int height, int width);
@@ -172,7 +176,7 @@ int dibr_b200_forward_f64(
     int batch, int num_faces, int height, int width, int feat_dim,
     const double* face_vertices_z, const double* face_vertices_image,
     const double* face_features, const double* face_normals_z, const uint8_t* valid_faces,
-    float multiplier, float eps, int mode, float sigmainv, double boxlen_m, int knum,
+    double multiplier, float eps, int mode, float sigmainv, double boxlen_m, int knum,
     double* interpolated_features, int64_t* face_idx, double* output_weights, double* soft_mask,
     void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
 int dibr_b200_backward_f64(
@@ -180,7 +184,7 @@ int dibr_b200_backward_f64(
     const double* grad_features, const double* grad_soft_mask,
     const int64_t* face_idx, const double* output_weights, const double* soft_mask,
     const double* face_vertices_image, const double* face_features,
-    float multiplier, float eps, float sigmainv, double boxlen_m, int knum,
+    double multiplier, float eps, float sigmainv, double boxlen_m, int knum,
     double* grad_face_vertices_image, double* grad_face_features,
     void* workspace, size_t workspace_bytes, int flags, dibr_b200_stream_t stream);
 

@@ -52,10 +52,10 @@ SIGNATURES = {
     "dibr_b200_backward_views": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i,
                                       _f, _f, _f, _f, _i, _vp, _vp, _vp, _sz, _i, _i, _i, _vp]),
     "dibr_b200_workspace_bytes_f64": (_sz, [_i, _i64, _i, _i]),
-    "dibr_b200_forward_f64": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _i, _f, _d, _i,
+    "dibr_b200_forward_f64": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _d, _f, _i, _f, _d, _i,
                                    _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dibr_b200_backward_f64": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                    _f, _f, _f, _d, _i, _vp, _vp, _vp, _sz, _i, _vp]),
+                                    _d, _f, _f, _d, _i, _vp, _vp, _vp, _sz, _i, _vp]),
     "dibr_b200_forward_bf16": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _i, _f, _f, _i,
                                     _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dibr_b200_backward_bf16": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,

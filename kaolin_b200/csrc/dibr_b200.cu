@@ -2600,21 +2600,24 @@ size_t dibr_b200_workspace_bytes_f64(int batch, int64_t total_faces, int height,
 int dibr_b200_forward_f64(int batch, int num_faces, int height, int width, int feat_dim,
                           const double* face_vertices_z, const double* face_vertices_image,
                           const double* face_features, const double* face_normals_z, const uint8_t* valid_faces,
-                          float multiplier, float eps, int mode, float sigmainv, double boxlen_m, int knum,
+                          double multiplier, float eps, int mode, float sigmainv, double boxlen_m, int knum,
                           double* interpolated_features, int64_t* face_idx, double* output_weights,
                           double* soft_mask, void* workspace, size_t workspace_bytes_, dibr_b200_stream_t stream) {
+  const float multiplier_f = (float)multiplier;      // the reference kernels' float parameter
   int rc = check_forward(true, batch, num_faces, height, width, feat_dim, mode, face_vertices_z, face_vertices_image,
-                         face_features, face_normals_z, valid_faces, multiplier, knum, interpolated_features, face_idx,
+                         face_features, face_normals_z, valid_faces, multiplier_f, knum, interpolated_features, face_idx,
                          output_weights, soft_mask);
   if (rc) return rc;
   const bool raster = mode & DIBR_B200_RASTER, soft = mode & DIBR_B200_SOFT_MASK;
   cudaStream_t st = (cudaStream_t)stream;
   F64Args a;
-  rc = f64_scene(a.s, batch, num_faces, height, width, multiplier, workspace, workspace_bytes_);
+  rc = f64_scene(a.s, batch, num_faces, height, width, multiplier_f, workspace, workspace_bytes_);
   if (rc) return rc;
-  rc = f64_bins(a.s, face_vertices_image, face_normals_z, valid_faces, boxlen_m, (raster ? 1 : 0) | (soft ? 2 : 0), st);
+  rc = f64_bins(a.s, face_vertices_image, face_normals_z, valid_faces, multiplier, boxlen_m,
+                (raster ? 1 : 0) | (soft ? 2 : 0), st);
   if (rc) return rc;
-  a.D = feat_dim; a.K = knum; a.mode = mode; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier;
+  a.D = feat_dim; a.K = knum; a.mode = mode; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier_f;
+  a.scale = multiplier;
   a.margin = boxlen_m; a.xy = face_vertices_image; a.z = face_vertices_z; a.feat = face_features;
   a.out_feat = interpolated_features; a.idx = face_idx; a.out_w = output_weights; a.out_soft = soft_mask;
   a.g_feat = nullptr; a.g_soft = nullptr; a.soft = nullptr; a.g_xy = nullptr; a.g_ff = nullptr;
@@ -2626,13 +2629,14 @@ int dibr_b200_forward_f64(int batch, int num_faces, int height, int width, int f
 int dibr_b200_backward_f64(int batch, int num_faces, int height, int width, int feat_dim,
                            const double* grad_features, const double* grad_soft_mask, const int64_t* face_idx,
                            const double* output_weights, const double* soft_mask, const double* face_vertices_image,
-                           const double* face_features, float multiplier, float eps, float sigmainv, double boxlen_m,
+                           const double* face_features, double multiplier, float eps, float sigmainv, double boxlen_m,
                            int knum, double* grad_face_vertices_image, double* grad_face_features, void* workspace,
                            size_t workspace_bytes_, int flags, dibr_b200_stream_t stream) {
   const int64_t NF = (int64_t)batch * num_faces;
+  const float multiplier_f = (float)multiplier;      // the reference kernels' float parameter
   F64Args a;
   int rc = check_backward(true, batch, num_faces, height, width, feat_dim, grad_features, grad_soft_mask, face_idx,
-                          output_weights, soft_mask, face_vertices_image, face_features, multiplier, 0.f, knum,
+                          output_weights, soft_mask, face_vertices_image, face_features, multiplier_f, 0.f, knum,
                           grad_face_vertices_image, grad_face_features, workspace, workspace_bytes_, 0, batch, a.s);
   if (rc) return rc;
   const bool run_raster = grad_features && feat_dim > 0;
@@ -2646,10 +2650,11 @@ int dibr_b200_backward_f64(int batch, int num_faces, int height, int width, int 
   if (NF == 0 || (!run_raster && !grad_soft_mask)) return 0;
   // the soft-mask branch needs the enlarged bins: forward's (BINS_VALID) or rebuilt here
   if (grad_soft_mask && !(flags & DIBR_B200_BINS_VALID)) {
-    rc = f64_bins(a.s, face_vertices_image, nullptr, nullptr, boxlen_m, 2, st);
+    rc = f64_bins(a.s, face_vertices_image, nullptr, nullptr, multiplier, boxlen_m, 2, st);
     if (rc) return rc;
   }
-  a.D = feat_dim; a.K = knum; a.mode = 0; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier;
+  a.D = feat_dim; a.K = knum; a.mode = 0; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier_f;
+  a.scale = multiplier;
   a.margin = boxlen_m; a.xy = face_vertices_image; a.z = nullptr; a.feat = face_features;
   a.out_feat = nullptr; a.idx = const_cast<int64_t*>(face_idx); a.out_w = const_cast<double*>(output_weights);
   a.out_soft = nullptr; a.g_feat = run_raster ? grad_features : nullptr; a.g_soft = grad_soft_mask; a.soft = soft_mask;

@@ -20,7 +20,8 @@
 struct F64Args {
   Scene s;
   int D, K, mode;
-  float eps, sigmainv, multiplier;
+  float eps, sigmainv, multiplier;                        // C floats, as the reference kernels take them
+  double scale;                                           // the multiplier the vertices are scaled by, in double
   double margin;                                          // boxlen * multiplier, in double
   const double* xy; const double* z; const double* feat;  // (NF,3,2) unscaled, (NF,3), (NF,3,D)
   double* out_feat; int64_t* idx; double* out_w; double* out_soft;
@@ -29,12 +30,11 @@ struct F64Args {
 };
 
 __global__ void __launch_bounds__(256) f64_prep_kernel(int64_t NF, const double* __restrict__ xy, const double* __restrict__ fnz,
-                                                       const uint8_t* __restrict__ valid_in, float multiplier, double margin,
+                                                       const uint8_t* __restrict__ valid_in, double m, double margin,
                                                        float* __restrict__ xyf, float* __restrict__ bt, float* __restrict__ bl,
                                                        uint8_t* __restrict__ valid) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= NF) return;
-  const double m = (double)multiplier;
   double v[6];
 #pragma unroll
   for (int k = 0; k < 6; ++k) { v[k] = __dmul_rn(xy[i * 6 + k], m); xyf[i * 6 + k] = (float)v[k]; }
@@ -64,7 +64,6 @@ template <typename Hit>
 __device__ __forceinline__ void f64_soft_walk(const F64Args& a, const TileCtx& c, TileSmem& sm, bool uncovered,
                                               double x0, double y0, Hit hit) {
   const Scene& s = a.s;
-  const double m = (double)a.multiplier;
   const int maxf = s.F;
   bool want = uncovered;
   int lo = -1;
@@ -77,7 +76,7 @@ __device__ __forceinline__ void f64_soft_walk(const F64Args& a, const TileCtx& c
       if (want && (((uint32_t)key) & c.sel) == c.sel) {
         const int f = (int)(key >> 32);
         double v[6], bb[4];
-        f64_face(a, c.fbase + f, m, v, bb);
+        f64_face(a, c.fbase + f, a.scale, v, bb);
         // dibr.py:33-39 in double: [min - boxlen*m, max + boxlen*m]; dibr_soft_mask_cuda.cu:95
         if (!(x0 < bb[0] - a.margin || x0 >= bb[2] + a.margin || y0 < bb[1] - a.margin || y0 >= bb[3] + a.margin))
           want = hit(f, v);
@@ -97,7 +96,6 @@ __global__ void __launch_bounds__(kThreads) dibr_f64_kernel(const __grid_constan
   load_bin_table(s, c, sm);
   __syncthreads();
   const double x0 = (double)c.x0, y0 = (double)c.y0;     // computed in float, widened (rasterization_cuda.cu:85-86)
-  const double m = (double)a.multiplier;
   int best = -1;
   if (!BWD && (a.mode & DIBR_B200_RASTER)) {
     double bz = -INFINITY, b0 = 0.0, b1 = 0.0, b2 = 0.0;
@@ -108,7 +106,7 @@ __global__ void __launch_bounds__(kThreads) dibr_f64_kernel(const __grid_constan
         const int x_lo = e.y & 0xffff, x_hi = (int)((unsigned)e.y >> 16), y_lo = e.z & 0xffff, y_hi = (int)((unsigned)e.z >> 16);
         if (c.px < x_lo || c.px >= x_hi || c.py < y_lo || c.py >= y_hi) continue;
         double v[6], bb[4];
-        f64_face(a, c.fbase + e.x, m, v, bb);
+        f64_face(a, c.fbase + e.x, a.scale, v, bb);
         if (x0 < bb[0] || x0 >= bb[2] || y0 < bb[1] || y0 >= bb[3]) continue;
         double w0, w1, w2;
         if (!dibr64::raster_weights((double)a.eps, x0, y0, v[0], v[1], v[2], v[3], v[4], v[5], w0, w1, w2)) continue;
@@ -204,7 +202,8 @@ F64Layout f64_layout(int B, int64_t NF, int H, int W) {
 }
 
 // Lays out the float scene of a double call (scaled vertices, conservative bboxes, validity) in the
-// workspace.  Host only: nothing is enqueued.
+// workspace.  Host only: nothing is enqueued.  `multiplier` is the C float the reference's kernels
+// take: it places the pixel centres.
 int f64_scene(Scene& s, int B, int F, int H, int W, float multiplier, void* ws, size_t ws_bytes) {
   const int64_t NF = (int64_t)B * F;
   const F64Layout L = f64_layout(B, NF, H, W);
@@ -219,12 +218,14 @@ int f64_scene(Scene& s, int B, int F, int H, int W, float multiplier, void* ws, 
   return 0;
 }
 
-// Fills the float scene laid out by f64_scene from the double inputs and bins it.
-int f64_bins(const Scene& s, const double* fvi, const double* fnz, const uint8_t* valid, double margin, int sets,
-             cudaStream_t st) {
+// Fills the float scene laid out by f64_scene from the double inputs, scaled by the double
+// multiplier `scale` (face_vertices_image * multiplier in torch, rasterization.py:320, dibr.py:32),
+// and bins it.
+int f64_bins(const Scene& s, const double* fvi, const double* fnz, const uint8_t* valid, double scale, double margin,
+             int sets, cudaStream_t st) {
   if (s.NF > 0)
     f64_prep_kernel<<<(unsigned)((s.NF + 255) / 256), 256, 0, st>>>(
-        s.NF, fvi, fnz, valid, s.multiplier, margin, const_cast<float*>(s.xy), const_cast<float*>(s.bbox_tight),
+        s.NF, fvi, fnz, valid, scale, margin, const_cast<float*>(s.xy), const_cast<float*>(s.bbox_tight),
         const_cast<float*>(s.bbox_large), const_cast<uint8_t*>(s.valid));
   return build_bins(s, sets, st);     // with no faces: zeroed counters, every pixel takes the empty path
 }

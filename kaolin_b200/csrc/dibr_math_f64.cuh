@@ -5,8 +5,11 @@
 // (w0 + w1) + w2, DADD of the copysign eps, three IEEE divisions; pixel centres computed in
 // float and widened), i.e. the <float> trees of dibr_math.cuh with double operations, so face_idx
 // is decided by the same comparisons.  The soft-mask distances / gradients follow the source
-// expressions with the same fma placement as the <float> trees; they are tolerance-checked
-// (1e-9) against the reference's double kernels, not bit-compared.
+// expressions with the same fma placement as the <float> trees, which is also the per-edge tree of
+// the reference's <double> soft-mask kernel.  face_idx, the weights, the interpolated features and
+// the forward soft mask are bit-compared with the reference's <double> kernels
+// (tests/test_f64_matrix_gpu.py); the gradients are compared to 1e-13 of their scale, as both sides
+// sum them with double atomics in different orders.
 #pragma once
 #include "dibr_math.cuh"
 
