@@ -7,20 +7,12 @@ wrappers: ``kaolin.render.mesh.rasterization`` / ``.dibr`` run unmodified with
 ``kaolin._C`` replaced by this module (tests/test_reference_wrappers.py: arity / dispatch on CPU,
 results on the GPU).
 """
-import ctypes
 import types
 
 import torch
 
 from . import _lib
-
-
-def _ptr(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream(dev):
-    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+from .render.mesh import _host
 
 
 def _check_all(func, named, float_dtype=torch.float32):
@@ -67,13 +59,6 @@ def _check_size(func, name, t, shape):
                            f"got {list(t.shape)}")
 
 
-def _workspace(batch, total_faces, height, width, dev):
-    n = _lib.lib().dibr_b200_workspace_bytes(batch, total_faces, height, width)
-    if n == 0:
-        raise RuntimeError("kaolin_b200: unsupported problem size")
-    return torch.empty(n, dtype=torch.uint8, device=dev)
-
-
 @_fp64_via_fp32
 def packed_rasterize_forward_cuda(height, width, face_vertices_z, face_vertices_image,
                                   face_bboxes, face_features, first_idx_face_per_mesh,
@@ -97,14 +82,12 @@ def packed_rasterize_forward_cuda(height, width, face_vertices_z, face_vertices_
     idx = torch.empty((batch_size, height, width), dtype=torch.int64, device=dev)
     w = torch.empty((batch_size, height, width, 3), dtype=torch.float32, device=dev)
     out = torch.empty((batch_size, height, width, feat_dim), dtype=torch.float32, device=dev)
-    ws = _workspace(batch_size, num_faces, height, width, dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_packed_rasterize_forward(
-            batch_size, num_faces, height, width, feat_dim, _ptr(face_vertices_z),
-            _ptr(face_vertices_image), _ptr(face_bboxes), _ptr(face_features),
-            _ptr(first_idx_face_per_mesh), float(multiplier), float(eps),
-            _ptr(out), _ptr(idx), _ptr(w), _ptr(ws), ws.numel(), _stream(dev))
-    _lib.check(st, fn)
+    ws = _host.workspace(batch_size, num_faces, height, width, dev)
+    _lib.call("dibr_b200_packed_rasterize_forward", dev,
+              batch_size, num_faces, height, width, feat_dim, face_vertices_z,
+              face_vertices_image, face_bboxes, face_features,
+              first_idx_face_per_mesh, float(multiplier), float(eps),
+              out, idx, w, ws, ws.numel(), what=fn)
     return [out, idx, w]
 
 
@@ -129,15 +112,12 @@ def rasterize_backward_cuda(grad_interpolated_features, interpolated_features, s
     g_xy = torch.empty_like(face_vertices_image)
     g_ff = torch.empty_like(face_features)
     # dibr_b200_rasterize_backward shares the fused backward's 16-byte pointer alignment requirement
-    from .render.mesh._host import aligned
     (grad_interpolated_features, selected_face_idx, output_weights, face_vertices_image, face_features) = map(
-        aligned, (grad_interpolated_features, selected_face_idx, output_weights, face_vertices_image, face_features))
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_rasterize_backward(
-            B, F, H, W, D, _ptr(grad_interpolated_features), _ptr(selected_face_idx),
-            _ptr(output_weights), _ptr(face_vertices_image), _ptr(face_features), float(eps),
-            _ptr(g_xy), _ptr(g_ff), _stream(dev))
-    _lib.check(st, fn)
+        _host.aligned, (grad_interpolated_features, selected_face_idx, output_weights, face_vertices_image, face_features))
+    _lib.call("dibr_b200_rasterize_backward", dev,
+              B, F, H, W, D, grad_interpolated_features, selected_face_idx,
+              output_weights, face_vertices_image, face_features, float(eps),
+              g_xy, g_ff, what=fn)
     return [g_xy, g_ff]
 
 
@@ -158,13 +138,11 @@ def dibr_soft_mask_forward_cuda(face_vertices_image, face_large_bboxes, selected
     prob = torch.empty((B, H, W, knum), dtype=torch.float32, device=dev)
     cidx = torch.empty((B, H, W, knum), dtype=torch.int64, device=dev)
     ctype = torch.empty((B, H, W, knum), dtype=torch.uint8, device=dev)
-    ws = _workspace(B, B * F, H, W, dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_soft_mask_forward(
-            B, F, H, W, int(knum), _ptr(face_vertices_image), _ptr(face_large_bboxes),
-            _ptr(selected_face_idx), float(sigmainv), float(multiplier),
-            _ptr(soft), _ptr(prob), _ptr(cidx), _ptr(ctype), _ptr(ws), ws.numel(), _stream(dev))
-    _lib.check(st, fn)
+    ws = _host.workspace(B, B * F, H, W, dev)
+    _lib.call("dibr_b200_soft_mask_forward", dev,
+              B, F, H, W, int(knum), face_vertices_image, face_large_bboxes,
+              selected_face_idx, float(sigmainv), float(multiplier),
+              soft, prob, cidx, ctype, ws, ws.numel(), what=fn)
     return [soft, prob, cidx, ctype]
 
 
@@ -191,12 +169,10 @@ def dibr_soft_mask_backward_cuda(grad_soft_mask, soft_mask, selected_face_idx, c
     _check_size(fn, "face_vertices_image", face_vertices_image, (B, F, 3, 2))
     g = torch.empty_like(face_vertices_image)
     sel = selected_face_idx.contiguous()
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_soft_mask_backward(
-            B, F, H, W, K, _ptr(grad_soft_mask), _ptr(soft_mask), _ptr(sel), _ptr(close_face_prob),
-            _ptr(close_face_idx), _ptr(close_face_dist_type), _ptr(face_vertices_image),
-            float(sigmainv), float(multiplier), _ptr(g), _stream(dev))
-    _lib.check(st, fn)
+    _lib.call("dibr_b200_soft_mask_backward", dev,
+              B, F, H, W, K, grad_soft_mask, soft_mask, sel, close_face_prob,
+              close_face_idx, close_face_dist_type, face_vertices_image,
+              float(sigmainv), float(multiplier), g, what=fn)
     return g
 
 
@@ -219,14 +195,11 @@ def deftet_sparse_render_forward_cuda(face_vertices_z, face_vertices_image, face
     depth = torch.empty((B, P, knum), dtype=torch.float32, device=dev)
     w0 = torch.empty((B, P, knum), dtype=torch.float32, device=dev)
     w1 = torch.empty((B, P, knum), dtype=torch.float32, device=dev)
-    n = _lib.lib().dibr_b200_deftet_workspace_bytes(B, F)
-    ws = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_deftet_sparse_render_forward(
-            B, F, P, int(knum), _ptr(face_vertices_z), _ptr(face_vertices_image), _ptr(face_bboxes),
-            _ptr(pixel_coords), _ptr(pixel_depth_ranges), float(eps), _ptr(idx), _ptr(depth), _ptr(w0), _ptr(w1),
-            _ptr(ws), ws.numel(), _stream(dev))
-    _lib.check(st, fn)
+    ws = _lib.scratch(_lib.lib().dibr_b200_deftet_workspace_bytes(B, F), dev)
+    _lib.call("dibr_b200_deftet_sparse_render_forward", dev,
+              B, F, P, int(knum), face_vertices_z, face_vertices_image, face_bboxes,
+              pixel_coords, pixel_depth_ranges, float(eps), idx, depth, w0, w1,
+              ws, ws.numel(), what=fn)
     return [idx, depth, w0, w1]
 
 
@@ -246,11 +219,9 @@ def deftet_sparse_render_backward_cuda(grad_interpolated_features, face_idx, wei
     _check_size(fn, "face_features", face_features, (B, F, 3, D))
     g_xy = torch.empty_like(face_vertices_image)
     g_ff = torch.empty_like(face_features)
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_deftet_sparse_render_backward(
-            B, F, P, K, D, _ptr(grad_interpolated_features), _ptr(face_idx), _ptr(weights),
-            _ptr(face_vertices_image), _ptr(face_features), float(eps), _ptr(g_xy), _ptr(g_ff), _stream(dev))
-    _lib.check(st, fn)
+    _lib.call("dibr_b200_deftet_sparse_render_backward", dev,
+              B, F, P, K, D, grad_interpolated_features, face_idx, weights,
+              face_vertices_image, face_features, float(eps), g_xy, g_ff, what=fn)
     return [g_xy, g_ff]
 
 

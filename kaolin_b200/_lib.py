@@ -1,13 +1,15 @@
 """ctypes binding of the C ABI (include/dibr_b200.h) + in-tree build of libdibr_b200.so.
 
 PyTorch is used for device memory and streams only; every compute call goes
-through the ``extern "C"`` entry points with raw device pointers.  There is no
-fallback: a missing library is an error.
+through the ``extern "C"`` entry points with raw device pointers, by ``call``.
+There is no fallback: a missing library is an error.
 """
 import ctypes
 import os
 import subprocess
 import threading
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
@@ -176,3 +178,35 @@ def check(status, what):
     if status == ESIZE:
         raise RuntimeError(f"{what}: image larger than 16384 px per side or index overflow")
     raise RuntimeError(f"{what}: CUDA error {status}")
+
+
+def ptr(t):
+    """A tensor as a ``void *`` argument (its data pointer); None stays NULL."""
+    return None if t is None else ctypes.c_void_p(t.data_ptr())
+
+
+def stream_ptr(device):
+    """The current stream of ``device`` as a ``cudaStream_t`` argument."""
+    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def call(name, device, *args, stream=None, what=None):
+    """Enqueue the entry point ``name`` on ``device`` and raise on a non-zero status (reported
+    under ``what``, by default ``name``).  Tensor arguments pass as their data pointers, every other
+    argument as it is.  Every enqueueing entry point takes its stream last: ``stream`` (a
+    ``torch.cuda.Stream``) or else ``device``'s current stream is appended.  The library launches on
+    the runtime's current device, so the call runs with ``device`` current."""
+    # Pointers and the stream go to ctypes as ints: SIGNATURES declares them ``void *``, and ctypes
+    # converts an int there in C, at a fraction of the cost of a c_void_p built in Python.
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    if stream is None:
+        stream = torch.cuda.current_stream(device)
+    with torch.cuda.device(device):
+        status = getattr(lib(), name)(*args, stream.cuda_stream)
+    check(status, what or name)
+
+
+def scratch(nbytes, device):
+    """A ``uint8`` workspace of ``nbytes`` bytes, at least one, so its pointer is never NULL: the
+    entry points reject a NULL workspace wherever they use one, and a size query may answer 0."""
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)

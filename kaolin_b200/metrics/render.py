@@ -19,10 +19,7 @@ class MaskIouB200(Function):
         hw = l.numel() // B
         sums = torch.empty((B, 2), dtype=torch.float32, device=l.device)
         loss = torch.empty((), dtype=torch.float32, device=l.device)
-        with torch.cuda.device(l.device):
-            st = _lib.lib().dibr_b200_mask_iou_forward(B, hw, _host.ptr(l), _host.ptr(r), _host.ptr(sums),
-                                                       _host.ptr(loss), _host.stream_ptr(l.device))
-        _lib.check(st, "dibr_b200_mask_iou_forward")
+        _lib.call("dibr_b200_mask_iou_forward", l.device, B, hw, l, r, sums, loss)
         ctx.save_for_backward(l, r, sums)
         return loss
 
@@ -34,11 +31,7 @@ class MaskIouB200(Function):
         g_l = torch.empty_like(l) if ctx.needs_input_grad[0] else None
         g_r = torch.empty_like(r) if ctx.needs_input_grad[1] else None
         g = g_loss.contiguous().to(torch.float32)
-        with torch.cuda.device(l.device):
-            st = _lib.lib().dibr_b200_mask_iou_backward(B, hw, _host.ptr(l), _host.ptr(r), _host.ptr(sums),
-                                                        _host.ptr(g), _host.ptr(g_l), _host.ptr(g_r),
-                                                        _host.stream_ptr(l.device))
-        _lib.check(st, "dibr_b200_mask_iou_backward")
+        _lib.call("dibr_b200_mask_iou_backward", l.device, B, hw, l, r, sums, g, g_l, g_r)
         return g_l, g_r
 
 

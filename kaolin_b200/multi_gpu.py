@@ -371,17 +371,13 @@ class PeerGradAllGather:
             s.wait_event(ready)
             off = pool.byte_offset(self.gen, kind, pool.rank)
             if self.engine == "mc":
-                st = _lib.lib().dibr_b200_peer_push_multicast(
-                    ctypes.c_void_p(local.data_ptr()), local.numel() * pool.esz, ctypes.c_void_p(pool.multicast_ptr),
-                    off, self.ctas, ctypes.c_void_p(s.cuda_stream))
-                _lib.check(st, "dibr_b200_peer_push_multicast")
+                _lib.call("dibr_b200_peer_push_multicast", dev, local, local.numel() * pool.esz, pool.multicast_ptr,
+                          off, self.ctas, stream=s)
                 return
             if pool.ptr_array is None:
                 pool.ptr_array = (ctypes.c_void_p * pool.world)(*[pool.ptrs[r] for r in order])
-            st = _lib.lib().dibr_b200_peer_push(ctypes.c_void_p(local.data_ptr()), local.numel() * pool.esz,
-                                                pool.ptr_array, pool.world, off, self.ctas,
-                                                ctypes.c_void_p(s.cuda_stream))
-            _lib.check(st, "dibr_b200_peer_push")
+            _lib.call("dibr_b200_peer_push", dev, local, local.numel() * pool.esz, pool.ptr_array, pool.world, off,
+                      self.ctas, stream=s)
             return
         for i, r in enumerate(order):
             s = pool.streams[i % len(pool.streams)]

@@ -42,8 +42,7 @@ class _Topology:
         V, (F, S) = int(num_vertices), faces.shape
         if V < 0:
             raise ValueError(f"{func}: num_vertices must be >= 0, got {V}")
-        lib = _lib.lib()
-        nbytes = lib.dibr_b200_mesh_topology_workspace_bytes(V, F, S)
+        nbytes = _lib.lib().dibr_b200_mesh_topology_workspace_bytes(V, F, S)
         if nbytes == 0:
             raise RuntimeError(f"{func}: {V} vertices or {F} faces of size {S} do not fit 32-bit indices")
         dev = faces.device
@@ -58,10 +57,9 @@ class _Topology:
         self.weight = torch.empty(V, dtype=torch.float32, device=dev)
         status = torch.empty(2, **i32)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _lib.check(lib.dibr_b200_mesh_topology_build(
-            V, F, S, _host.ptr(faces), _host.ptr(self.corner_ptr), _host.ptr(self.corners), _host.ptr(self.adj_ptr),
-            _host.ptr(self._adj), _host.ptr(self.degree), _host.ptr(self.weight), _host.ptr(status), _host.ptr(ws), nbytes,
-            _host.stream_ptr(dev)), func)
+        _lib.call("dibr_b200_mesh_topology_build", dev,
+                  V, F, S, faces, self.corner_ptr, self.corners, self.adj_ptr, self._adj, self.degree, self.weight,
+                  status, ws, nbytes, what=func)
         edges, error = status.tolist()          # the build's one device-to-host read
         if error:
             raise IndexError(f"{func}: faces holds an index outside [0, {V})")
@@ -73,17 +71,16 @@ class _Topology:
         y = torch.empty_like(x)
         V, C = x.shape[-2], x.shape[-1]
         batch = x.numel() // max(V * C, 1)
-        _lib.check(_lib.lib().dibr_b200_laplacian_apply(
-            batch, V, C, _host.ptr(self.adj_ptr), _host.ptr(self._adj), _host.ptr(self.weight), _host.ptr(x),
-            int(transpose), int(smooth), _host.ptr(y), _host.stream_ptr(x.device)), "laplacian_apply")
+        _lib.call("dibr_b200_laplacian_apply", x.device,
+                  batch, V, C, self.adj_ptr, self._adj, self.weight, x, int(transpose), int(smooth), y,
+                  what="laplacian_apply")
         return y
 
     def dense(self, laplacian):
         V = self.num_vertices
         out = torch.empty((V, V), dtype=torch.float32, device=self.faces.device)
-        _lib.check(_lib.lib().dibr_b200_mesh_dense(
-            V, int(laplacian), _host.ptr(self.adj_ptr), _host.ptr(self._adj), _host.ptr(self.weight), _host.ptr(out),
-            _host.stream_ptr(out.device)), "uniform_laplacian" if laplacian else "adjacency_matrix")
+        _lib.call("dibr_b200_mesh_dense", out.device, V, int(laplacian), self.adj_ptr, self._adj, self.weight, out,
+                  what="uniform_laplacian" if laplacian else "adjacency_matrix")
         return out
 
 
@@ -134,9 +131,8 @@ def adjacency_matrix(num_vertices, faces, sparse=True):
         return topo.dense(False)
     E = topo.num_edges
     indices = torch.empty((2, E), dtype=torch.int64, device=faces.device)
-    _lib.check(_lib.lib().dibr_b200_adjacency_coo(
-        topo.num_vertices, E, _host.ptr(topo.adj_ptr), _host.ptr(topo._adj), _host.ptr(indices),
-        _host.stream_ptr(faces.device)), "adjacency_matrix")
+    _lib.call("dibr_b200_adjacency_coo", faces.device, topo.num_vertices, E, topo.adj_ptr, topo._adj, indices,
+              what="adjacency_matrix")
     values = torch.ones(E, dtype=torch.float32, device=faces.device)
     return torch.sparse_coo_tensor(indices, values, (topo.num_vertices, topo.num_vertices))
 
@@ -154,9 +150,8 @@ class _Average(torch.autograd.Function):
         B, F, S, N = face_features.shape
         V = topo.num_vertices
         out = torch.empty((B, V, N), dtype=torch.float32, device=face_features.device)
-        _lib.check(_lib.lib().dibr_b200_vertex_average_forward(
-            B, V, F, S, N, _host.ptr(topo.corner_ptr), _host.ptr(topo.corners), _host.ptr(face_features),
-            _host.ptr(out), _host.stream_ptr(out.device)), "average_face_vertex_features")
+        _lib.call("dibr_b200_vertex_average_forward", out.device,
+                  B, V, F, S, N, topo.corner_ptr, topo.corners, face_features, out, what="average_face_vertex_features")
         ctx.shape = face_features.shape
         return out
 
@@ -166,9 +161,9 @@ class _Average(torch.autograd.Function):
         B, F, S, N = ctx.shape
         grad = grad.contiguous()
         g_ff = torch.empty(ctx.shape, dtype=torch.float32, device=grad.device)
-        _lib.check(_lib.lib().dibr_b200_vertex_average_backward(
-            B, topo.num_vertices, F, S, N, _host.ptr(topo.faces), _host.ptr(topo.corner_ptr), _host.ptr(grad),
-            _host.ptr(g_ff), _host.stream_ptr(grad.device)), "average_face_vertex_features")
+        _lib.call("dibr_b200_vertex_average_backward", grad.device,
+                  B, topo.num_vertices, F, S, N, topo.faces, topo.corner_ptr, grad, g_ff,
+                  what="average_face_vertex_features")
         return g_ff, None
 
 

@@ -297,12 +297,8 @@ class SgShadeB200(Function):
         B, H, W = face_idx.shape
         diffuse, specular, img = (torch.empty((B, H, W, 3), dtype=torch.float32, device=albedo.device)
                                   for _ in range(3))
-        dev = albedo.device
-        with torch.cuda.device(dev):
-            st = _lib.lib().dibr_b200_sg_shade_forward(
-                B, H, W, amplitude.shape[0], _host.ptr(cam), *[_host.ptr(t) for t in ins], _host.ptr(diffuse),
-                _host.ptr(specular), _host.ptr(img), _host.stream_ptr(dev))
-        _lib.check(st, "dibr_b200_sg_shade_forward")
+        _lib.call("dibr_b200_sg_shade_forward", albedo.device,
+                  B, H, W, amplitude.shape[0], cam, *ins, diffuse, specular, img)
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(cam, *ins)
         return diffuse, specular, img
@@ -318,16 +314,11 @@ class SgShadeB200(Function):
         B, H, W = face_idx.shape
         L = amplitude.shape[0]
         dev = albedo.device
-        ws = torch.empty(max(int(_lib.lib().dibr_b200_sg_shade_workspace_bytes(L)) if any(wants[4:]) else 0, 1),
-                         dtype=torch.uint8, device=dev)
+        ws = _lib.scratch(_lib.lib().dibr_b200_sg_shade_workspace_bytes(L) if any(wants[4:]) else 0, dev)
         gouts = [None if g is None else g.contiguous() for g in (g_diffuse, g_specular, g_img)]
-        with torch.cuda.device(dev):
-            st = _lib.lib().dibr_b200_sg_shade_backward(
-                B, H, W, L, _host.ptr(cam), *[_host.ptr(t) for t in (face_idx, albedo, spec_albedo, roughness,
-                                                                     normals, amplitude, direction, sharpness)],
-                *[_host.ptr(g) for g in gouts], *[_host.ptr(g) for g in grads], _host.ptr(ws), ws.numel(),
-                _host.stream_ptr(dev))
-        _lib.check(st, "dibr_b200_sg_shade_backward")
+        _lib.call("dibr_b200_sg_shade_backward", dev,
+                  B, H, W, L, cam, face_idx, albedo, spec_albedo, roughness, normals, amplitude, direction, sharpness,
+                  *gouts, *grads, ws, ws.numel())
         return (None, None) + tuple(grads)
 
 

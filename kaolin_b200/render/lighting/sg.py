@@ -25,10 +25,6 @@ def _c(t):
     return None if t is None else t.contiguous()
 
 
-def _workspace(nbytes, device):
-    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
-
-
 class UnbatchedReducedSgInnerProductB200(Function):
     @staticmethod
     def forward(ctx, amplitude, direction, sharpness, other_amplitude, other_direction, other_sharpness):
@@ -45,12 +41,7 @@ class UnbatchedReducedSgInnerProductB200(Function):
 
 def forward_sg_inner_product(a, d, s, oa, od, os_):
     out = torch.empty_like(a)
-    dev = a.device
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_sg_inner_product_forward(
-            a.shape[0], oa.shape[0], _host.ptr(a), _host.ptr(d), _host.ptr(s), _host.ptr(oa), _host.ptr(od),
-            _host.ptr(os_), _host.ptr(out), _host.stream_ptr(dev))
-    _lib.check(st, "dibr_b200_sg_inner_product_forward")
+    _lib.call("dibr_b200_sg_inner_product_forward", a.device, a.shape[0], oa.shape[0], a, d, s, oa, od, os_, out)
     return out
 
 
@@ -58,13 +49,9 @@ def backward_sg_inner_product(grad_out, a, d, s, oa, od, os_, wants=(True,) * 6)
     """-> [grad_amplitude, grad_direction, grad_sharpness, grad_other_*]; None where not wanted."""
     grads = [torch.empty_like(t) if w else None for t, w in zip((a, d, s, oa, od, os_), wants)]
     dev = a.device
-    ws = _workspace(_lib.lib().dibr_b200_sg_inner_product_workspace_bytes(oa.shape[0]) if any(wants[3:]) else 0, dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().dibr_b200_sg_inner_product_backward(
-            a.shape[0], oa.shape[0], _host.ptr(grad_out), _host.ptr(a), _host.ptr(d), _host.ptr(s), _host.ptr(oa),
-            _host.ptr(od), _host.ptr(os_), *[_host.ptr(g) for g in grads], _host.ptr(ws), ws.numel(),
-            _host.stream_ptr(dev))
-    _lib.check(st, "dibr_b200_sg_inner_product_backward")
+    ws = _lib.scratch(_lib.lib().dibr_b200_sg_inner_product_workspace_bytes(oa.shape[0]) if any(wants[3:]) else 0, dev)
+    _lib.call("dibr_b200_sg_inner_product_backward", dev,
+              a.shape[0], oa.shape[0], grad_out, a, d, s, oa, od, os_, *grads, ws, ws.numel())
     return grads
 
 
@@ -79,11 +66,8 @@ class DiffuseB200(Function):
         L = 1 if model == _lib.LIGHT_SH9 else amplitude.shape[0]
         shape = (N,) if (model == _lib.LIGHT_SH9 and albedo is None) else (N, 3)
         out = torch.empty(shape, dtype=torch.float32, device=normal.device)
-        with torch.cuda.device(normal.device):
-            st = _lib.lib().dibr_b200_diffuse_forward(
-                model, N, L, _host.ptr(amplitude), _host.ptr(direction), _host.ptr(sharpness), _host.ptr(normal),
-                _host.ptr(albedo), _host.ptr(out), _host.stream_ptr(normal.device))
-        _lib.check(st, "dibr_b200_diffuse_forward")
+        _lib.call("dibr_b200_diffuse_forward", normal.device,
+                  model, N, L, amplitude, direction, sharpness, normal, albedo, out)
         ctx.model, ctx.L = model, L
         ctx.save_for_backward(amplitude, direction, sharpness, normal, albedo)
         return out
@@ -97,14 +81,10 @@ class DiffuseB200(Function):
         g_amp, g_dir, g_sharp = new(amplitude, w_amp), new(direction, w_dir), new(sharpness, w_sharp)
         g_n, g_al = new(normal, w_n), new(albedo, w_al)
         wants_light = any(g is not None for g in (g_amp, g_dir, g_sharp))
-        ws = _workspace(_lib.lib().dibr_b200_diffuse_workspace_bytes(ctx.model, ctx.L) if wants_light else 0, dev)
-        with torch.cuda.device(dev):
-            st = _lib.lib().dibr_b200_diffuse_backward(
-                ctx.model, normal.shape[0], ctx.L, _host.ptr(amplitude), _host.ptr(direction), _host.ptr(sharpness),
-                _host.ptr(normal), _host.ptr(albedo), _host.ptr(grad_out.contiguous()), _host.ptr(g_n),
-                _host.ptr(g_al), _host.ptr(g_amp), _host.ptr(g_dir), _host.ptr(g_sharp), _host.ptr(ws), ws.numel(),
-                _host.stream_ptr(dev))
-        _lib.check(st, "dibr_b200_diffuse_backward")
+        ws = _lib.scratch(_lib.lib().dibr_b200_diffuse_workspace_bytes(ctx.model, ctx.L) if wants_light else 0, dev)
+        _lib.call("dibr_b200_diffuse_backward", dev,
+                  ctx.model, normal.shape[0], ctx.L, amplitude, direction, sharpness, normal, albedo,
+                  grad_out.contiguous(), g_n, g_al, g_amp, g_dir, g_sharp, ws, ws.numel())
         return None, g_amp, g_dir, g_sharp, g_n, g_al
 
 
@@ -169,11 +149,7 @@ class SpecularB200(Function):
     def forward(ctx, amplitude, direction, sharpness, normal, roughness, view, spec_albedo):
         ins = [_c(t) for t in (amplitude, direction, sharpness, normal, roughness, view, spec_albedo)]
         out = torch.empty_like(ins[3])
-        with torch.cuda.device(out.device):
-            st = _lib.lib().dibr_b200_specular_forward(
-                out.shape[0], ins[0].shape[0], *[_host.ptr(t) for t in ins], _host.ptr(out),
-                _host.stream_ptr(out.device))
-        _lib.check(st, "dibr_b200_specular_forward")
+        _lib.call("dibr_b200_specular_forward", out.device, out.shape[0], ins[0].shape[0], *ins, out)
         ctx.save_for_backward(*ins)
         return out
 
@@ -183,14 +159,11 @@ class SpecularB200(Function):
         wants = ctx.needs_input_grad
         grads = [torch.empty_like(t) if w else None for t, w in zip(ins, wants)]
         dev = ins[3].device
-        ws = _workspace(_lib.lib().dibr_b200_specular_workspace_bytes(ins[0].shape[0]) if any(wants[:3]) else 0, dev)
+        ws = _lib.scratch(_lib.lib().dibr_b200_specular_workspace_bytes(ins[0].shape[0]) if any(wants[:3]) else 0, dev)
         g_amp, g_dir, g_sharp, g_n, g_r, g_v, g_s = grads
-        with torch.cuda.device(dev):
-            st = _lib.lib().dibr_b200_specular_backward(
-                ins[3].shape[0], ins[0].shape[0], *[_host.ptr(t) for t in ins], _host.ptr(grad_out.contiguous()),
-                _host.ptr(g_n), _host.ptr(g_r), _host.ptr(g_v), _host.ptr(g_s), _host.ptr(g_amp), _host.ptr(g_dir),
-                _host.ptr(g_sharp), _host.ptr(ws), ws.numel(), _host.stream_ptr(dev))
-        _lib.check(st, "dibr_b200_specular_backward")
+        _lib.call("dibr_b200_specular_backward", dev,
+                  ins[3].shape[0], ins[0].shape[0], *ins, grad_out.contiguous(),
+                  g_n, g_r, g_v, g_s, g_amp, g_dir, g_sharp, ws, ws.numel())
         return tuple(grads)
 
 

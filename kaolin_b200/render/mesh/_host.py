@@ -1,19 +1,12 @@
 """Host-side plumbing shared by the autograd wrappers: argument checks in the
 style of the reference's C++ wrappers (rasterization.cpp:70-85,
-dibr_soft_mask.cpp:63-82), workspace allocation, and the ctypes calls."""
-import ctypes
-
+dibr_soft_mask.cpp:63-82), workspace allocation, and the library calls."""
 import torch
 
 from ... import _lib
-
-
-def ptr(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def stream_ptr(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+# Pointer and stream arguments for calling an entry point by hand; the tests that assert raw status
+# codes take them from here.
+from ..._lib import ptr, stream_ptr  # noqa: F401
 
 
 def aligned(t):
@@ -147,12 +140,10 @@ def forward(mode, height, width, fvz, fvi, ff, fnz, valid_u8, multiplier, eps,
         return feat, idx, wts, soft, None
     ws = workspace(B, B * F, height, width, dev, knum if soft_on else 0, f64)
     name = "dibr_b200_forward_f64" if f64 else "dibr_b200_forward"
-    with torch.cuda.device(dev):
-        st = getattr(_lib.lib(), name + "_bf16" if bf16 else name)(
-            B, F, height, width, D, ptr(fvz), ptr(fvi), ptr(ff), ptr(fnz), ptr(valid_u8),
-            float(multiplier), float(eps), mode, float(sigmainv), float(boxlen_m), int(knum),
-            ptr(feat), ptr(idx), ptr(wts), ptr(soft), ptr(ws), ws.numel(), stream_ptr(dev))
-    _lib.check(st, name)
+    _lib.call(name + "_bf16" if bf16 else name, dev,
+              B, F, height, width, D, fvz, fvi, ff, fnz, valid_u8,
+              float(multiplier), float(eps), mode, float(sigmainv), float(boxlen_m), int(knum),
+              feat, idx, wts, soft, ws, ws.numel(), what=name)
     return feat, idx, wts, soft, ws
 
 
@@ -163,21 +154,16 @@ def _backward_call(B, F, height, width, D, g_feat, g_soft, face_idx, wts, soft, 
     if g_feat is not None and ff is not None and g_feat.dtype != ff.dtype:
         raise RuntimeError(f"dibr_b200_backward: grad_features is {g_feat.dtype}, face_features is {ff.dtype}")
     if views is not None:
-        with torch.cuda.device(dev):
-            st = _lib.lib().dibr_b200_backward_views(
-                B, F, height, width, D, ptr(g_feat), ptr(g_soft), ptr(face_idx), ptr(wts), ptr(soft),
-                ptr(fvi), ptr(ff), int(bf16), float(multiplier), float(eps), float(sigmainv), float(boxlen_m),
-                int(knum), ptr(g_fvi), ptr(g_ff), ptr(ws), ws_bytes, int(flags), int(views[0]), int(views[1]),
-                stream_ptr(dev))
-        _lib.check(st, "dibr_b200_backward_views")
+        _lib.call("dibr_b200_backward_views", dev,
+                  B, F, height, width, D, g_feat, g_soft, face_idx, wts, soft,
+                  fvi, ff, int(bf16), float(multiplier), float(eps), float(sigmainv), float(boxlen_m),
+                  int(knum), g_fvi, g_ff, ws, ws_bytes, int(flags), int(views[0]), int(views[1]))
         return
     name = "dibr_b200_backward_f64" if fvi.dtype == torch.float64 else "dibr_b200_backward"
-    with torch.cuda.device(dev):
-        st = getattr(_lib.lib(), name + "_bf16" if bf16 else name)(
-            B, F, height, width, D, ptr(g_feat), ptr(g_soft), ptr(face_idx), ptr(wts), ptr(soft),
-            ptr(fvi), ptr(ff), float(multiplier), float(eps), float(sigmainv), float(boxlen_m),
-            int(knum), ptr(g_fvi), ptr(g_ff), ptr(ws), ws_bytes, int(flags), stream_ptr(dev))
-    _lib.check(st, name)
+    _lib.call(name + "_bf16" if bf16 else name, dev,
+              B, F, height, width, D, g_feat, g_soft, face_idx, wts, soft,
+              fvi, ff, float(multiplier), float(eps), float(sigmainv), float(boxlen_m),
+              int(knum), g_fvi, g_ff, ws, ws_bytes, int(flags), what=name)
 
 
 def backward(height, width, g_feat, g_soft, face_idx, wts, soft, fvi, ff, multiplier, eps,

@@ -38,11 +38,7 @@ class PrepareVerticesB200(Function):
         fvc = torch.empty((B, F, 3, 3), dtype=torch.float32, device=v.device)
         fvi = torch.empty((B, F, 3, 2), dtype=torch.float32, device=v.device)
         fn = torch.empty((B, F, 3), dtype=torch.float32, device=v.device)
-        with torch.cuda.device(v.device):
-            st = _lib.lib().dibr_b200_prepare_vertices_forward(
-                B, V, F, _host.ptr(v), _host.ptr(f), _host.ptr(T), _host.ptr(R), _host.ptr(t), proj,
-                _host.ptr(fvc), _host.ptr(fvi), _host.ptr(fn), _host.stream_ptr(v.device))
-        _lib.check(st, "dibr_b200_prepare_vertices_forward")
+        _lib.call("dibr_b200_prepare_vertices_forward", v.device, B, V, F, v, f, T, R, t, proj, fvc, fvi, fn)
         ctx.save_for_backward(v, f, T, R, t)
         ctx.proj = proj
         return fvc, fvi, fn
@@ -55,12 +51,8 @@ class PrepareVerticesB200(Function):
         c = lambda g: None if g is None else g.contiguous()
         g_fvc, g_fvi, g_fn = c(g_fvc), c(g_fvi), c(g_fn)
         g_vc = torch.empty((B, V, 3), dtype=torch.float32, device=v.device)
-        with torch.cuda.device(v.device):
-            st = _lib.lib().dibr_b200_prepare_vertices_backward(
-                B, V, F, _host.ptr(v), _host.ptr(f), _host.ptr(T), _host.ptr(R), _host.ptr(t), ctx.proj,
-                _host.ptr(g_fvc), _host.ptr(g_fvi), _host.ptr(g_fn), _host.ptr(g_vc),
-                _host.stream_ptr(v.device))
-        _lib.check(st, "dibr_b200_prepare_vertices_backward")
+        _lib.call("dibr_b200_prepare_vertices_backward", v.device,
+                  B, V, F, v, f, T, R, t, ctx.proj, g_fvc, g_fvi, g_fn, g_vc)
         # the camera map is linear: back through it with library GEMMs ((B,V,3) x (3,3))
         g_v = g_T = g_R = g_t = None
         if T is not None:
@@ -120,11 +112,7 @@ class TextureMappingB200(Function):
         B, C, Ht, Wt = tex.shape
         N = uv.numel() // (2 * B)
         out = torch.empty((B, N, C), dtype=torch.float32, device=uv.device)
-        with torch.cuda.device(uv.device):
-            st = _lib.lib().dibr_b200_texture_mapping_forward(
-                B, N, C, Ht, Wt, _host.ptr(uv), _host.ptr(tex), int(nearest), _host.ptr(out),
-                _host.stream_ptr(uv.device))
-        _lib.check(st, "dibr_b200_texture_mapping_forward")
+        _lib.call("dibr_b200_texture_mapping_forward", uv.device, B, N, C, Ht, Wt, uv, tex, int(nearest), out)
         ctx.save_for_backward(uv, tex)
         ctx.nearest = int(nearest)
         return out
@@ -136,11 +124,8 @@ class TextureMappingB200(Function):
         N = uv.numel() // (2 * B)
         g_tex = torch.empty_like(tex) if ctx.needs_input_grad[1] else None
         g_uv = torch.empty_like(uv) if ctx.needs_input_grad[0] else None
-        with torch.cuda.device(uv.device):
-            st = _lib.lib().dibr_b200_texture_mapping_backward(
-                B, N, C, Ht, Wt, _host.ptr(uv), _host.ptr(tex), ctx.nearest, _host.ptr(g_out.contiguous()),
-                _host.ptr(g_tex), _host.ptr(g_uv), _host.stream_ptr(uv.device))
-        _lib.check(st, "dibr_b200_texture_mapping_backward")
+        _lib.call("dibr_b200_texture_mapping_backward", uv.device,
+                  B, N, C, Ht, Wt, uv, tex, ctx.nearest, g_out.contiguous(), g_tex, g_uv)
         return g_uv, g_tex, None
 
 

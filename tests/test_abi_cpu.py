@@ -1,7 +1,8 @@
 """CPU-side checks of the boundary: the C-ABI library loads and exports every
 symbol include/dibr_b200.h declares, argument errors are detected on the host
-without a GPU, the Python layer mirrors the reference signatures and refuses to
-run without CUDA (no CPU fallback)."""
+without a GPU, the Python layer mirrors the reference signatures, calls the
+library through one helper and refuses to run without CUDA (no CPU fallback)."""
+import ast
 import ctypes
 import inspect
 import os
@@ -151,6 +152,31 @@ def test_product_never_imports_the_oracle():
                 src = open(os.path.join(dirpath, f)).read()
                 assert "import oracle" not in src and "from oracle" not in src, f
                 assert "oracle/" not in src.replace("tests/", ""), f
+
+
+def test_library_is_called_only_through_lib_call():
+    """Work is enqueued only through ``_lib.call``, which makes the tensors' device current, passes
+    its stream and checks the status.  Elsewhere in the package the library is asked only for sizes,
+    its version and traces, and no stream or pointer is converted by hand."""
+    pkg = os.path.join(ROOT, "kaolin_b200")
+    query = re.compile(r"dibr_b200_(\w*workspace_bytes\w*|version|trace_begin|trace_end)$")
+    found = []
+    for dirpath, _, files in os.walk(pkg):
+        for f in files:
+            path = os.path.join(dirpath, f)
+            if not f.endswith(".py") or path == os.path.join(pkg, "_lib.py"):
+                continue
+            for node in ast.walk(ast.parse(open(path).read(), path)):
+                where = f"{os.path.relpath(path, ROOT)}:{getattr(node, 'lineno', '?')}"
+                if isinstance(node, ast.Attribute) and node.attr == "cuda_stream":
+                    found.append(f"{where}: .cuda_stream")
+                if isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute):
+                    name, owner = node.func.attr, node.func.value
+                    if name.startswith("dibr_b200_") and not query.match(name):
+                        found.append(f"{where}: {name}()")
+                    if name == "c_void_p" and isinstance(owner, ast.Name) and owner.id == "ctypes":
+                        found.append(f"{where}: ctypes.c_void_p()")
+    assert not found, "\n".join(found)
 
 
 def test_hit_cache_sizing_policy():
