@@ -46,6 +46,16 @@ def check_tensors(func, named, dtype=torch.float32):
     return dev
 
 
+def check_float32(func, named):
+    """Every tensor is float32.  ``check_tensors`` lets integer and bool tensors through (index
+    arguments share its lists); the kernels read these arguments as ``float``, so a tensor of any
+    other element type must not reach them."""
+    for name, t in named:
+        if t is not None and t.dtype != torch.float32:
+            raise RuntimeError(f"\"{func}\" not implemented for '{str(t.dtype).replace('torch.', '')}' "
+                               f"({name}: kaolin_b200 reads it as float32)")
+
+
 def check_size(func, name, t, shape):
     if tuple(t.shape) != tuple(shape):
         raise RuntimeError(f"{func}: expected {name} of size {list(shape)}, got {list(t.shape)}")

@@ -27,6 +27,9 @@ def _proj3(camera_proj):
 class PrepareVerticesB200(Function):
     @staticmethod
     def forward(ctx, vertices, faces, camera_proj, camera_rot, camera_trans, camera_transform):
+        # an output the loss does not use arrives in backward as None (a NULL pointer: the kernel
+        # skips that branch) instead of a tensor of zeros it would read and multiply through
+        ctx.set_materialize_grads(False)
         v = vertices.contiguous()
         f = faces.contiguous()
         B, V = v.shape[0], v.shape[1]
@@ -38,9 +41,11 @@ class PrepareVerticesB200(Function):
         fvc = torch.empty((B, F, 3, 3), dtype=torch.float32, device=v.device)
         fvi = torch.empty((B, F, 3, 2), dtype=torch.float32, device=v.device)
         fn = torch.empty((B, F, 3), dtype=torch.float32, device=v.device)
-        _lib.call("dibr_b200_prepare_vertices_forward", v.device, B, V, F, v, f, T, R, t, proj, fvc, fvi, fn)
+        if F:       # an empty mesh has empty outputs (and no storage to point the kernel at)
+            _lib.call("dibr_b200_prepare_vertices_forward", v.device, B, V, F, v, f, T, R, t, proj, fvc, fvi, fn)
         ctx.save_for_backward(v, f, T, R, t)
         ctx.proj = proj
+        ctx.trans_shape = None if camera_trans is None else camera_trans.shape     # (B, 3) or (B, 1, 3)
         return fvc, fvi, fn
 
     @staticmethod
@@ -50,9 +55,10 @@ class PrepareVerticesB200(Function):
         F = f.shape[0]
         c = lambda g: None if g is None else g.contiguous()
         g_fvc, g_fvi, g_fn = c(g_fvc), c(g_fvi), c(g_fn)
-        g_vc = torch.empty((B, V, 3), dtype=torch.float32, device=v.device)
-        _lib.call("dibr_b200_prepare_vertices_backward", v.device,
-                  B, V, F, v, f, T, R, t, ctx.proj, g_fvc, g_fvi, g_fn, g_vc)
+        g_vc = (torch.empty if F else torch.zeros)((B, V, 3), dtype=torch.float32, device=v.device)
+        if F:
+            _lib.call("dibr_b200_prepare_vertices_backward", v.device,
+                      B, V, F, v, f, T, R, t, ctx.proj, g_fvc, g_fvi, g_fn, g_vc)
         # the camera map is linear: back through it with library GEMMs ((B,V,3) x (3,3))
         g_v = g_T = g_R = g_t = None
         if T is not None:
@@ -67,7 +73,7 @@ class PrepareVerticesB200(Function):
             if ctx.needs_input_grad[3]:
                 g_R = g_vc.transpose(1, 2) @ (v - t.view(B, 1, 3))
             if ctx.needs_input_grad[4]:
-                g_t = -g_d.sum(dim=1)
+                g_t = -g_d.sum(dim=1).view(ctx.trans_shape)
         return g_v, None, None, g_R, g_t, g_T
 
 
@@ -79,6 +85,15 @@ def prepare_vertices(vertices, faces, camera_proj, camera_rot=None, camera_trans
     Returns ``(face_vertices_camera (B,F,3,3), face_vertices_image (B,F,3,2), face_normals (B,F,3))``.
     Gradients flow to ``vertices`` and to the camera transform / rotation / translation;
     ``camera_proj`` is treated as a constant.
+
+    ``vertices`` and the camera tensors must be float32 and ``faces`` int64; any other element
+    type, integer and bool included, raises.  ``camera_trans`` may be (B, 3) or (B, 1, 3).
+    A face of zero area ((a, a, b), three collinear vertices) gets the normal 0 and, as the
+    reference's ``norm`` subgradient does, passes no normal gradient to its vertices.  A vertex
+    on the camera plane (z = 0) gives inf / NaN image coordinates on the faces that use it, as in
+    the reference, and on no other face.  The entries of ``faces`` are not range-checked: an index
+    outside [0, num_vertices) is read as it is (``kaolin_b200.ops.mesh`` raises IndexError for the
+    same mistake, at the cost of a host synchronisation this call does not make).
     """
     if camera_transform is None:
         assert camera_trans is not None and camera_rot is not None, \
@@ -88,6 +103,9 @@ def prepare_vertices(vertices, faces, camera_proj, camera_rot=None, camera_trans
             "camera_trans and camera_rot must be None when camera_transform is defined"
     _host.check_tensors("prepare_vertices", [("vertices", vertices), ("faces", faces),
                                              ("camera_rot", camera_rot), ("camera_trans", camera_trans),
+                                             ("camera_transform", camera_transform)])
+    _host.check_float32("prepare_vertices", [("vertices", vertices), ("camera_rot", camera_rot),
+                                             ("camera_trans", camera_trans),
                                              ("camera_transform", camera_transform)])
     if vertices.dim() != 3 or vertices.shape[-1] != 3:
         raise RuntimeError("prepare_vertices: vertices must be of shape (batch_size, num_vertices, 3)")
@@ -108,11 +126,14 @@ class TextureMappingB200(Function):
     @staticmethod
     def forward(ctx, texture_coordinates, texture_maps, nearest):
         uv = texture_coordinates.contiguous()
+        if uv.data_ptr() % 8:       # the kernels load (u, v) as one float2; a contiguous view at an odd
+            uv = uv.clone()         # element offset is legal input and is not copied by contiguous()
         tex = texture_maps.contiguous()
         B, C, Ht, Wt = tex.shape
         N = uv.numel() // (2 * B)
         out = torch.empty((B, N, C), dtype=torch.float32, device=uv.device)
-        _lib.call("dibr_b200_texture_mapping_forward", uv.device, B, N, C, Ht, Wt, uv, tex, int(nearest), out)
+        if N:       # no points: an empty output (and no storage to point the kernel at)
+            _lib.call("dibr_b200_texture_mapping_forward", uv.device, B, N, C, Ht, Wt, uv, tex, int(nearest), out)
         ctx.save_for_backward(uv, tex)
         ctx.nearest = int(nearest)
         return out
@@ -124,8 +145,11 @@ class TextureMappingB200(Function):
         N = uv.numel() // (2 * B)
         g_tex = torch.empty_like(tex) if ctx.needs_input_grad[1] else None
         g_uv = torch.empty_like(uv) if ctx.needs_input_grad[0] else None
-        _lib.call("dibr_b200_texture_mapping_backward", uv.device,
-                  B, N, C, Ht, Wt, uv, tex, ctx.nearest, g_out.contiguous(), g_tex, g_uv)
+        if N:
+            _lib.call("dibr_b200_texture_mapping_backward", uv.device,
+                      B, N, C, Ht, Wt, uv, tex, ctx.nearest, g_out.contiguous(), g_tex, g_uv)
+        elif g_tex is not None:
+            g_tex.zero_()
         return g_uv, g_tex, None
 
 
@@ -133,10 +157,21 @@ def texture_mapping(texture_coordinates, texture_maps, mode='nearest'):
     r"""Interpolates ``texture_maps`` (B,C,h',w') at dense (B,h,w,2) or sparse (B,N,2) OpenGL texture
     coordinates in [0,1] (kaolin.render.mesh.utils.texture_mapping, utils.py:22-79): clamp,
     y flip, ``grid_sample(align_corners=False, padding_mode='border')``.  ``mode``: 'nearest'
-    or 'bilinear'.  Returns (B,h,w,C) or (B,N,C)."""
+    or 'bilinear'.  Returns (B,h,w,C) or (B,N,C).
+
+    Both arguments must be float32; any other element type, integer and bool included, raises.
+    'nearest' rounds half to even, as ``grid_sample`` does, and gives the coordinates a zero
+    gradient.  In 'bilinear' the coordinate gradient is zero where the clamp to [0, 1] or the
+    border clip acts: outside the open interval (0, 1) and within half a texel of either edge.
+    +-inf clamp like any other value.  One deliberate difference from the reference: a NaN
+    coordinate is read as 0 (u: the leftmost column, v: the bottom row) and gets a zero gradient,
+    where ``grid_sample`` propagates the NaN and what it then samples differs between its CPU and
+    CUDA kernels and between forward and backward."""
     if mode not in ('nearest', 'bilinear'):
         raise ValueError(f"texture_mapping: mode must be 'nearest' or 'bilinear', got '{mode}'")
     _host.check_tensors("texture_mapping", [("texture_coordinates", texture_coordinates),
+                                            ("texture_maps", texture_maps)])
+    _host.check_float32("texture_mapping", [("texture_coordinates", texture_coordinates),
                                             ("texture_maps", texture_maps)])
     if texture_maps.dim() != 4 or texture_coordinates.shape[-1] != 2 \
             or texture_coordinates.shape[0] != texture_maps.shape[0]:
