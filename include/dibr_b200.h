@@ -568,6 +568,58 @@ int dibr_b200_adjacency_coo(int num_vertices, int64_t num_edges, const int32_t* 
                             int64_t* indices, dibr_b200_stream_t stream);
 
 /*
+ * One level of Loop subdivision (kaolin/ops/mesh/trianglemesh.py:482-612, subdivide_trianglemesh) for
+ * a triangle mesh of V vertices and F faces (F, 3) int64, on top of its topology
+ * (dibr_b200_mesh_topology_build with face_size 3).  The reference's unique edges in lexicographic
+ * order are the adjacency entries (i, j) with j >= i, in CSR order; edge e becomes vertex V + e.
+ * dibr_b200_loop_subdivision_build writes, in caller-owned buffers:
+ *   edge_ptr (V+1) int32          exclusive scan over rows of the number of neighbours j >= i;
+ *                                 edge_ptr[V] = E, the edge count (E <= 3F)
+ *   adj_edge (2*F*3) int32        the edge id of every adjacency entry (first adj_ptr[V] used)
+ *   face_edge (F, 3) int32        the ids of edges (f0,f1), (f1,f2), (f2,f0) of each face (the
+ *                                 reference's inverse_indices)
+ *   edges (3F, 4) int32           first E rows: {a, b, f0, f1}, a <= b the endpoints; f0 <= f1 the
+ *                                 faces of its two face edges when it has exactly two, else -1, -1
+ *   new_faces (4F, 3) int64       the next level's faces: for each face, in face order,
+ *                                 (v0, v1, v2, V+e01, V+e12, V+e20)[[1,4,3], [0,3,5], [2,5,4], [5,3,4]]
+ *   status (1) int32              E.  Read it to size the next level; nothing else has to come back.
+ * Needs workspace >= dibr_b200_loop_subdivision_workspace_bytes(); no atomics, deterministic.  When the
+ * topology build reported an index outside [0, V), the outputs are not usable.
+ *
+ * dibr_b200_loop_subdivision_forward: vertices (batch, V, 3) f32 -> out (batch, V + E, 3), one thread
+ * per output vertex, reading vertices only (the odd vertices use the input, not the updated ones):
+ *   even i   (1 - a_i) x_i + (a_i / n_i) sum_{j in N(i)} x_j      n_i = the degree, self-loop included
+ *   odd e    two faces: (both faces' 3 vertices + both endpoints) / 8; otherwise (x_a + x_b) / 2
+ * alpha NULL: a_i = the reference's default weight _get_alpha(n_i) * n_i in fp32 (NaN for n_i = 0).
+ * alpha (batch, V) f32: a_i = alpha[b, i]; alpha_out (batch, V + E) or NULL gets the next level's
+ * alpha: alpha[b, i] for even rows, the odd stencils over alpha for odd rows.
+ *
+ * dibr_b200_loop_subdivision_backward: the transpose, one thread per input vertex, as gathers over the
+ * same structures (adjacency entries: neighbours and edge endpoints; corners -> face_edge: the 1/8 face
+ * terms of two-face edges).  grad_out (batch, V + E, 3); grad_alpha_out (batch, V + E) or NULL (zero);
+ * grad_vertices (batch, V, 3) or NULL; grad_alpha (batch, V) or NULL, which needs alpha and vertices:
+ *   grad_alpha_i = (g_i . sum_{j in N(i)} x_j) / n_i - g_i . x_i + the gradient through alpha_out,
+ *   the first two terms in fp64 (they nearly cancel on a smooth surface).
+ * No atomics: every output is bit-reproducible.
+ */
+size_t dibr_b200_loop_subdivision_workspace_bytes(int num_vertices, int64_t num_faces);
+int dibr_b200_loop_subdivision_build(int num_vertices, int64_t num_faces, const int64_t* faces,
+                                     const int32_t* corner_ptr, const int32_t* corners, const int32_t* adj_ptr,
+                                     const int32_t* adj, int32_t* edge_ptr, int32_t* adj_edge, int32_t* face_edge,
+                                     int32_t* edges, int64_t* new_faces, int32_t* status, void* workspace,
+                                     size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_loop_subdivision_forward(int batch, int num_vertices, int num_edges, const int32_t* adj_ptr,
+                                       const int32_t* adj, const int32_t* edges, const int64_t* faces,
+                                       const float* vertices, const float* alpha, float* out, float* alpha_out,
+                                       dibr_b200_stream_t stream);
+int dibr_b200_loop_subdivision_backward(int batch, int num_vertices, int num_edges, const int32_t* corner_ptr,
+                                        const int32_t* corners, const int32_t* adj_ptr, const int32_t* adj,
+                                        const int32_t* adj_edge, const int32_t* face_edge, const int32_t* edges,
+                                        const float* vertices, const float* alpha, const float* grad_out,
+                                        const float* grad_alpha_out, float* grad_vertices, float* grad_alpha,
+                                        dibr_b200_stream_t stream);
+
+/*
  * Exchange step of the view-sharded path (SURVEY.md 8e; kaolin_b200/csrc/peer_push.cu): the
  * reference has no multi-GPU code - its callers all-gather the per-view gradients with
  * torch.distributed.  All-gather by STORES over NVLink: copies `bytes` (multiple of 16) from the

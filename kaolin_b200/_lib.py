@@ -109,6 +109,11 @@ SIGNATURES = {
     "dibr_b200_vertex_average_backward": (_i, [_i, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "dibr_b200_mesh_dense": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp]),
     "dibr_b200_adjacency_coo": (_i, [_i, _i64, _vp, _vp, _vp, _vp]),
+    # Loop subdivision (ops.mesh.subdivide_trianglemesh, LoopSubdivision; csrc/mesh_topology.cu)
+    "dibr_b200_loop_subdivision_workspace_bytes": (_sz, [_i, _i64]),
+    "dibr_b200_loop_subdivision_build": (_i, [_i, _i64] + [_vp] * 11 + [_vp, _sz, _vp]),
+    "dibr_b200_loop_subdivision_forward": (_i, [_i, _i, _i] + [_vp] * 8 + [_vp]),
+    "dibr_b200_loop_subdivision_backward": (_i, [_i, _i, _i] + [_vp] * 13 + [_vp]),
 }
 
 

@@ -429,6 +429,262 @@ __global__ void __launch_bounds__(kThreads) adjacency_coo_kernel(int V, int64_t 
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Loop subdivision (kaolin.ops.mesh.subdivide_trianglemesh), one level on top of the topology of a
+// triangle mesh.  The reference's unique edges, in lexicographic order, are the adjacency entries
+// (i, j) with j >= i in CSR order, so edge ids are a scan over rows of the number of such entries:
+// the entry at position p of row a has the id p + edge_ptr[a + 1] - adj_ptr[a + 1].  Edge e becomes
+// vertex V + e; edges[e] = {a, b, f0, f1} with a <= b, and f0 <= f1 the faces of its two face edges
+// when it has exactly two, f0 = f1 = -1 for any other count.
+struct Subdiv {
+  int V, F;
+  const int64_t* faces;
+  const int* corner_ptr; const int* corners; const int* adj_ptr; const int* adj;
+  int* count; int* edge_ptr; int* adj_edge; int* face_edge; int4* edges; int64_t* new_faces;
+};
+
+__device__ __forceinline__ int lower_bound_row(const int* __restrict__ adj, int lo, int hi, int key) {
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(adj + mid) < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// The id of edge (a, b), a <= b both in [0, V); -1 when b is not a neighbour of a.
+__device__ __forceinline__ int edge_id(const Subdiv& s, int a, int b) {
+  const int e1 = __ldg(s.adj_ptr + a + 1);
+  const int p = lower_bound_row(s.adj, __ldg(s.adj_ptr + a), e1, b);
+  return p < e1 && __ldg(s.adj + p) == b ? p + s.edge_ptr[a + 1] - e1 : -1;
+}
+
+// count[i] = the number of neighbours j >= i of row i.
+__global__ void __launch_bounds__(kThreads) subdiv_count_kernel(Subdiv s) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= s.V) return;
+  const int e1 = __ldg(s.adj_ptr + i + 1);
+  s.count[i] = e1 - lower_bound_row(s.adj, __ldg(s.adj_ptr + i), e1, i);
+}
+
+// One thread per adjacency entry (i, j): its edge id, and for j >= i the edge record.  The face edges
+// (f, k) of edge (i, j) are found among the corners of i: corner k of f starts face edge k, whose
+// other end is faces[f, k+1], and ends face edge k-1, whose other end is faces[f, k-1] (counted there
+// only when j != i, so that a self-loop's face edge is counted once).  Entries naming a vertex outside
+// [0, V) exist only when the topology build reported an error; they get id -1.
+__global__ void __launch_bounds__(kThreads) subdiv_edges_kernel(Subdiv s, int64_t capacity) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= capacity) return;
+  const int p = (int)q, V = s.V;
+  if (p >= __ldg(s.adj_ptr + V)) return;
+  int lo = 0, hi = V + 1;                       // the row of p: the last i with adj_ptr[i] <= p
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(s.adj_ptr + mid) <= p) lo = mid + 1; else hi = mid;
+  }
+  const int i = lo - 1, j = __ldg(s.adj + p);
+  if (!valid_vertex(j, V)) { s.adj_edge[p] = -1; return; }
+  if (j < i) { s.adj_edge[p] = edge_id(s, j, i); return; }
+  const int id = p + s.edge_ptr[i + 1] - __ldg(s.adj_ptr + i + 1);
+  s.adj_edge[p] = id;
+  int n = 0, f0 = -1, f1 = -1;
+  for (int c = __ldg(s.corner_ptr + i), c1 = __ldg(s.corner_ptr + i + 1); c < c1; ++c) {
+    const int corner = __ldg(s.corners + c), f = corner / 3, k = corner - 3 * f;
+    const int64_t* row = s.faces + 3 * (int64_t)f;
+    const int m = (__ldg(row + (k == 2 ? 0 : k + 1)) == j) + (j != i && __ldg(row + (k == 0 ? 2 : k - 1)) == j);
+    for (int u = 0; u < m; ++u, ++n) {
+      if (n == 0) f0 = f;
+      else if (n == 1) f1 = f;
+    }
+  }
+  if (n != 2) f0 = f1 = -1;
+  else if (f1 < f0) { const int t = f0; f0 = f1; f1 = t; }
+  s.edges[id] = make_int4(i, j, f0, f1);
+}
+
+// One thread per face: the ids of its edges (f0,f1), (f1,f2), (f2,f0) and its four child faces
+// (v0, v1, v2, V+e01, V+e12, V+e20)[[1,4,3], [0,3,5], [2,5,4], [5,3,4]].
+__global__ void __launch_bounds__(kThreads) subdiv_faces_kernel(Subdiv s) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= s.F) return;
+  const int64_t* row = s.faces + 3 * (int64_t)f;
+  int64_t v[6];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) v[k] = __ldg(row + k);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const int64_t a = v[k] < v[k == 2 ? 0 : k + 1] ? v[k] : v[k == 2 ? 0 : k + 1];
+    const int64_t b = v[k] < v[k == 2 ? 0 : k + 1] ? v[k == 2 ? 0 : k + 1] : v[k];
+    const int e = valid_vertex(a, s.V) && valid_vertex(b, s.V) ? edge_id(s, (int)a, (int)b) : -1;
+    s.face_edge[3 * f + k] = e;
+    v[3 + k] = (int64_t)s.V + e;
+  }
+  constexpr int kChild[12] = {1, 4, 3, 0, 3, 5, 2, 5, 4, 5, 3, 4};
+  int64_t* out = s.new_faces + 12 * (int64_t)f;
+#pragma unroll
+  for (int u = 0; u < 12; ++u) out[u] = v[kChild[u]];
+}
+
+struct SubdivLayout {
+  size_t count, sums, bytes;
+};
+
+SubdivLayout subdiv_layout(int V) {
+  SubdivLayout l;
+  const size_t tiles = (size_t)(V + kScanTile - 1) / kScanTile + 1;
+  l.count = 0;
+  l.sums = align_up(sizeof(int) * (size_t)V, 256);
+  l.bytes = l.sums + align_up(sizeof(int) * tiles, 256);
+  return l;
+}
+
+// The reference's default weight of a vertex of n neighbours, _get_alpha(n) * n, in its fp32 steps:
+// torch evaluates 2*pi / n as reciprocal(n) * 2*pi.  n = 0 gives NaN.
+__device__ __forceinline__ float default_alpha(int deg) {
+  const float n = (float)deg;
+  const float c = __fadd_rn(0.375f, __fmul_rn(0.25f, cosf(__fmul_rn(1.0f / n, 6.28318530717958648f))));
+  const float a = deg == 3 ? 0.1875f : __fsub_rn(0.625f, __fmul_rn(c, c)) / n;
+  return __fmul_rn(a, n);
+}
+
+// One thread per output vertex (view b, row r < V + E):
+//   r < V  even:  (1 - a_r) x_r + (a_r / n_r) sum_{j in N(r)} x_j
+//   r >= V odd, edge e = r - V = (a, b):  two faces: (sum of both faces' vertices + x_a + x_b) / 8,
+//          otherwise (x_a + x_b) / 2.
+// ALPHA: a is the given (B, V) alpha, and alpha_out (if not NULL) gets the next level's alpha: a_r for
+// even rows, the odd stencil over a for odd rows.  Otherwise a is default_alpha(n).
+template <bool ALPHA>
+__global__ void __launch_bounds__(kThreads) subdiv_forward_kernel(int64_t total, int V, int E,
+                                                                  const int* __restrict__ adj_ptr,
+                                                                  const int* __restrict__ adj,
+                                                                  const int4* __restrict__ edges,
+                                                                  const int64_t* __restrict__ faces,
+                                                                  const float* __restrict__ x,
+                                                                  const float* __restrict__ alpha,
+                                                                  float* __restrict__ y, float* __restrict__ alpha_out) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int W = V + E;
+  const int64_t b = t / W;
+  const int r = (int)(t - b * W);
+  const float* xb = x + b * V * 3;
+  const float* ab = ALPHA ? alpha + b * V : nullptr;
+  float o0, o1, o2, oa = 0.f;
+  if (r < V) {
+    const int p0 = __ldg(adj_ptr + r), p1 = __ldg(adj_ptr + r + 1);
+    float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+    for (int p = p0; p < p1; ++p) {
+      const float* xj = xb + 3 * (int64_t)__ldg(adj + p);
+      s0 += __ldg(xj); s1 += __ldg(xj + 1); s2 += __ldg(xj + 2);
+    }
+    const float a = ALPHA ? __ldg(ab + r) : default_alpha(p1 - p0);
+    const float w = a / (float)(p1 - p0), u = 1.0f - a;
+    const float* xr = xb + 3 * (int64_t)r;
+    o0 = u * __ldg(xr) + w * s0; o1 = u * __ldg(xr + 1) + w * s1; o2 = u * __ldg(xr + 2) + w * s2;
+    oa = ALPHA ? a : 0.f;
+  } else {
+    const int4 e = __ldg(edges + (r - V));
+    const float *xa = xb + 3 * (int64_t)e.x, *xe = xb + 3 * (int64_t)e.y;
+    if (e.z < 0) {
+      o0 = (__ldg(xa) + __ldg(xe)) * 0.5f; o1 = (__ldg(xa + 1) + __ldg(xe + 1)) * 0.5f;
+      o2 = (__ldg(xa + 2) + __ldg(xe + 2)) * 0.5f;
+      if (ALPHA) oa = (__ldg(ab + e.x) + __ldg(ab + e.y)) * 0.5f;
+    } else {
+      int64_t v[8];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        v[k] = __ldg(faces + 3 * (int64_t)e.z + k);
+        v[3 + k] = __ldg(faces + 3 * (int64_t)e.w + k);
+      }
+      v[6] = e.x; v[7] = e.y;
+      o0 = o1 = o2 = 0.f;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float* xv = xb + 3 * v[k];
+        o0 += __ldg(xv); o1 += __ldg(xv + 1); o2 += __ldg(xv + 2);
+        if (ALPHA) oa += __ldg(ab + v[k]);
+      }
+      o0 *= 0.125f; o1 *= 0.125f; o2 *= 0.125f; oa *= 0.125f;
+    }
+  }
+  float* yr = y + 3 * t;
+  yr[0] = o0; yr[1] = o1; yr[2] = o2;
+  if (ALPHA && alpha_out) alpha_out[t] = oa;
+}
+
+// One thread per input vertex (view b, row j): the transpose of the forward, as a gather.
+//   even self term   (1 - a_j) g_j
+//   even neighbours  sum_{i in N(j)} (a_i / n_i) g_i               (the adjacency is symmetric)
+//   edge endpoints   for each entry (j, i): w g_{V+e}, w = 1/8 (two faces) or 1/2, twice for i == j
+//   face terms       for each corner of j in face f, each face edge of f with two faces: 1/8 g_{V+e}
+// ALPHA (given alpha): grad_alpha_j = (g_j . s_j) / n_j - g_j . x_j (in fp64, then rounded), plus the
+// carried alpha's gradient ga_j and the same endpoint and face terms over ga_{V+e}.
+template <bool ALPHA>
+__global__ void __launch_bounds__(kThreads) subdiv_backward_kernel(
+    int64_t total, int V, int E, const int* __restrict__ corner_ptr, const int* __restrict__ corners,
+    const int* __restrict__ adj_ptr, const int* __restrict__ adj, const int* __restrict__ adj_edge,
+    const int* __restrict__ face_edge, const int4* __restrict__ edges, const float* __restrict__ x,
+    const float* __restrict__ alpha, const float* __restrict__ gy, const float* __restrict__ gao,
+    float* __restrict__ gx, float* __restrict__ ga) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int64_t b = t / V;
+  const int j = (int)(t - b * V), W = V + E;
+  const float* gyb = gy + b * W * 3;
+  const float* gab = ALPHA && gao ? gao + b * W : nullptr;
+  const float* xb = x + b * V * 3;
+  const float* ab = ALPHA ? alpha + b * V : nullptr;
+  const int* edge_two = reinterpret_cast<const int*>(edges) + 2;      // f0 of edge e at edge_two[4 e]
+  const bool want_ga = ALPHA && ga;
+  const int p0 = __ldg(adj_ptr + j), p1 = __ldg(adj_ptr + j + 1);
+  const float* gj = gyb + 3 * (int64_t)j;
+  const float gj0 = __ldg(gj), gj1 = __ldg(gj + 1), gj2 = __ldg(gj + 2);
+  float n0 = 0.f, n1 = 0.f, n2 = 0.f;      // even neighbour terms
+  float e0 = 0.f, e1 = 0.f, e2 = 0.f, ea = 0.f;   // edge terms
+  // sum of the neighbours, for grad_alpha, in fp64: (g . s) / n and g . x nearly cancel on a smooth
+  // surface, and the reference's CPU reductions accumulate in double
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+  for (int p = p0; p < p1; ++p) {
+    const int i = __ldg(adj + p);
+    const int q0 = __ldg(adj_ptr + i), q1 = __ldg(adj_ptr + i + 1);
+    const float wi = (ALPHA ? __ldg(ab + i) : default_alpha(q1 - q0)) / (float)(q1 - q0);
+    const float* gi = gyb + 3 * (int64_t)i;
+    n0 += wi * __ldg(gi); n1 += wi * __ldg(gi + 1); n2 += wi * __ldg(gi + 2);
+    if (want_ga) {
+      const float* xi = xb + 3 * (int64_t)i;
+      s0 += __ldg(xi); s1 += __ldg(xi + 1); s2 += __ldg(xi + 2);
+    }
+    const int e = __ldg(adj_edge + p);
+    float w = __ldg(edge_two + 4 * (int64_t)e) < 0 ? 0.5f : 0.125f;
+    if (i == j) w += w;
+    const float* ge = gyb + 3 * ((int64_t)V + e);
+    e0 += w * __ldg(ge); e1 += w * __ldg(ge + 1); e2 += w * __ldg(ge + 2);
+    if (gab) ea += w * __ldg(gab + V + e);
+  }
+  for (int c = __ldg(corner_ptr + j), c1 = __ldg(corner_ptr + j + 1); c < c1; ++c) {
+    const int* fe = face_edge + 3 * (__ldg(corners + c) / 3);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const int e = __ldg(fe + k);
+      if (__ldg(edge_two + 4 * (int64_t)e) < 0) continue;
+      const float* ge = gyb + 3 * ((int64_t)V + e);
+      e0 += 0.125f * __ldg(ge); e1 += 0.125f * __ldg(ge + 1); e2 += 0.125f * __ldg(ge + 2);
+      if (gab) ea += 0.125f * __ldg(gab + V + e);
+    }
+  }
+  const float aj = ALPHA ? __ldg(ab + j) : default_alpha(p1 - p0);
+  if (gx) {
+    const float u = 1.0f - aj;
+    float* o = gx + 3 * t;
+    o[0] = u * gj0 + n0 + e0; o[1] = u * gj1 + n1 + e1; o[2] = u * gj2 + n2 + e2;
+  }
+  if (want_ga) {
+    const float* xj = xb + 3 * (int64_t)j;
+    const double gs = (double)gj0 * s0 + (double)gj1 * s1 + (double)gj2 * s2;
+    const double gv = (double)gj0 * __ldg(xj) + (double)gj1 * __ldg(xj + 1) + (double)gj2 * __ldg(xj + 2);
+    ga[t] = (float)(gs / (double)(p1 - p0) - gv) + (gab ? __ldg(gab + j) : 0.f) + ea;
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -565,6 +821,96 @@ int dibr_b200_adjacency_coo(int num_vertices, int64_t num_edges, const int32_t* 
   Span s("adjacency_coo_kernel", st);
   adjacency_coo_kernel<<<grid_for(32 * (int64_t)num_vertices, kThreads), kThreads, 0, st>>>(num_vertices, num_edges,
                                                                                             adj_ptr, adj, indices);
+  return (int)cudaGetLastError();
+}
+
+size_t dibr_b200_loop_subdivision_workspace_bytes(int num_vertices, int64_t num_faces) {
+  if (topo_dims(num_vertices, num_faces, 3)) return 0;
+  return subdiv_layout(num_vertices).bytes;
+}
+
+int dibr_b200_loop_subdivision_build(int num_vertices, int64_t num_faces, const int64_t* faces,
+                                     const int32_t* corner_ptr, const int32_t* corners, const int32_t* adj_ptr,
+                                     const int32_t* adj, int32_t* edge_ptr, int32_t* adj_edge, int32_t* face_edge,
+                                     int32_t* edges, int64_t* new_faces, int32_t* status, void* workspace,
+                                     size_t workspace_bytes, dibr_b200_stream_t stream) {
+  if (const int e = topo_dims(num_vertices, num_faces, 3)) return e;
+  if (!corner_ptr || !adj_ptr || !edge_ptr || !status || !workspace) return DIBR_B200_EINVAL;
+  if (num_faces > 0 && (!faces || !corners || !adj || !adj_edge || !face_edge || !edges || !new_faces))
+    return DIBR_B200_EINVAL;
+  const SubdivLayout l = subdiv_layout(num_vertices);
+  if (workspace_bytes < l.bytes) return DIBR_B200_EWORKSPACE;
+  char* ws = (char*)workspace;
+  Subdiv s;
+  s.V = num_vertices; s.F = (int)num_faces; s.faces = faces;
+  s.corner_ptr = corner_ptr; s.corners = corners; s.adj_ptr = adj_ptr; s.adj = adj;
+  s.count = (int*)(ws + l.count); s.edge_ptr = edge_ptr; s.adj_edge = adj_edge; s.face_edge = face_edge;
+  s.edges = (int4*)edges; s.new_faces = new_faces;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int V = num_vertices;
+  if (V > 0) { Span sp("subdiv_count_kernel", st); subdiv_count_kernel<<<grid_for(V, kThreads), kThreads, 0, st>>>(s); }
+  if (int e = exclusive_scan(s.count, V, (int*)(ws + l.sums), edge_ptr, st)) return e;
+  if (num_faces > 0) {
+    const int64_t capacity = 6 * num_faces;       // the adjacency holds at most 2 * F * 3 entries
+    { Span sp("subdiv_edges_kernel", st); subdiv_edges_kernel<<<grid_for(capacity, kThreads), kThreads, 0, st>>>(s, capacity); }
+    { Span sp("subdiv_faces_kernel", st); subdiv_faces_kernel<<<grid_for(num_faces, kThreads), kThreads, 0, st>>>(s); }
+  }
+  cudaMemcpyAsync(status, edge_ptr + V, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+  return (int)cudaGetLastError();
+}
+
+int dibr_b200_loop_subdivision_forward(int batch, int num_vertices, int num_edges, const int32_t* adj_ptr,
+                                       const int32_t* adj, const int32_t* edges, const int64_t* faces,
+                                       const float* vertices, const float* alpha, float* out, float* alpha_out,
+                                       dibr_b200_stream_t stream) {
+  if (batch < 0 || num_vertices < 0 || num_edges < 0 || (int64_t)num_vertices + num_edges >= INT32_MAX)
+    return DIBR_B200_EINVAL;
+  if (alpha_out && !alpha) return DIBR_B200_EINVAL;
+  const int64_t total = (int64_t)batch * (num_vertices + num_edges);
+  if (total == 0) return 0;
+  if (!adj_ptr || !out || (num_vertices > 0 && !vertices)) return DIBR_B200_EINVAL;
+  if (num_edges > 0 && (!adj || !edges || !faces)) return DIBR_B200_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int4* e4 = (const int4*)edges;
+  if (alpha) {
+    Span s("subdiv_forward_kernel<alpha>", st);
+    subdiv_forward_kernel<true><<<grid_for(total, kThreads), kThreads, 0, st>>>(
+        total, num_vertices, num_edges, adj_ptr, adj, e4, faces, vertices, alpha, out, alpha_out);
+  } else {
+    Span s("subdiv_forward_kernel", st);
+    subdiv_forward_kernel<false><<<grid_for(total, kThreads), kThreads, 0, st>>>(
+        total, num_vertices, num_edges, adj_ptr, adj, e4, faces, vertices, nullptr, out, nullptr);
+  }
+  return (int)cudaGetLastError();
+}
+
+int dibr_b200_loop_subdivision_backward(int batch, int num_vertices, int num_edges, const int32_t* corner_ptr,
+                                        const int32_t* corners, const int32_t* adj_ptr, const int32_t* adj,
+                                        const int32_t* adj_edge, const int32_t* face_edge, const int32_t* edges,
+                                        const float* vertices, const float* alpha, const float* grad_out,
+                                        const float* grad_alpha_out, float* grad_vertices, float* grad_alpha,
+                                        dibr_b200_stream_t stream) {
+  if (batch < 0 || num_vertices < 0 || num_edges < 0 || (int64_t)num_vertices + num_edges >= INT32_MAX)
+    return DIBR_B200_EINVAL;
+  if ((grad_alpha_out || grad_alpha) && !alpha) return DIBR_B200_EINVAL;
+  if (grad_alpha && !vertices) return DIBR_B200_EINVAL;
+  const int64_t total = (int64_t)batch * num_vertices;
+  if (total == 0 || (!grad_vertices && !grad_alpha)) return 0;
+  if (!corner_ptr || !adj_ptr || !grad_out) return DIBR_B200_EINVAL;
+  if (num_edges > 0 && (!corners || !adj || !adj_edge || !face_edge || !edges)) return DIBR_B200_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int4* e4 = (const int4*)edges;
+  if (alpha) {
+    Span s("subdiv_backward_kernel<alpha>", st);
+    subdiv_backward_kernel<true><<<grid_for(total, kThreads), kThreads, 0, st>>>(
+        total, num_vertices, num_edges, corner_ptr, corners, adj_ptr, adj, adj_edge, face_edge, e4, vertices, alpha,
+        grad_out, grad_alpha_out, grad_vertices, grad_alpha);
+  } else {
+    Span s("subdiv_backward_kernel", st);
+    subdiv_backward_kernel<false><<<grid_for(total, kThreads), kThreads, 0, st>>>(
+        total, num_vertices, num_edges, corner_ptr, corners, adj_ptr, adj, adj_edge, face_edge, e4, vertices, nullptr,
+        grad_out, nullptr, grad_vertices, nullptr);
+  }
   return (int)cudaGetLastError();
 }
 

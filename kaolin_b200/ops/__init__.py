@@ -1,2 +1,3 @@
-"""kaolin.ops drop-ins: the mesh Laplacian, adjacency and vertex averaging on sm_90a kernels."""
+"""kaolin.ops drop-ins: the mesh Laplacian, adjacency, vertex averaging and Loop subdivision on sm_90a
+kernels."""
 from . import mesh  # noqa: F401

@@ -12,6 +12,13 @@ builds it once::
     loss = (L @ (vertices - vertices_init)).pow(2).mean()
 
 Deliberate deviation: a face index outside [0, V) raises ``IndexError`` (the reference does not check).
+
+Loop subdivision (trianglemesh.py:482-612) is built on the same topology: ``subdivide_trianglemesh``
+has the reference's signature and builds every level on each call; ``LoopSubdivision`` builds them
+once and applies them with autograd to the vertices and a learnable per-vertex alpha::
+
+    S = LoopSubdivision(V, faces, 2)          # coarse-to-fine DIB-R, or DMTet's learnable alpha
+    fine_vertices = S(vertices, alpha)        # fine faces: S.faces
 """
 import torch
 
@@ -19,7 +26,7 @@ from .. import _lib
 from ..render.mesh import _host
 
 __all__ = ["adjacency_matrix", "uniform_laplacian", "compute_vertex_normals", "average_face_vertex_features",
-           "UniformLaplacian"]
+           "UniformLaplacian", "subdivide_trianglemesh", "LoopSubdivision"]
 
 
 def _check(func, typed):
@@ -33,9 +40,11 @@ def _check(func, typed):
 
 
 class _Topology:
-    """The corner and adjacency CSRs of one mesh (see include/dibr_b200.h)."""
+    """The corner and adjacency CSRs of one mesh (see include/dibr_b200.h).  With ``status`` (an int32
+    CUDA tensor of at least 2 elements) the build writes its status there and the caller reads it and
+    calls ``_finish``; otherwise the constructor reads it."""
 
-    def __init__(self, func, num_vertices, faces):
+    def __init__(self, func, num_vertices, faces, status=None):
         _check(func, [("faces", faces, torch.int64)])
         if faces.dim() != 2 or faces.shape[1] < 3:
             raise RuntimeError(f"{func}: expected faces of shape (num_faces, face_size >= 3), got {list(faces.shape)}")
@@ -55,14 +64,19 @@ class _Topology:
         self._adj = torch.empty(max(2 * F * S, 1), **i32)
         self.degree = torch.empty(V, **i32)
         self.weight = torch.empty(V, dtype=torch.float32, device=dev)
-        status = torch.empty(2, **i32)
+        own = status is None
+        if own:
+            status = torch.empty(2, **i32)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         _lib.call("dibr_b200_mesh_topology_build", dev,
                   V, F, S, faces, self.corner_ptr, self.corners, self.adj_ptr, self._adj, self.degree, self.weight,
                   status, ws, nbytes, what=func)
-        edges, error = status.tolist()          # the build's one device-to-host read
+        if own:
+            self._finish(func, *status.tolist())          # the build's one device-to-host read
+
+    def _finish(self, func, edges, error):
         if error:
-            raise IndexError(f"{func}: faces holds an index outside [0, {V})")
+            raise IndexError(f"{func}: faces holds an index outside [0, {self.num_vertices})")
         self.num_edges = edges
         self.adj = self._adj[:edges]
 
@@ -185,3 +199,152 @@ def compute_vertex_normals(faces, face_normals, num_vertices=None):
     r"""kaolin.ops.mesh.compute_vertex_normals: ``average_face_vertex_features`` of the per-corner
     normals (B, F, S, 3) -> (B, V, 3)."""
     return average_face_vertex_features(faces, face_normals, num_vertices=num_vertices)
+
+
+class _SubdivisionLevel:
+    """One level of Loop subdivision: the topology of (num_vertices, faces), its edges and the next
+    level's faces (see include/dibr_b200.h), built with one device-to-host read, the edge count."""
+
+    def __init__(self, func, num_vertices, faces):
+        V, F = num_vertices, faces.shape[0]
+        dev = faces.device
+        status = torch.empty(3, dtype=torch.int32, device=dev)
+        self.topo = _Topology(func, V, faces, status=status)
+        nbytes = _lib.lib().dibr_b200_loop_subdivision_workspace_bytes(V, F)
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.num_vertices, self.faces = V, self.topo.faces
+        self.edge_ptr = torch.empty(V + 1, **i32)
+        self.adj_edge = torch.empty(max(6 * F, 1), **i32)
+        self.face_edge = torch.empty(max(3 * F, 1), **i32)
+        self.edges = torch.empty((max(3 * F, 1), 4), **i32)
+        self.new_faces = torch.empty((4 * F, 3), dtype=torch.int64, device=dev)
+        ws = _lib.scratch(nbytes, dev)
+        _lib.call("dibr_b200_loop_subdivision_build", dev,
+                  V, F, self.faces, self.topo.corner_ptr, self.topo.corners,
+                  self.topo.adj_ptr, self.topo._adj, self.edge_ptr, self.adj_edge, self.face_edge, self.edges,
+                  self.new_faces, status[2:], ws, nbytes, what=func)
+        adj_entries, error, E = status.tolist()          # the level's one device-to-host read
+        self.topo._finish(func, adj_entries, error)
+        self.num_edges = E
+
+
+class _SubdivideStep(torch.autograd.Function):
+    """One level applied to x (B, V, 3) and alpha (B, V) or None -> y (B, V + E, 3), plus the next
+    level's alpha (B, V + E) when ``carry``."""
+
+    @staticmethod
+    def forward(ctx, x, alpha, level, carry):
+        ctx.set_materialize_grads(False)
+        t = level.topo
+        B, V, E = x.shape[0], level.num_vertices, level.num_edges
+        y = torch.empty((B, V + E, 3), dtype=torch.float32, device=x.device)
+        a_out = torch.empty((B, V + E), dtype=torch.float32, device=x.device) if carry else None
+        _lib.call("dibr_b200_loop_subdivision_forward", x.device,
+                  B, V, E, t.adj_ptr, t._adj, level.edges, level.faces, x, alpha, y, a_out,
+                  what="subdivide_trianglemesh")
+        ctx.level, ctx.shape = level, x.shape
+        need_alpha = alpha is not None and ctx.needs_input_grad[1]
+        ctx.save_for_backward(x if need_alpha else None, alpha)
+        return y if a_out is None else (y, a_out)
+
+    @staticmethod
+    def backward(ctx, grad, grad_alpha=None):
+        x, alpha = ctx.saved_tensors
+        level, t = ctx.level, ctx.level.topo
+        B, V, _ = ctx.shape
+        E = level.num_edges
+        dev = level.faces.device
+        if grad is None:
+            grad = torch.zeros((B, V + E, 3), dtype=torch.float32, device=dev)
+        gx = torch.empty(ctx.shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] else None
+        ga = torch.empty((B, V), dtype=torch.float32, device=dev) if x is not None else None
+        _lib.call("dibr_b200_loop_subdivision_backward", dev,
+                  B, V, E, t.corner_ptr, t.corners, t.adj_ptr, t._adj, level.adj_edge, level.face_edge, level.edges,
+                  x, alpha, grad.contiguous(), None if grad_alpha is None else grad_alpha.contiguous(), gx, ga,
+                  what="subdivide_trianglemesh")
+        return gx, ga, None, None
+
+
+def _check_faces(func, faces):
+    _check(func, [("faces", faces, torch.int64)])
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError(f"{func}: expected triangle faces of shape (num_faces, 3), got {list(faces.shape)}")
+
+
+class LoopSubdivision:
+    r"""Loop subdivision of one triangle mesh, every level built once.
+
+    ``S = LoopSubdivision(num_vertices, faces, iterations)`` builds the topology and the edges of
+    every level; ``S(vertices, alpha=None)`` then computes
+    ``subdivide_trianglemesh(vertices, faces, iterations, alpha)[0]`` with autograd to ``vertices``
+    and ``alpha`` and no host synchronisation, and ``S.faces`` is the final
+    :math:`(F \cdot 4^\text{iterations}, 3)` faces.  ``vertices`` (B, num_vertices, 3) and
+    ``alpha`` (B, num_vertices) are float32 for any B.  Each level is one kernel forward and one
+    backward; no floating-point atomics, so results are bit-reproducible.
+    """
+
+    def __init__(self, num_vertices, faces, iterations):
+        func = "LoopSubdivision"
+        _check_faces(func, faces)
+        V, iterations = int(num_vertices), int(iterations)
+        if V < 0 or iterations < 0:
+            raise ValueError(f"{func}: num_vertices and iterations must be >= 0, got {V} and {iterations}")
+        self.num_vertices, self.iterations = V, iterations
+        self._levels = []
+        f = faces.contiguous() if iterations else faces
+        for _ in range(iterations):
+            if _lib.lib().dibr_b200_loop_subdivision_workspace_bytes(V, f.shape[0]) == 0:
+                raise RuntimeError(f"{func}: {V} vertices or {f.shape[0]} faces do not fit 32-bit indices")
+            level = _SubdivisionLevel(func, V, f)
+            self._levels.append(level)
+            V, f = V + level.num_edges, level.new_faces
+        self.faces = f
+        self.num_output_vertices = V
+
+    def __call__(self, vertices, alpha=None):
+        func = "LoopSubdivision"
+        typed = [("vertices", vertices, torch.float32), ("faces", self.faces, torch.int64)]
+        if alpha is not None:
+            typed.append(("alpha", alpha, torch.float32))
+        _check(func, typed)
+        V = self.num_vertices
+        if vertices.dim() != 3 or vertices.shape[1:] != (V, 3):
+            raise RuntimeError(f"{func}: expected vertices of shape (B, {V}, 3), got {list(vertices.shape)}")
+        if alpha is not None and tuple(alpha.shape) != (vertices.shape[0], V):
+            raise RuntimeError(f"{func}: expected alpha of shape ({vertices.shape[0]}, {V}), got {list(alpha.shape)}")
+        if not self._levels:
+            return vertices
+        x = vertices.contiguous()
+        a = None if alpha is None else alpha.contiguous()
+        for k, level in enumerate(self._levels):
+            carry = a is not None and k + 1 < len(self._levels)
+            out = _SubdivideStep.apply(x, a, level, carry)
+            x, a = out if carry else (out, None)
+        return x
+
+
+def subdivide_trianglemesh(vertices, faces, iterations, alpha=None):
+    r"""kaolin.ops.mesh.subdivide_trianglemesh: ``iterations`` levels of Loop subdivision of
+    ``vertices`` (B, V, 3) float32 with the unbatched ``faces`` (F, 3) int64 -> (vertices
+    (B, V', 3), faces (F·4^iterations, 3)).  ``alpha`` (B, V) float32, if given, is the per-vertex
+    smoothing weight (with autograd), carried to the new vertices from level to level as the
+    reference does; otherwise each level uses Loop's weights.  The reference's quirks are kept: a vertex
+    referenced by no face (and every vertex when F = 0) comes out NaN, whatever alpha is;
+    ``iterations = 0`` returns the inputs.  The topology is built on every call, as the reference
+    does; ``LoopSubdivision`` builds it once.
+
+    Deliberate deviations: any B works (the reference raises for B > 1) and a given alpha must be
+    (B, V); a face index outside [0, V) raises ``IndexError``; faces that are not triangles raise (the
+    reference mis-indexes them); only float32 is accepted (the reference's buffers are float32).
+    """
+    func = "subdivide_trianglemesh"
+    _check_faces(func, faces)
+    _check(func, [("vertices", vertices, torch.float32), ("faces", faces, torch.int64)])
+    if vertices.dim() != 3 or vertices.shape[-1] != 3:
+        raise RuntimeError(f"{func}: expected vertices of shape (B, V, 3), got {list(vertices.shape)}")
+    if int(iterations) == 0:
+        if alpha is not None:
+            _check(func, [("alpha", alpha, torch.float32), ("faces", faces, torch.int64)])
+        return vertices, faces
+    S = LoopSubdivision(vertices.shape[1], faces, iterations)
+    return S(vertices, alpha), S.faces
