@@ -620,6 +620,81 @@ int dibr_b200_loop_subdivision_backward(int batch, int num_vertices, int num_edg
                                         dibr_b200_stream_t stream);
 
 /*
+ * Tet-mesh topology for `tets` (T, 4) int64 over V vertices (csrc/mesh_topology.cu): the adjacency of
+ * dibr_b200_mesh_topology_build, but with all three other corners of a tet as each corner's
+ * neighbours, so every tet contributes its six edges (faces keep their cyclic edges).  Edges are
+ * numbered as for Loop subdivision: the adjacency entries (i, j) with j >= i in CSR order, which is
+ * the lexicographic order of the reference's unique(dim=0) over the tets' sorted edges; a degenerate
+ * tet's self-loop (i, i) is an edge.  dibr_b200_tet_topology_build writes, in caller-owned buffers:
+ *   adj_ptr (V+1), adj (12T) int32   the adjacency CSR (first adj_ptr[V] entries used)
+ *   edges (6T, 2) int32              first E rows: {a, b}, a <= b
+ *   adj_edge (12T) int32             the edge id of every adjacency entry, in both directions
+ *   tet_edge (T, 6) int32            the edge ids of corner pairs 01, 02, 03, 12, 13, 23 of each tet
+ *   status (3) int32                 {E, error, adj_ptr[V]}: error is non-zero when a tet index lies
+ *                                    outside [0, V); the outputs are then not usable.
+ * Needs 12T < 2^31 and V < 2^31 - 1 (else DIBR_B200_ESIZE) and workspace >=
+ * dibr_b200_tet_topology_workspace_bytes(); deterministic.  Read status; nothing else comes back.
+ */
+size_t dibr_b200_tet_topology_workspace_bytes(int num_vertices, int64_t num_tets);
+int dibr_b200_tet_topology_build(int num_vertices, int64_t num_tets, const int64_t* tets, int32_t* adj_ptr,
+                                 int32_t* adj, int32_t* edges, int32_t* adj_edge, int32_t* tet_edge, int32_t* status,
+                                 void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
+ * Marching tetrahedra (kaolin/ops/conversions/tetmesh.py:57-168) for B views of one tet grid, on its
+ * topology (above).  occ = sdf > 0 (0 and NaN are outside).  Each view's output vertices are its
+ * sign-change edges (occ(a) != occ(b)) in edge order, at (x_a (-s_b) + x_b s_a) / (s_a + (-s_b)),
+ * each step rounded as the reference's element-wise ops.  A tet's case is sum_k occ(corner k) 2^k;
+ * its faces follow the case table (dibr_b200_marching_tets_case_table), those of one-triangle tets
+ * first, in tet order, then both of each two-triangle tet, in tet order.
+ *   dibr_b200_marching_tets_count: flags every (view, edge) and classifies every (view, tet), and
+ *     writes scan (B*(E + 2T) + 1) int32, the exclusive scan of [edge flags | one-triangle | two-
+ *     triangle flags], and counts (B, 3) int32 {vertices, one-triangle tets, two-triangle tets}: the
+ *     one value to read back to size the outputs.  Workspace >= dibr_b200_marching_tets_workspace_bytes.
+ *   dibr_b200_marching_tets_emit: writes, all views in one array each, view after view,
+ *     out_vertices (sum nv, 3) f32, out_faces (sum nf, 3) int64 (vertex ids per view, nf = n1 + 2 n2),
+ *     out_tet_idx (sum nf) int64 or NULL, and vid (B, E) int32: the row of each (view, edge) in
+ *     out_vertices, -1 where the edge has no sign change.
+ *   dibr_b200_marching_tets_backward: grad_out (sum nv, 3) -> grad_vertices (B, V, 3) and grad_sdf
+ *     (B, V), either NULL: one thread per (view, vertex) over its adjacency row, no atomics.
+ * B*(E + 2T) must be < 2^31 - 1 (else DIBR_B200_ESIZE).
+ * dibr_b200_marching_tets_case_table (host): pairs (16, 2, 3, 2) int32, the corners (i, j) of the edge
+ * of each vertex of each triangle of each case, -1 where the case has fewer triangles.
+ */
+int dibr_b200_marching_tets_case_table(int32_t* pairs);
+size_t dibr_b200_marching_tets_workspace_bytes(int batch, int num_edges, int64_t num_tets);
+int dibr_b200_marching_tets_count(int batch, int num_vertices, int num_edges, int64_t num_tets, const int32_t* edges,
+                                  const int64_t* tets, const float* sdf, int32_t* scan, int32_t* counts,
+                                  void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_marching_tets_emit(int batch, int num_vertices, int num_edges, int64_t num_tets, const int32_t* edges,
+                                 const int64_t* tets, const int32_t* tet_edge, const float* vertices, const float* sdf,
+                                 const int32_t* scan, int32_t* vid, float* out_vertices, int64_t* out_faces,
+                                 int64_t* out_tet_idx, dibr_b200_stream_t stream);
+int dibr_b200_marching_tets_backward(int batch, int num_vertices, int num_edges, const int32_t* adj_ptr,
+                                     const int32_t* adj, const int32_t* adj_edge, const float* vertices,
+                                     const float* sdf, const int32_t* vid, const float* grad_out,
+                                     float* grad_vertices, float* grad_sdf, dibr_b200_stream_t stream);
+
+/*
+ * subdivide_tetmesh (kaolin/ops/mesh/tetmesh.py:85-181) on the tet topology: vertices (B, V, 3) and
+ * features (B, V, channels) or NULL -> out_vertices (B, V + E, 3), out_features: rows < V copied, row
+ * V + e the midpoint (y_a + y_b) * 0.5 of edge e; out_tets (8T, 4) int64 or NULL: child k of tet t at
+ * row k*T + t, over (v0, v1, v2, v3, V+e01, V+e02, V+e03, V+e12, V+e13, V+e23):
+ *   [0,4,5,6] [1,7,4,8] [2,5,7,9] [3,6,9,8] [4,5,6,8] [4,5,8,7] [9,5,8,6] [9,5,7,8].
+ * Backward: one thread per input vertex, its row's gradient plus half of each of its edges' rows.
+ * V + E >= 2^31 - 1 or 12T >= 2^31 gives DIBR_B200_ESIZE; negative sizes or a NULL buffer that is
+ * used give DIBR_B200_EINVAL.
+ */
+int dibr_b200_tet_subdivide_forward(int batch, int num_vertices, int num_edges, int64_t num_tets, int channels,
+                                    const int32_t* edges, const int64_t* tets, const int32_t* tet_edge,
+                                    const float* vertices, const float* features, float* out_vertices,
+                                    float* out_features, int64_t* out_tets, dibr_b200_stream_t stream);
+int dibr_b200_tet_subdivide_backward(int batch, int num_vertices, int num_edges, int channels, const int32_t* adj_ptr,
+                                     const int32_t* adj, const int32_t* adj_edge, const float* grad_out_vertices,
+                                     const float* grad_out_features, float* grad_vertices, float* grad_features,
+                                     dibr_b200_stream_t stream);
+
+/*
  * Exchange step of the view-sharded path (SURVEY.md 8e; kaolin_b200/csrc/peer_push.cu): the
  * reference has no multi-GPU code - its callers all-gather the per-view gradients with
  * torch.distributed.  All-gather by STORES over NVLink: copies `bytes` (multiple of 16) from the

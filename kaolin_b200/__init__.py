@@ -7,9 +7,11 @@ either side of the rasterizer in the DIB-R loop (``render.mesh.prepare_vertices`
 (``render.lighting``, ``render.easy_render``), and the mesh Laplacian regulariser of the loss
 (``ops.mesh.{adjacency_matrix, uniform_laplacian, average_face_vertex_features,
 compute_vertex_normals}``, ``metrics.trianglemesh.uniform_laplacian_smoothing``, and
-``ops.mesh.UniformLaplacian``, which applies the Laplacian without its V x V matrix), and Loop
+``ops.mesh.UniformLaplacian``, which applies the Laplacian without its V x V matrix), Loop
 subdivision (``ops.mesh.subdivide_trianglemesh`` and ``ops.mesh.LoopSubdivision``, which builds its
-levels once); see DESIGN.md for scope.  There is no CPU fallback: every entry point
+levels once), and DMTet's tet-grid operators (``ops.conversions.marching_tetrahedra``,
+``ops.conversions.MarchingTetrahedra``, which builds the grid's topology once, and
+``ops.mesh.subdivide_tetmesh``); see DESIGN.md for scope.  There is no CPU fallback: every entry point
 raises if the CUDA library (kaolin_b200/csrc, built in-tree) is missing or the
 tensors are not on a CUDA device.
 """

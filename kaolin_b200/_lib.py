@@ -114,6 +114,16 @@ SIGNATURES = {
     "dibr_b200_loop_subdivision_build": (_i, [_i, _i64] + [_vp] * 11 + [_vp, _sz, _vp]),
     "dibr_b200_loop_subdivision_forward": (_i, [_i, _i, _i] + [_vp] * 8 + [_vp]),
     "dibr_b200_loop_subdivision_backward": (_i, [_i, _i, _i] + [_vp] * 13 + [_vp]),
+    # tet meshes: marching tetrahedra (ops.conversions) and subdivide_tetmesh (ops.mesh)
+    "dibr_b200_tet_topology_workspace_bytes": (_sz, [_i, _i64]),
+    "dibr_b200_tet_topology_build": (_i, [_i, _i64] + [_vp] * 7 + [_vp, _sz, _vp]),
+    "dibr_b200_marching_tets_case_table": (_i, [_vp]),
+    "dibr_b200_marching_tets_workspace_bytes": (_sz, [_i, _i, _i64]),
+    "dibr_b200_marching_tets_count": (_i, [_i, _i, _i, _i64] + [_vp] * 5 + [_vp, _sz, _vp]),
+    "dibr_b200_marching_tets_emit": (_i, [_i, _i, _i, _i64] + [_vp] * 10 + [_vp]),
+    "dibr_b200_marching_tets_backward": (_i, [_i, _i, _i] + [_vp] * 9 + [_vp]),
+    "dibr_b200_tet_subdivide_forward": (_i, [_i, _i, _i, _i64, _i] + [_vp] * 8 + [_vp]),
+    "dibr_b200_tet_subdivide_backward": (_i, [_i, _i, _i, _i] + [_vp] * 7 + [_vp]),
 }
 
 
@@ -209,6 +219,14 @@ def call(name, device, *args, stream=None, what=None):
     with torch.cuda.device(device):
         status = getattr(lib(), name)(*args, stream.cuda_stream)
     check(status, what or name)
+
+
+def marching_tets_case_table():
+    """The library's marching-tetrahedra case table (a host query, no device work): 16 * 2 * 3 * 2
+    corner indices, -1 where a case has fewer triangles (include/dibr_b200.h)."""
+    out = (ctypes.c_int32 * (16 * 12))()
+    check(lib().dibr_b200_marching_tets_case_table(out), "marching_tets_case_table")
+    return list(out)
 
 
 def scratch(nbytes, device):

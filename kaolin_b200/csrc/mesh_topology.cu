@@ -16,6 +16,9 @@
 // makes the result independent of the order of the atomics: the build is deterministic.
 //
 // Every per-step kernel is a gather over one of the CSRs: no atomics, bit-reproducible.
+//
+// The same build serves Loop subdivision (triangle meshes) and, with all other corners of a cell as
+// each corner's neighbours, tet meshes: marching tetrahedra and subdivide_tetmesh (end of the file).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -134,7 +137,8 @@ int exclusive_scan(const int* in, int n, int* sums, int* out, cudaStream_t st) {
 // Build.
 struct Topo {
   int V, S;
-  int F;              // fits: 2*F*S < 2^31 is checked on the host
+  int R;              // raw neighbours per corner: 2 (faces: the cyclic ones) or S - 1 (cells: all others)
+  int F;              // fits: R*F*S < 2^31 is checked on the host
   const int64_t* faces;
   int* corner_ptr; int* corners; int* adj_ptr; int* adj; int* degree; float* weight; int* status;
   int* count; int* raw; int* sums; int* long_rows; int* long_count;
@@ -151,8 +155,9 @@ __global__ void __launch_bounds__(kThreads) topo_count_kernel(Topo t) {
 }
 
 // Each corner takes a slot of its vertex's row (in whatever order the atomics give) and writes its key
-// and its two raw neighbours; the row sort below puts them in order.  Corners with an index outside
-// [0, V) were counted nowhere and write nothing.
+// and its R raw neighbours (R = 2: the cyclic ones, faces[f, k +- 1]; otherwise every other corner of
+// the cell); the row sort below puts them in order.  Corners with an index outside [0, V) were counted
+// nowhere and write nothing.
 __global__ void __launch_bounds__(kThreads) topo_fill_kernel(Topo t) {
   const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= (int64_t)t.F * t.S) return;
@@ -162,8 +167,14 @@ __global__ void __launch_bounds__(kThreads) topo_fill_kernel(Topo t) {
   const int p = t.corner_ptr[v] + atomicSub(t.count + v, 1) - 1;
   t.corners[p] = k * t.F + f;
   const int64_t* row = t.faces + (int64_t)f * t.S;
-  t.raw[2 * (int64_t)p] = (int)row[k + 1 == t.S ? 0 : k + 1];
-  t.raw[2 * (int64_t)p + 1] = (int)row[k == 0 ? t.S - 1 : k - 1];
+  int* out = t.raw + (int64_t)t.R * p;
+  if (t.R == 2) {
+    out[0] = (int)row[k + 1 == t.S ? 0 : k + 1];
+    out[1] = (int)row[k == 0 ? t.S - 1 : k - 1];
+  } else {
+    for (int u = 0, m = 0; u < t.S; ++u)
+      if (u != k) out[m++] = (int)row[u];
+  }
 }
 
 __device__ __forceinline__ void insertion_sort(int* a, int n) {
@@ -198,10 +209,10 @@ __global__ void __launch_bounds__(kThreads) topo_sort_rows_kernel(Topo t) {
   int* keys = t.corners + b;
   insertion_sort(keys, n);
   for (int i = 0; i < n; ++i) keys[i] = key_to_corner(keys[i], t.F, t.S);
-  int* nb = t.raw + 2 * (int64_t)b;
-  insertion_sort(nb, 2 * n);
+  int* nb = t.raw + (int64_t)t.R * b;
+  insertion_sort(nb, t.R * n);
   int u = 0;
-  for (int i = 0; i < 2 * n; ++i)
+  for (int i = 0; i < t.R * n; ++i)
     if (i == 0 || nb[i] != nb[u - 1]) nb[u++] = nb[i];
   finish_row(t, v, u);
 }
@@ -236,8 +247,8 @@ __global__ void __launch_bounds__(kScanThreads) topo_sort_long_kernel(Topo t) {
     int* keys = t.corners + b;
     block_bitonic_sort(keys, n);
     for (int i = threadIdx.x; i < n; i += blockDim.x) keys[i] = key_to_corner(keys[i], t.F, t.S);
-    int* nb = t.raw + 2 * (int64_t)b;
-    const int m = 2 * n;
+    int* nb = t.raw + (int64_t)t.R * b;
+    const int m = t.R * n;
     block_bitonic_sort(nb, m);
     // in-place deduplication: chunk by chunk, each thread reads its value and its predecessor before
     // any write of the chunk; writes land at or below the chunk's first index, so only the value
@@ -267,7 +278,7 @@ __global__ void __launch_bounds__(kThreads) topo_compact_kernel(Topo t) {
   if (w == 0 && lane == 0) t.status[0] = t.adj_ptr[t.V];
   if (w >= t.V) return;
   const int v = (int)w;
-  const int* src = t.raw + 2 * (int64_t)t.corner_ptr[v];
+  const int* src = t.raw + (int64_t)t.R * t.corner_ptr[v];
   const int b = t.adj_ptr[v], n = t.adj_ptr[v + 1] - b;
   for (int i = lane; i < n; i += 32) t.adj[b + i] = src[i];
 }
@@ -276,24 +287,48 @@ struct TopoLayout {
   size_t count, raw, sums, long_rows, long_count, bytes;
 };
 
-TopoLayout topo_layout(int V, int64_t corners) {
+TopoLayout topo_layout(int V, int64_t corners, int R) {
   TopoLayout l;
   const size_t tiles = (size_t)(V + kScanTile - 1) / kScanTile + 1;
   l.count = 0;
   l.raw = align_up(l.count + sizeof(int) * (size_t)V, 256);
-  l.sums = align_up(l.raw + sizeof(int) * 2 * (size_t)corners, 256);
+  l.sums = align_up(l.raw + sizeof(int) * R * (size_t)corners, 256);
   l.long_rows = align_up(l.sums + sizeof(int) * tiles, 256);
   l.long_count = align_up(l.long_rows + sizeof(int) * (size_t)V, 256);
   l.bytes = l.long_count + 256;
   return l;
 }
 
-// 0, or the error: V must leave room for V + 1 offsets, and the 2*F*S raw neighbour entries (so
+// 0, or the error: V must leave room for V + 1 offsets, and the R*F*S raw neighbour entries (so
 // every offset and every key k*F + f) must fit a 32-bit int.
-int topo_dims(int V, int64_t F, int S) {
+int topo_dims(int V, int64_t F, int S, int R = 2) {
   if (V < 0 || F < 0 || S < 3) return DIBR_B200_EINVAL;
-  if (V == INT32_MAX || F > (int64_t)INT32_MAX / S / 2) return DIBR_B200_ESIZE;
+  if (V == INT32_MAX || F > (int64_t)INT32_MAX / S / R) return DIBR_B200_ESIZE;
   return 0;
+}
+
+// The build of both CSRs, with the layout l in ws; arguments checked by the caller.
+int topo_build(Topo& t, char* ws, const TopoLayout& l, cudaStream_t st) {
+  t.count = (int*)(ws + l.count); t.raw = (int*)(ws + l.raw); t.sums = (int*)(ws + l.sums);
+  t.long_rows = (int*)(ws + l.long_rows); t.long_count = (int*)(ws + l.long_count);
+  const int V = t.V;
+  const int64_t FS = (int64_t)t.F * t.S;
+  if (cudaMemsetAsync(t.status, 0, 2 * sizeof(int), st) != cudaSuccess) return (int)cudaGetLastError();
+  if (V > 0 && cudaMemsetAsync(t.count, 0, sizeof(int) * (size_t)V, st) != cudaSuccess) return (int)cudaGetLastError();
+  if (cudaMemsetAsync(t.long_count, 0, sizeof(int), st) != cudaSuccess) return (int)cudaGetLastError();
+  if (FS > 0) { Span s("topo_count_kernel", st); topo_count_kernel<<<grid_for(FS, kThreads), kThreads, 0, st>>>(t); }
+  if (int e = exclusive_scan(t.count, V, t.sums, t.corner_ptr, st)) return e;
+  if (FS > 0) { Span s("topo_fill_kernel", st); topo_fill_kernel<<<grid_for(FS, kThreads), kThreads, 0, st>>>(t); }
+  if (V > 0) {
+    { Span s("topo_sort_rows_kernel", st); topo_sort_rows_kernel<<<grid_for(V, kThreads), kThreads, 0, st>>>(t); }
+    { Span s("topo_sort_long_kernel", st); topo_sort_long_kernel<<<kLongCtas, kScanThreads, 0, st>>>(t); }
+  }
+  if (int e = exclusive_scan(t.degree, V, t.sums, t.adj_ptr, st)) return e;
+  {
+    Span s("topo_compact_kernel", st);
+    topo_compact_kernel<<<grid_for(32 * (int64_t)(V > 0 ? V : 1), kThreads), kThreads, 0, st>>>(t);
+  }
+  return (int)cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -441,6 +476,7 @@ struct Subdiv {
   const int64_t* faces;
   const int* corner_ptr; const int* corners; const int* adj_ptr; const int* adj;
   int* count; int* edge_ptr; int* adj_edge; int* face_edge; int4* edges; int64_t* new_faces;
+  int2* pairs;        // tet meshes: {a, b} per edge instead of the face record
 };
 
 __device__ __forceinline__ int lower_bound_row(const int* __restrict__ adj, int lo, int hi, int key) {
@@ -466,11 +502,13 @@ __global__ void __launch_bounds__(kThreads) subdiv_count_kernel(Subdiv s) {
   s.count[i] = e1 - lower_bound_row(s.adj, __ldg(s.adj_ptr + i), e1, i);
 }
 
-// One thread per adjacency entry (i, j): its edge id, and for j >= i the edge record.  The face edges
-// (f, k) of edge (i, j) are found among the corners of i: corner k of f starts face edge k, whose
+// One thread per adjacency entry (i, j): its edge id, and for j >= i the edge record: FACES (triangle
+// meshes) the int4 record with the edge's two faces, otherwise (tet meshes) the pair {i, j}.  The face
+// edges (f, k) of edge (i, j) are found among the corners of i: corner k of f starts face edge k, whose
 // other end is faces[f, k+1], and ends face edge k-1, whose other end is faces[f, k-1] (counted there
 // only when j != i, so that a self-loop's face edge is counted once).  Entries naming a vertex outside
 // [0, V) exist only when the topology build reported an error; they get id -1.
+template <bool FACES>
 __global__ void __launch_bounds__(kThreads) subdiv_edges_kernel(Subdiv s, int64_t capacity) {
   const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= capacity) return;
@@ -486,6 +524,7 @@ __global__ void __launch_bounds__(kThreads) subdiv_edges_kernel(Subdiv s, int64_
   if (j < i) { s.adj_edge[p] = edge_id(s, j, i); return; }
   const int id = p + s.edge_ptr[i + 1] - __ldg(s.adj_ptr + i + 1);
   s.adj_edge[p] = id;
+  if (!FACES) { s.pairs[id] = make_int2(i, j); return; }
   int n = 0, f0 = -1, f1 = -1;
   for (int c = __ldg(s.corner_ptr + i), c1 = __ldg(s.corner_ptr + i + 1); c < c1; ++c) {
     const int corner = __ldg(s.corners + c), f = corner / 3, k = corner - 3 * f;
@@ -685,13 +724,303 @@ __global__ void __launch_bounds__(kThreads) subdiv_backward_kernel(
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Tet meshes (kaolin.ops.conversions.marching_tetrahedra, kaolin.ops.mesh.subdivide_tetmesh).  The
+// topology is that of the cells (T, 4) with all three other corners as each corner's neighbours, so
+// the adjacency holds the six edges of every tet; edges are numbered as for Loop subdivision, and
+// tet_edge (T, 6) holds each tet's corner pairs 01, 02, 03, 12, 13, 23 as edge ids.
+__global__ void __launch_bounds__(kThreads) tet_edges_kernel(Subdiv s) {
+  constexpr int kTetPairA[6] = {0, 0, 0, 1, 1, 2};
+  constexpr int kTetPairB[6] = {1, 2, 3, 2, 3, 3};
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= s.F) return;
+  const int64_t* row = s.faces + 4 * (int64_t)t;
+  int64_t v[4];
+  bool ok = true;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { v[k] = __ldg(row + k); ok = ok && valid_vertex(v[k], s.V); }
+#pragma unroll
+  for (int u = 0; u < 6; ++u) {
+    const int64_t a = v[kTetPairA[u]], b = v[kTetPairB[u]];
+    s.face_edge[6 * (int64_t)t + u] = ok ? edge_id(s, (int)(a < b ? a : b), (int)(a < b ? b : a)) : -1;
+  }
+}
+
+struct TetLayout {
+  TopoLayout topo;
+  size_t corner_ptr, corners, degree, weight, status, edge_ptr, bytes;
+};
+
+TetLayout tet_layout(int V, int64_t T) {
+  TetLayout l;
+  l.topo = topo_layout(V, 4 * T, 3);
+  l.corner_ptr = align_up(l.topo.bytes, 256);
+  l.corners = align_up(l.corner_ptr + sizeof(int) * ((size_t)V + 1), 256);
+  l.degree = align_up(l.corners + sizeof(int) * 4 * (size_t)T, 256);
+  l.weight = align_up(l.degree + sizeof(int) * (size_t)V, 256);
+  l.status = align_up(l.weight + sizeof(float) * (size_t)V, 256);
+  l.edge_ptr = l.status + 256;
+  l.bytes = align_up(l.edge_ptr + sizeof(int) * ((size_t)V + 1), 256);
+  return l;
+}
+
+// Marching tetrahedra.  occ(v) = sdf(v) > 0 (0 and NaN are outside).  A tet's case is
+// c = sum_k occ(corner k) 2^k; it has one triangle when 1 or 3 corners are inside, two when 2 are.
+// Its triangles, in the order the reference emits them: each is three corner pairs, each pair one
+// hex byte "ij" (the edge between corners i and j); slots past the case's triangles are 0.  Every
+// pair a case uses joins an inside and an outside corner, so it always has an output vertex.
+#define DIBR_B200_MT_CASES                                                                                \
+  {                                                                                                       \
+    0x000000000000ull, 0x020103000000ull, 0x130112000000ull, 0x021303021213ull, 0x120223000000ull,         \
+    0x031201032312ull, 0x021301022313ull, 0x130323000000ull, 0x132303000000ull, 0x130201132302ull,         \
+    0x120301122303ull, 0x021223000000ull, 0x130203131202ull, 0x120113000000ull, 0x030102000000ull,         \
+    0x000000000000ull                                                                                     \
+  }
+__constant__ uint64_t kMtCases[16] = DIBR_B200_MT_CASES;
+const uint64_t kMtCasesHost[16] = DIBR_B200_MT_CASES;
+
+// Pair k (0..5) of a case word -> the tet's edge slot (0..5: 01, 02, 03, 12, 13, 23).
+__host__ __device__ __forceinline__ int mt_pair_slot(uint64_t word, int k, int* a = nullptr, int* b = nullptr) {
+  const int byte = (int)(word >> (40 - 8 * k)) & 0xff, i = byte >> 4, j = byte & 15;
+  if (a) { *a = i; *b = j; }
+  return i + j - 1 + (i > 0);
+}
+
+__device__ __forceinline__ int mt_triangles(int c) {
+  const int n = __popc(c);
+  return n == 2 ? 2 : (n & 1);
+}
+
+struct MTets {
+  int B, V, E, T;
+  const int2* edges; const int64_t* tets; const int* tet_edge; const float* x; const float* sdf;
+  int* flags; const int* scan; int* vid; float* out_v; int64_t* out_f; int64_t* out_tet;
+};
+
+__device__ __forceinline__ int mt_case(const MTets& m, int b, int t) {
+  const int64_t* row = m.tets + 4 * (int64_t)t;
+  const float* s = m.sdf + (int64_t)b * m.V;
+  int c = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) c |= (__ldg(s + __ldg(row + k)) > 0.f) << k;
+  return c;
+}
+
+// flags = [B*E sign-change flags | B*T one-triangle flags | B*T two-triangle flags], one thread each
+// for the first B*E and the next B*T.
+__global__ void __launch_bounds__(kThreads) mt_classify_kernel(MTets m) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t BE = (int64_t)m.B * m.E, BT = (int64_t)m.B * m.T;
+  if (q < BE) {
+    const int b = (int)(q / m.E);
+    const int2 e = __ldg(m.edges + (q - (int64_t)b * m.E));
+    const float* s = m.sdf + (int64_t)b * m.V;
+    m.flags[q] = (__ldg(s + e.x) > 0.f) != (__ldg(s + e.y) > 0.f);
+  } else if (q < BE + BT) {
+    const int64_t r = q - BE;
+    const int b = (int)(r / m.T);
+    const int n = mt_triangles(mt_case(m, b, (int)(r - (int64_t)b * m.T)));
+    m.flags[BE + r] = n == 1;
+    m.flags[BE + BT + r] = n == 2;
+  }
+}
+
+// counts[b] = {vertices, one-triangle tets, two-triangle tets} of view b, from the scan of the flags.
+__global__ void __launch_bounds__(kThreads) mt_counts_kernel(MTets m, int* __restrict__ counts) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= m.B) return;
+  const int64_t BE = (int64_t)m.B * m.E, BT = (int64_t)m.B * m.T, E = m.E, T = m.T;
+  counts[3 * b] = m.scan[(b + 1) * E] - m.scan[b * E];
+  counts[3 * b + 1] = m.scan[BE + (b + 1) * T] - m.scan[BE + b * T];
+  counts[3 * b + 2] = m.scan[BE + BT + (b + 1) * T] - m.scan[BE + BT + b * T];
+}
+
+// One thread per (view, edge): a sign-change edge (a, b) gets the output row scan[q] (rows of all
+// views in one array, view by view) and the vertex (x_a (-s_b) + x_b s_a) / (s_a + (-s_b)), rounded
+// step by step as the reference's separate element-wise ops are; vid[q] is the row, or -1.
+__global__ void __launch_bounds__(kThreads) mt_vertices_kernel(MTets m) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= (int64_t)m.B * m.E) return;
+  const int row = __ldg(m.scan + q);
+  if (__ldg(m.scan + q + 1) == row) { m.vid[q] = -1; return; }
+  m.vid[q] = row;
+  const int b = (int)(q / m.E);
+  const int2 e = __ldg(m.edges + (q - (int64_t)b * m.E));
+  const int64_t ia = (int64_t)b * m.V + e.x, ib = (int64_t)b * m.V + e.y;
+  const float sa = __ldg(m.sdf + ia), nb = -__ldg(m.sdf + ib);
+  const float den = __fadd_rn(sa, nb);
+  float* o = m.out_v + 3 * (int64_t)row;
+#pragma unroll
+  for (int c = 0; c < 3; ++c)
+    o[c] = __fdiv_rn(__fadd_rn(__fmul_rn(__ldg(m.x + 3 * ia + c), nb), __fmul_rn(__ldg(m.x + 3 * ib + c), sa)), den);
+}
+
+// One thread per (view, tet): its triangles at their rows.  In view b, the faces of one-triangle tets
+// come first in tet order, then two per two-triangle tet; views follow each other in one array.
+// Vertex ids are per view.
+__global__ void __launch_bounds__(kThreads) mt_faces_kernel(MTets m) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t BE = (int64_t)m.B * m.E, BT = (int64_t)m.B * m.T;
+  if (r >= BT) return;
+  const int b = (int)(r / m.T), t = (int)(r - (int64_t)b * m.T);
+  const int c = mt_case(m, b, t), n = mt_triangles(c);
+  if (n == 0) return;
+  const int* one = m.scan + BE;          // exclusive scan of the one-triangle flags (continued by the two-)
+  const int* two = one + BT;
+  const int64_t v0 = (int64_t)b * m.T;
+  const int one0 = __ldg(one + v0) - __ldg(one), two0 = __ldg(two + v0) - __ldg(two);
+  int64_t f = one0 + 2 * (int64_t)two0;  // the view's first face
+  if (n == 1) f += __ldg(one + r) - __ldg(one + v0);
+  else f += (__ldg(one + v0 + m.T) - __ldg(one + v0)) + 2 * (int64_t)(__ldg(two + r) - __ldg(two + v0));
+  const uint64_t word = kMtCases[c];
+  const int* te = m.tet_edge + 6 * (int64_t)t;
+  const int* vid = m.vid + (int64_t)b * m.E;
+  const int base = __ldg(m.scan + (int64_t)b * m.E);
+  for (int k = 0; k < 3 * n; ++k) m.out_f[3 * f + k] = vid[__ldg(te + mt_pair_slot(word, k))] - base;
+  if (m.out_tet) for (int k = 0; k < n; ++k) m.out_tet[f + k] = t;
+}
+
+// One thread per (view, vertex i): the gradients of its sign-change edges, read from grad_out at each
+// edge's vertex row, summed over i's adjacency row.  For an edge (a, b), with n = -s_b,
+// d = s_a + n, num = x_a n + x_b s_a and y = num / d, as the reference's autograd forms them:
+//   gn = g / d,  gd = sum_c -g_c ((num_c / d) / d)
+//   x_a: gn n    x_b: gn s_a    s_a: sum_c gn_c x_b,c + gd    s_b: -(sum_c gn_c x_a,c + gd)
+__global__ void __launch_bounds__(kThreads) mt_backward_kernel(int64_t total, int V, int E, const int* __restrict__ adj_ptr,
+                                                               const int* __restrict__ adj,
+                                                               const int* __restrict__ adj_edge,
+                                                               const float* __restrict__ x, const float* __restrict__ sdf,
+                                                               const int* __restrict__ vid, const float* __restrict__ g,
+                                                               float* __restrict__ gx, float* __restrict__ gs) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= total) return;
+  const int64_t b = q / V;
+  const int i = (int)(q - b * V);
+  const float* xb = x + b * V * 3;
+  const float* sb = sdf + b * V;
+  const int* vb = vid + b * E;
+  float o0 = 0.f, o1 = 0.f, o2 = 0.f, os = 0.f;
+  for (int p = __ldg(adj_ptr + i), p1 = __ldg(adj_ptr + i + 1); p < p1; ++p) {
+    const int row = __ldg(vb + __ldg(adj_edge + p));
+    if (row < 0) continue;
+    const int j = __ldg(adj + p);
+    const bool first = i < j;               // i is the edge's endpoint a
+    const int ia = first ? i : j, ib = first ? j : i;
+    const float sa = __ldg(sb + ia), n = -__ldg(sb + ib);
+    const float d = __fadd_rn(sa, n);
+    float gn[3], xa[3], xe[3], gd = 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      xa[c] = __ldg(xb + 3 * (int64_t)ia + c);
+      xe[c] = __ldg(xb + 3 * (int64_t)ib + c);
+      const float gc = __ldg(g + 3 * (int64_t)row + c);
+      const float num = __fadd_rn(__fmul_rn(xa[c], n), __fmul_rn(xe[c], sa));
+      gn[c] = __fdiv_rn(gc, d);
+      gd = __fadd_rn(gd, __fmul_rn(-gc, __fdiv_rn(__fdiv_rn(num, d), d)));
+    }
+    if (first) {
+      o0 += __fmul_rn(gn[0], n); o1 += __fmul_rn(gn[1], n); o2 += __fmul_rn(gn[2], n);
+      os += __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(gn[0], xe[0]), __fmul_rn(gn[1], xe[1])), __fmul_rn(gn[2], xe[2])), gd);
+    } else {
+      o0 += __fmul_rn(gn[0], sa); o1 += __fmul_rn(gn[1], sa); o2 += __fmul_rn(gn[2], sa);
+      os -= __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(gn[0], xa[0]), __fmul_rn(gn[1], xa[1])), __fmul_rn(gn[2], xa[2])), gd);
+    }
+  }
+  if (gx) { gx[3 * q] = o0; gx[3 * q + 1] = o1; gx[3 * q + 2] = o2; }
+  if (gs) gs[q] = os;
+}
+
+// subdivide_tetmesh: one thread per output row (view b, row r < V + E) of the positions (3 channels)
+// and the features (D channels, if any): row r < V is vertex r, row V + e the midpoint of edge e,
+// (y_a + y_b) * 0.5 (the reference's mean of two).
+__global__ void __launch_bounds__(kThreads) tet_subdivide_forward_kernel(int64_t total, int V, int E, int D,
+                                                                         const int2* __restrict__ edges,
+                                                                         const float* __restrict__ x,
+                                                                         const float* __restrict__ f,
+                                                                         float* __restrict__ y, float* __restrict__ yf) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= total) return;
+  const int W = V + E;
+  const int64_t b = q / W;
+  const int r = (int)(q - b * W);
+  int a = r, c = r;
+  if (r >= V) { const int2 e = __ldg(edges + (r - V)); a = e.x; c = e.y; }
+  const int64_t ia = b * V + a, ic = b * V + c;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float u = __ldg(x + 3 * ia + k);
+    y[3 * q + k] = r < V ? u : __fmul_rn(__fadd_rn(u, __ldg(x + 3 * ic + k)), 0.5f);
+  }
+  for (int k = 0; k < D; ++k) {
+    const float u = __ldg(f + D * ia + k);
+    yf[D * q + k] = r < V ? u : __fmul_rn(__fadd_rn(u, __ldg(f + D * ic + k)), 0.5f);
+  }
+}
+
+// One thread per tet: its eight children, child k at row k*T + t, over the ten vertices
+// (v0, v1, v2, v3, V+e01, V+e02, V+e03, V+e12, V+e13, V+e23): a corner tet at each corner, then
+// four tets of the inner octahedron around its diagonal (e01, e23).
+__global__ void __launch_bounds__(kThreads) tet_children_kernel(int V, int T, const int64_t* __restrict__ tets,
+                                                                const int* __restrict__ tet_edge,
+                                                                int64_t* __restrict__ out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= T) return;
+  int64_t v[10];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) v[k] = __ldg(tets + 4 * (int64_t)t + k);
+#pragma unroll
+  for (int k = 0; k < 6; ++k) v[4 + k] = (int64_t)V + __ldg(tet_edge + 6 * (int64_t)t + k);
+  constexpr int kChild[32] = {0, 4, 5, 6,  1, 7, 4, 8,  2, 5, 7, 9,  3, 6, 9, 8,
+                              4, 5, 6, 8,  4, 5, 8, 7,  9, 5, 8, 6,  9, 5, 7, 8};
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    int64_t* o = out + 4 * ((int64_t)k * T + t);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) o[u] = v[kChild[4 * k + u]];
+  }
+}
+
+// One thread per (view b, input vertex i): its own row's gradient plus half that of every edge row
+// of i's adjacency row (a self-loop's row is all of i's: twice a half).
+__global__ void __launch_bounds__(kThreads) tet_subdivide_backward_kernel(int64_t total, int V, int E, int D,
+                                                                          const int* __restrict__ adj_ptr,
+                                                                          const int* __restrict__ adj,
+                                                                          const int* __restrict__ adj_edge,
+                                                                          const float* __restrict__ gy,
+                                                                          const float* __restrict__ gyf,
+                                                                          float* __restrict__ gx, float* __restrict__ gf) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= total) return;
+  const int64_t b = q / V;
+  const int i = (int)(q - b * V);
+  const int64_t own = b * (V + E) + i, edge0 = b * (V + E) + V;
+  const int p0 = __ldg(adj_ptr + i), p1 = __ldg(adj_ptr + i + 1);
+  if (gx) {
+    float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+    for (int p = p0; p < p1; ++p) {
+      const float w = __ldg(adj + p) == i ? 1.0f : 0.5f;
+      const float* ge = gy + 3 * (edge0 + __ldg(adj_edge + p));
+      s0 += w * __ldg(ge); s1 += w * __ldg(ge + 1); s2 += w * __ldg(ge + 2);
+    }
+    gx[3 * q] = __ldg(gy + 3 * own) + s0; gx[3 * q + 1] = __ldg(gy + 3 * own + 1) + s1;
+    gx[3 * q + 2] = __ldg(gy + 3 * own + 2) + s2;
+  }
+  if (gf) {
+    for (int k = 0; k < D; ++k) {
+      float s = 0.f;
+      for (int p = p0; p < p1; ++p)
+        s += (__ldg(adj + p) == i ? 1.0f : 0.5f) * __ldg(gyf + D * (edge0 + __ldg(adj_edge + p)) + k);
+      gf[D * q + k] = __ldg(gyf + D * own + k) + s;
+    }
+  }
+}
+
 }  // namespace
 
 extern "C" {
 
 size_t dibr_b200_mesh_topology_workspace_bytes(int num_vertices, int64_t num_faces, int face_size) {
   if (topo_dims(num_vertices, num_faces, face_size)) return 0;
-  return topo_layout(num_vertices, num_faces * face_size).bytes;
+  return topo_layout(num_vertices, num_faces * face_size, 2).bytes;
 }
 
 int dibr_b200_mesh_topology_build(int num_vertices, int64_t num_faces, int face_size, const int64_t* faces,
@@ -703,33 +1032,13 @@ int dibr_b200_mesh_topology_build(int num_vertices, int64_t num_faces, int face_
   if (!corner_ptr || !adj_ptr || !status || !workspace) return DIBR_B200_EINVAL;
   if (FS > 0 && (!faces || !corners || !adj)) return DIBR_B200_EINVAL;
   if (num_vertices > 0 && (!degree || !weight)) return DIBR_B200_EINVAL;
-  const TopoLayout l = topo_layout(num_vertices, FS);
+  const TopoLayout l = topo_layout(num_vertices, FS, 2);
   if (workspace_bytes < l.bytes) return DIBR_B200_EWORKSPACE;
-  char* ws = (char*)workspace;
   Topo t;
-  t.V = num_vertices; t.S = face_size; t.F = (int)num_faces; t.faces = faces;
+  t.V = num_vertices; t.S = face_size; t.R = 2; t.F = (int)num_faces; t.faces = faces;
   t.corner_ptr = corner_ptr; t.corners = corners; t.adj_ptr = adj_ptr; t.adj = adj; t.degree = degree;
   t.weight = weight; t.status = status;
-  t.count = (int*)(ws + l.count); t.raw = (int*)(ws + l.raw); t.sums = (int*)(ws + l.sums);
-  t.long_rows = (int*)(ws + l.long_rows); t.long_count = (int*)(ws + l.long_count);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int V = num_vertices;
-  if (cudaMemsetAsync(status, 0, 2 * sizeof(int), st) != cudaSuccess) return (int)cudaGetLastError();
-  if (V > 0 && cudaMemsetAsync(t.count, 0, sizeof(int) * (size_t)V, st) != cudaSuccess) return (int)cudaGetLastError();
-  if (cudaMemsetAsync(t.long_count, 0, sizeof(int), st) != cudaSuccess) return (int)cudaGetLastError();
-  if (FS > 0) { Span s("topo_count_kernel", st); topo_count_kernel<<<grid_for(FS, kThreads), kThreads, 0, st>>>(t); }
-  if (int e = exclusive_scan(t.count, V, t.sums, corner_ptr, st)) return e;
-  if (FS > 0) { Span s("topo_fill_kernel", st); topo_fill_kernel<<<grid_for(FS, kThreads), kThreads, 0, st>>>(t); }
-  if (V > 0) {
-    { Span s("topo_sort_rows_kernel", st); topo_sort_rows_kernel<<<grid_for(V, kThreads), kThreads, 0, st>>>(t); }
-    { Span s("topo_sort_long_kernel", st); topo_sort_long_kernel<<<kLongCtas, kScanThreads, 0, st>>>(t); }
-  }
-  if (int e = exclusive_scan(degree, V, t.sums, adj_ptr, st)) return e;
-  {
-    Span s("topo_compact_kernel", st);
-    topo_compact_kernel<<<grid_for(32 * (int64_t)(V > 0 ? V : 1), kThreads), kThreads, 0, st>>>(t);
-  }
-  return (int)cudaGetLastError();
+  return topo_build(t, (char*)workspace, l, (cudaStream_t)stream);
 }
 
 int dibr_b200_laplacian_apply(int batch, int num_vertices, int channels, const int32_t* adj_ptr, const int32_t* adj,
@@ -852,7 +1161,7 @@ int dibr_b200_loop_subdivision_build(int num_vertices, int64_t num_faces, const 
   if (int e = exclusive_scan(s.count, V, (int*)(ws + l.sums), edge_ptr, st)) return e;
   if (num_faces > 0) {
     const int64_t capacity = 6 * num_faces;       // the adjacency holds at most 2 * F * 3 entries
-    { Span sp("subdiv_edges_kernel", st); subdiv_edges_kernel<<<grid_for(capacity, kThreads), kThreads, 0, st>>>(s, capacity); }
+    { Span sp("subdiv_edges_kernel", st); subdiv_edges_kernel<true><<<grid_for(capacity, kThreads), kThreads, 0, st>>>(s, capacity); }
     { Span sp("subdiv_faces_kernel", st); subdiv_faces_kernel<<<grid_for(num_faces, kThreads), kThreads, 0, st>>>(s); }
   }
   cudaMemcpyAsync(status, edge_ptr + V, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
@@ -911,6 +1220,178 @@ int dibr_b200_loop_subdivision_backward(int batch, int num_vertices, int num_edg
         total, num_vertices, num_edges, corner_ptr, corners, adj_ptr, adj, adj_edge, face_edge, e4, vertices, nullptr,
         grad_out, nullptr, grad_vertices, nullptr);
   }
+  return (int)cudaGetLastError();
+}
+
+size_t dibr_b200_tet_topology_workspace_bytes(int num_vertices, int64_t num_tets) {
+  if (topo_dims(num_vertices, num_tets, 4, 3)) return 0;
+  return tet_layout(num_vertices, num_tets).bytes;
+}
+
+int dibr_b200_tet_topology_build(int num_vertices, int64_t num_tets, const int64_t* tets, int32_t* adj_ptr,
+                                 int32_t* adj, int32_t* edges, int32_t* adj_edge, int32_t* tet_edge, int32_t* status,
+                                 void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream) {
+  if (const int e = topo_dims(num_vertices, num_tets, 4, 3)) return e;
+  if (!adj_ptr || !status || !workspace) return DIBR_B200_EINVAL;
+  if (num_tets > 0 && (!tets || !adj || !edges || !adj_edge || !tet_edge)) return DIBR_B200_EINVAL;
+  const TetLayout l = tet_layout(num_vertices, num_tets);
+  if (workspace_bytes < l.bytes) return DIBR_B200_EWORKSPACE;
+  char* ws = (char*)workspace;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int V = num_vertices;
+  Topo t;
+  t.V = V; t.S = 4; t.R = 3; t.F = (int)num_tets; t.faces = tets;
+  t.corner_ptr = (int*)(ws + l.corner_ptr); t.corners = (int*)(ws + l.corners); t.adj_ptr = adj_ptr; t.adj = adj;
+  t.degree = (int*)(ws + l.degree); t.weight = (float*)(ws + l.weight); t.status = (int*)(ws + l.status);
+  if (int e = topo_build(t, ws, l.topo, st)) return e;
+  // the topology's count (all zero again) and scan partials serve the edge numbering
+  Subdiv s;
+  s.V = V; s.F = (int)num_tets; s.faces = tets;
+  s.corner_ptr = t.corner_ptr; s.corners = t.corners; s.adj_ptr = adj_ptr; s.adj = adj;
+  s.count = t.count; s.edge_ptr = (int*)(ws + l.edge_ptr); s.adj_edge = adj_edge; s.face_edge = tet_edge;
+  s.edges = nullptr; s.new_faces = nullptr; s.pairs = (int2*)edges;
+  if (V > 0) { Span sp("subdiv_count_kernel", st); subdiv_count_kernel<<<grid_for(V, kThreads), kThreads, 0, st>>>(s); }
+  if (int e = exclusive_scan(s.count, V, t.sums, s.edge_ptr, st)) return e;
+  if (num_tets > 0) {
+    const int64_t capacity = 12 * num_tets;       // the adjacency holds at most 3 * T * 4 entries
+    { Span sp("subdiv_edges_kernel<pairs>", st); subdiv_edges_kernel<false><<<grid_for(capacity, kThreads), kThreads, 0, st>>>(s, capacity); }
+    { Span sp("tet_edges_kernel", st); tet_edges_kernel<<<grid_for(num_tets, kThreads), kThreads, 0, st>>>(s); }
+  }
+  cudaMemcpyAsync(status, s.edge_ptr + V, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+  cudaMemcpyAsync(status + 1, t.status + 1, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+  cudaMemcpyAsync(status + 2, t.status, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+  return (int)cudaGetLastError();
+}
+
+int dibr_b200_marching_tets_case_table(int32_t* pairs) {
+  if (!pairs) return DIBR_B200_EINVAL;
+  for (int c = 0; c < 16; ++c) {
+    const int n = __builtin_popcount(c) == 2 ? 2 : (__builtin_popcount(c) & 1);
+    for (int k = 0; k < 6; ++k) {
+      int a = -1, b = -1;
+      if (k < 3 * n) mt_pair_slot(kMtCasesHost[c], k, &a, &b);
+      pairs[12 * c + 2 * k] = a;
+      pairs[12 * c + 2 * k + 1] = b;
+    }
+  }
+  return 0;
+}
+
+// B*(E + 2T) flags and their scan must be indexable by int.
+static int mt_dims(int batch, int V, int E, int64_t T) {
+  if (batch < 0 || V < 0 || E < 0 || T < 0) return DIBR_B200_EINVAL;
+  if ((int64_t)batch * ((int64_t)E + 2 * T) >= INT32_MAX || T > INT32_MAX / 12) return DIBR_B200_ESIZE;
+  return 0;
+}
+
+size_t dibr_b200_marching_tets_workspace_bytes(int batch, int num_edges, int64_t num_tets) {
+  if (mt_dims(batch, 0, num_edges, num_tets)) return 0;
+  const int64_t n = (int64_t)batch * (num_edges + 2 * num_tets);
+  const size_t tiles = (size_t)(n + kScanTile - 1) / kScanTile + 1;
+  return align_up(sizeof(int) * (size_t)n, 256) + align_up(sizeof(int) * tiles, 256);
+}
+
+int dibr_b200_marching_tets_count(int batch, int num_vertices, int num_edges, int64_t num_tets, const int32_t* edges,
+                                  const int64_t* tets, const float* sdf, int32_t* scan, int32_t* counts,
+                                  void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream) {
+  if (const int e = mt_dims(batch, num_vertices, num_edges, num_tets)) return e;
+  if (!scan || !workspace) return DIBR_B200_EINVAL;
+  if (batch > 0 && !counts) return DIBR_B200_EINVAL;
+  if (num_edges > 0 && !edges) return DIBR_B200_EINVAL;
+  if (num_tets > 0 && !tets) return DIBR_B200_EINVAL;
+  if (batch > 0 && num_vertices > 0 && !sdf) return DIBR_B200_EINVAL;
+  if (workspace_bytes < dibr_b200_marching_tets_workspace_bytes(batch, num_edges, num_tets)) return DIBR_B200_EWORKSPACE;
+  MTets m = {};
+  m.B = batch; m.V = num_vertices; m.E = num_edges; m.T = (int)num_tets;
+  m.edges = (const int2*)edges; m.tets = tets; m.sdf = sdf; m.flags = (int*)workspace; m.scan = scan;
+  const int64_t n = (int64_t)batch * (num_edges + 2 * num_tets);
+  int* sums = (int*)((char*)workspace + align_up(sizeof(int) * (size_t)n, 256));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t classify = (int64_t)batch * (num_edges + num_tets);
+  if (classify > 0) { Span s("mt_classify_kernel", st); mt_classify_kernel<<<grid_for(classify, kThreads), kThreads, 0, st>>>(m); }
+  if (int e = exclusive_scan(m.flags, (int)n, sums, scan, st)) return e;
+  if (batch > 0) { Span s("mt_counts_kernel", st); mt_counts_kernel<<<grid_for(batch, kThreads), kThreads, 0, st>>>(m, counts); }
+  return (int)cudaGetLastError();
+}
+
+int dibr_b200_marching_tets_emit(int batch, int num_vertices, int num_edges, int64_t num_tets, const int32_t* edges,
+                                 const int64_t* tets, const int32_t* tet_edge, const float* vertices, const float* sdf,
+                                 const int32_t* scan, int32_t* vid, float* out_vertices, int64_t* out_faces,
+                                 int64_t* out_tet_idx, dibr_b200_stream_t stream) {
+  if (const int e = mt_dims(batch, num_vertices, num_edges, num_tets)) return e;
+  const int64_t BE = (int64_t)batch * num_edges, BT = (int64_t)batch * num_tets;
+  if (BE + BT == 0) return 0;
+  if (!scan || !sdf || !out_vertices || !out_faces) return DIBR_B200_EINVAL;
+  if (BE > 0 && (!edges || !vid || !vertices)) return DIBR_B200_EINVAL;
+  if (BT > 0 && (!tets || !tet_edge || !vid)) return DIBR_B200_EINVAL;
+  MTets m = {};
+  m.B = batch; m.V = num_vertices; m.E = num_edges; m.T = (int)num_tets;
+  m.edges = (const int2*)edges; m.tets = tets; m.tet_edge = tet_edge; m.x = vertices; m.sdf = sdf; m.scan = scan;
+  m.vid = vid; m.out_v = out_vertices; m.out_f = out_faces; m.out_tet = out_tet_idx;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (BE > 0) { Span s("mt_vertices_kernel", st); mt_vertices_kernel<<<grid_for(BE, kThreads), kThreads, 0, st>>>(m); }
+  if (BT > 0) { Span s("mt_faces_kernel", st); mt_faces_kernel<<<grid_for(BT, kThreads), kThreads, 0, st>>>(m); }
+  return (int)cudaGetLastError();
+}
+
+int dibr_b200_marching_tets_backward(int batch, int num_vertices, int num_edges, const int32_t* adj_ptr,
+                                     const int32_t* adj, const int32_t* adj_edge, const float* vertices,
+                                     const float* sdf, const int32_t* vid, const float* grad_out,
+                                     float* grad_vertices, float* grad_sdf, dibr_b200_stream_t stream) {
+  if (batch < 0 || num_vertices < 0 || num_edges < 0) return DIBR_B200_EINVAL;
+  const int64_t total = (int64_t)batch * num_vertices;
+  if (total == 0 || (!grad_vertices && !grad_sdf)) return 0;
+  if (!adj_ptr || !vertices || !sdf) return DIBR_B200_EINVAL;
+  if (num_edges > 0 && (!adj || !adj_edge || !vid || !grad_out)) return DIBR_B200_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  Span s("mt_backward_kernel", st);
+  mt_backward_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(total, num_vertices, num_edges, adj_ptr, adj,
+                                                                     adj_edge, vertices, sdf, vid, grad_out,
+                                                                     grad_vertices, grad_sdf);
+  return (int)cudaGetLastError();
+}
+
+int dibr_b200_tet_subdivide_forward(int batch, int num_vertices, int num_edges, int64_t num_tets, int channels,
+                                    const int32_t* edges, const int64_t* tets, const int32_t* tet_edge,
+                                    const float* vertices, const float* features, float* out_vertices,
+                                    float* out_features, int64_t* out_tets, dibr_b200_stream_t stream) {
+  if (batch < 0 || num_vertices < 0 || num_edges < 0 || num_tets < 0 || channels < 0) return DIBR_B200_EINVAL;
+  if ((int64_t)num_vertices + num_edges >= INT32_MAX || num_tets > INT32_MAX / 12) return DIBR_B200_ESIZE;
+  if (channels > 0 && (!features || !out_features)) return DIBR_B200_EINVAL;
+  const int64_t total = (int64_t)batch * (num_vertices + num_edges);
+  if (total > 0 && (!vertices || !out_vertices || (num_edges > 0 && !edges))) return DIBR_B200_EINVAL;
+  if (out_tets && num_tets > 0 && (!tets || !tet_edge)) return DIBR_B200_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (total > 0) {
+    Span s("tet_subdivide_forward_kernel", st);
+    tet_subdivide_forward_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(
+        total, num_vertices, num_edges, channels, (const int2*)edges, vertices, features, out_vertices, out_features);
+  }
+  if (out_tets && num_tets > 0) {
+    Span s("tet_children_kernel", st);
+    tet_children_kernel<<<grid_for(num_tets, kThreads), kThreads, 0, st>>>(num_vertices, (int)num_tets, tets, tet_edge,
+                                                                           out_tets);
+  }
+  return (int)cudaGetLastError();
+}
+
+int dibr_b200_tet_subdivide_backward(int batch, int num_vertices, int num_edges, int channels, const int32_t* adj_ptr,
+                                     const int32_t* adj, const int32_t* adj_edge, const float* grad_out_vertices,
+                                     const float* grad_out_features, float* grad_vertices, float* grad_features,
+                                     dibr_b200_stream_t stream) {
+  if (batch < 0 || num_vertices < 0 || num_edges < 0 || channels < 0) return DIBR_B200_EINVAL;
+  if ((int64_t)num_vertices + num_edges >= INT32_MAX) return DIBR_B200_ESIZE;
+  if (grad_features && channels > 0 && !grad_out_features) return DIBR_B200_EINVAL;
+  if (grad_vertices && !grad_out_vertices) return DIBR_B200_EINVAL;
+  const int64_t total = (int64_t)batch * num_vertices;
+  if (channels == 0) grad_features = nullptr;
+  if (total == 0 || (!grad_vertices && !grad_features)) return 0;
+  if (!adj_ptr || (num_edges > 0 && (!adj || !adj_edge))) return DIBR_B200_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  Span s("tet_subdivide_backward_kernel", st);
+  tet_subdivide_backward_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(
+      total, num_vertices, num_edges, channels, adj_ptr, adj, adj_edge, grad_out_vertices, grad_out_features,
+      grad_vertices, grad_features);
   return (int)cudaGetLastError();
 }
 

@@ -1,3 +1,4 @@
-"""kaolin.ops drop-ins: the mesh Laplacian, adjacency, vertex averaging and Loop subdivision on sm_90a
-kernels."""
+"""kaolin.ops drop-ins: the mesh Laplacian, adjacency, vertex averaging, Loop subdivision, tet-mesh
+subdivision and marching tetrahedra on sm_90a kernels."""
 from . import mesh  # noqa: F401
+from . import conversions  # noqa: F401

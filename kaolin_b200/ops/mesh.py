@@ -19,6 +19,9 @@ once and applies them with autograd to the vertices and a learnable per-vertex a
 
     S = LoopSubdivision(V, faces, 2)          # coarse-to-fine DIB-R, or DMTet's learnable alpha
     fine_vertices = S(vertices, alpha)        # fine faces: S.faces
+
+``subdivide_tetmesh`` (tetmesh.py:85-181) refines a tet grid on the topology of its tets, which
+marching tetrahedra (``kaolin_b200.ops.conversions``) shares.
 """
 import torch
 
@@ -26,7 +29,7 @@ from .. import _lib
 from ..render.mesh import _host
 
 __all__ = ["adjacency_matrix", "uniform_laplacian", "compute_vertex_normals", "average_face_vertex_features",
-           "UniformLaplacian", "subdivide_trianglemesh", "LoopSubdivision"]
+           "UniformLaplacian", "subdivide_trianglemesh", "LoopSubdivision", "subdivide_tetmesh"]
 
 
 def _check(func, typed):
@@ -348,3 +351,106 @@ def subdivide_trianglemesh(vertices, faces, iterations, alpha=None):
         return vertices, faces
     S = LoopSubdivision(vertices.shape[1], faces, iterations)
     return S(vertices, alpha), S.faces
+
+
+def _trim(t, n):
+    """The first n rows of a capacity-sized build output, as their own allocation (at least one row, so
+    its pointer is never NULL)."""
+    return t[:max(int(n), 1)].clone()
+
+
+class _TetTopology:
+    """The topology of a tet mesh (see include/dibr_b200.h): the adjacency CSR with all six edges of
+    every tet, the unique edges (E, 2), each adjacency entry's edge id and each tet's six edge ids, built
+    with one device-to-host read.  Shared by ``subdivide_tetmesh`` and marching tetrahedra."""
+
+    def __init__(self, func, num_vertices, tets):
+        _check(func, [("tets", tets, torch.int64)])
+        if tets.dim() != 2 or tets.shape[1] != 4:
+            raise RuntimeError(f"{func}: expected tets of shape (num_tets, 4), got {list(tets.shape)}")
+        V, T = int(num_vertices), tets.shape[0]
+        if V < 0:
+            raise ValueError(f"{func}: num_vertices must be >= 0, got {V}")
+        nbytes = _lib.lib().dibr_b200_tet_topology_workspace_bytes(V, T)
+        if nbytes == 0:
+            raise RuntimeError(f"{func}: {V} vertices or {T} tets do not fit 32-bit indices")
+        dev = tets.device
+        tets = tets.contiguous()
+        i32 = dict(dtype=torch.int32, device=dev)
+        adj_ptr = torch.empty(V + 1, **i32)
+        adj = torch.empty(max(12 * T, 1), **i32)
+        edges = torch.empty((max(6 * T, 1), 2), **i32)
+        adj_edge = torch.empty(max(12 * T, 1), **i32)
+        tet_edge = torch.empty((max(T, 1), 6), **i32)
+        status = torch.empty(3, **i32)
+        ws = _lib.scratch(nbytes, dev)
+        _lib.call("dibr_b200_tet_topology_build", dev,
+                  V, T, tets, adj_ptr, adj, edges, adj_edge, tet_edge, status, ws, nbytes, what=func)
+        E, error, entries = status.tolist()              # the build's one device-to-host read
+        if error:
+            raise IndexError(f"{func}: tets holds an index outside [0, {V})")
+        self.num_vertices, self.num_tets, self.num_edges, self.tets = V, T, E, tets
+        self.adj_ptr, self.tet_edge = adj_ptr, tet_edge
+        self.adj, self.adj_edge, self.edges = _trim(adj, entries), _trim(adj_edge, entries), _trim(edges, E)
+
+
+class _TetSubdivide(torch.autograd.Function):
+    """x (B, V, 3) and f (B, V, D) -> (y (B, V + E, 3), yf (B, V + E, D)); fills new_tets (8T, 4)."""
+
+    @staticmethod
+    def forward(ctx, x, f, topo, new_tets):
+        ctx.set_materialize_grads(False)
+        B, V, D = x.shape[0], topo.num_vertices, f.shape[-1]
+        E = topo.num_edges
+        y = torch.empty((B, V + E, 3), dtype=torch.float32, device=x.device)
+        yf = torch.empty((B, V + E, D), dtype=torch.float32, device=x.device)
+        _lib.call("dibr_b200_tet_subdivide_forward", x.device,
+                  B, V, E, topo.num_tets, D, topo.edges, topo.tets, topo.tet_edge, x, f if D else None, y,
+                  yf if D else None, new_tets, what="subdivide_tetmesh")
+        ctx.topo, ctx.shape = topo, (B, V, D)
+        return y, yf
+
+    @staticmethod
+    def backward(ctx, gy, gyf):
+        topo = ctx.topo
+        B, V, D = ctx.shape
+        dev = topo.tets.device
+        gx = torch.empty((B, V, 3), dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] and gy is not None else None
+        gf = (torch.empty((B, V, D), dtype=torch.float32, device=dev)
+              if ctx.needs_input_grad[1] and gyf is not None and D else None)
+        if gx is not None or gf is not None:
+            _lib.call("dibr_b200_tet_subdivide_backward", dev,
+                      B, V, topo.num_edges, D, topo.adj_ptr, topo.adj, topo.adj_edge,
+                      None if gx is None else gy.contiguous(), None if gf is None else gyf.contiguous(), gx, gf,
+                      what="subdivide_tetmesh")
+        return gx, gf, None, None
+
+
+def subdivide_tetmesh(vertices, tetrahedrons, features=None):
+    r"""kaolin.ops.mesh.subdivide_tetmesh: each tetrahedron split into eight at its edge midpoints.
+
+    ``vertices`` (B, V, 3) float32 and the unbatched ``tetrahedrons`` (T, 4) int64 -> (vertices
+    (B, V + E, 3), tetrahedrons (8T, 4) int64), and the features (B, V + E, D) when ``features``
+    (B, V, D) float32 is given.  Edge e (the grid's unique edges in lexicographic order) becomes vertex
+    V + e, at the mean of its endpoints' positions and features; the eight child blocks follow the
+    reference's order.  Autograd flows to the vertices and the features, with no atomics.  The topology
+    is built on every call, as the reference does.
+
+    Deliberate deviations: only float32 vertices and features and int64 tetrahedrons are accepted; a
+    tet index outside [0, V) raises ``IndexError``.
+    """
+    func = "subdivide_tetmesh"
+    typed = [("vertices", vertices, torch.float32), ("tetrahedrons", tetrahedrons, torch.int64)]
+    if features is not None:
+        typed.append(("features", features, torch.float32))
+    _check(func, typed)
+    if vertices.dim() != 3 or vertices.shape[-1] != 3:
+        raise RuntimeError(f"{func}: expected vertices of shape (B, V, 3), got {list(vertices.shape)}")
+    B, V = vertices.shape[:2]
+    if features is not None and (features.dim() != 3 or tuple(features.shape[:2]) != (B, V)):
+        raise RuntimeError(f"{func}: expected features of shape ({B}, {V}, D), got {list(features.shape)}")
+    topo = _TetTopology(func, V, tetrahedrons)
+    new_tets = torch.empty((8 * topo.num_tets, 4), dtype=torch.int64, device=vertices.device)
+    f = vertices.new_empty((B, V, 0)) if features is None else features.contiguous()
+    y, yf = _TetSubdivide.apply(vertices.contiguous(), f, topo, new_tets)
+    return (y, new_tets) if features is None else (y, new_tets, yf)

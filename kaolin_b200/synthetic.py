@@ -114,6 +114,24 @@ def triangle_soup(batch, num_faces, seed=0, coverage=1.5):
     return fvz, fvi, fnz
 
 
+def freudenthal_grid(res):
+    """A tet grid over [-0.5, 0.5]^3: (res + 1)^3 vertices (V, 3) float32 and 6 res^3 tets (T, 4)
+    int64, each cube cell split into six tets around its diagonal (0,0,0)-(1,1,1) (the Freudenthal,
+    or Kuhn, triangulation), so neighbouring cells share their faces' diagonals."""
+    n = res + 1
+    g = np.arange(n, dtype=np.float64) / res - 0.5
+    verts = np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3).astype(np.float32)
+    i, j, k = (a.reshape(-1) for a in np.meshgrid(*(np.arange(res),) * 3, indexing="ij"))
+    idx = lambda a, b, c: ((i + a) * n + (j + b)) * n + (k + c)
+    unit = np.eye(3, dtype=np.int64)
+    tets = []
+    for p in ((0, 1, 2), (0, 2, 1), (1, 0, 2), (1, 2, 0), (2, 0, 1), (2, 1, 0)):
+        c1 = unit[p[0]]
+        c2 = c1 + unit[p[1]]
+        tets.append(np.stack([idx(0, 0, 0), idx(*c1), idx(*c2), idx(1, 1, 1)], 1))
+    return verts, np.stack(tets, 1).reshape(-1, 4).astype(np.int64)
+
+
 def random_features(batch, num_faces, dim, seed=0):
     rng = np.random.default_rng(seed + 7919)
     return rng.uniform(size=(batch, num_faces, 3, dim)).astype(np.float32)
