@@ -42,20 +42,19 @@
 
 #include "../../include/dibr_b200.h"
 #include "dibr_math.cuh"
+#include "workspace_layout.h"
 
 namespace {
 
 using namespace dibr;
+using namespace dibr_layout;
 
-constexpr int kTile = 16;
 constexpr int kThreads = 256;
 constexpr int kChunk = 256;
-constexpr int kMaxLevels = 6;   // 16 * 4^5 = 16384 px
 constexpr int kSoftCap = 1024;  // soft-mask candidates sorted per pass
 constexpr int kRound = 12;      // hits a pixel contributes to one pair round
 constexpr int kPairCap = kThreads * kRound;
 constexpr unsigned kFull = 0xffffffffu;
-constexpr int kBandRec = 24;    // ints per record of the soft-mask work list
 
 // ---------------------------------------------------------------------------
 // Scene description shared by all kernels (passed by value).
@@ -94,8 +93,6 @@ struct Scene {
   int* band_list;         // [B*nty*ntx][kBandRec] work list of the soft-mask kernels: per tile
                           //   {linear tile id, 8 x uncovered-pixel ballot, 6 x (large-bin offset, size), pad}
 };
-
-__host__ __device__ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // ---------------------------------------------------------------------------
 // Per-kernel timing for bench.py's roofline table (dibr_b200_trace_begin/_end):
@@ -1938,8 +1935,7 @@ struct RwCfg {
   // rows padded to an ODD number of 16-byte chunks: 8 consecutive rows then cover all 32 banks
   static constexpr int pad_odd(int bytes) { return ((bytes / 16) & 1) ? bytes : bytes + 16; }
   static constexpr int kIdxPitch = pad_odd(kRwSlab * 8);        // 32 -> 48
-  static constexpr int kVals = 6 + 3 * DT;
-  static constexpr int kAcc = (kVals + 3) & ~3;                 // floats per face record
+  static constexpr int kAcc = face_record_floats(DT);           // floats per face record
 };
 // upstream-gradient rows: fp32 (16*D bytes, 16-byte chunks) or bf16 (8*D bytes; D odd -> 8-byte chunks,
 // rows of 24 bytes are read with LDS.64: a half warp covers the 32 banks)
@@ -1950,8 +1946,6 @@ struct RwG {
   static constexpr int kPitch = kChunk == 16 ? RwCfg<DT>::pad_odd(kRow) : kRow;
   static constexpr int kStage = 32 * (RwCfg<DT>::kIdxPitch + kPitch);
 };
-constexpr int kAccMax = 20;  // D = 4
-
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
@@ -2235,55 +2229,6 @@ __global__ void __launch_bounds__(256) soft_bwd_lists_kernel(const __grid_consta
 
 // ---------------------------------------------------------------------------
 // Host side.
-int levels_for(int H, int W) {
-  int L = 1;
-  while ((kTile << (2 * (L - 1))) < (H > W ? H : W)) ++L;
-  return L;
-}
-
-int bins_per_view(int H, int W) {
-  int nb = 0;
-  const int L = levels_for(H, W);
-  for (int l = 0; l < L; ++l) {
-    const int t = kTile << (2 * l);
-    nb += ((W + t - 1) / t) * ((H + t - 1) / t);
-  }
-  return nb;
-}
-
-// Workspace layout (all pieces 256-byte aligned):
-//   cnt [2*B*NB] int + pool_ctr + fb_ctr + band_ctr | off [2*B*NB] int | fb_list, band_list [tiles] int |
-//   entries [2*4*NF] int4 | acc [NF][<=20] f32 (rasterize backward) | pool_hdr [pool_tiles] int4 |
-//   pool_data [pool_tiles][3][256*K] u32
-struct Layout {
-  size_t cnt, off, mode, ent, acc, base;
-  size_t acc_at() const { return cnt + off + mode + ent; }   // offset of the face records
-};
-
-Layout layout_for(int B, int64_t NF, int H, int W) {
-  Layout L;
-  const size_t tiles = (size_t)((W + kTile - 1) / kTile) * ((H + kTile - 1) / kTile) * B;
-  L.cnt = align_up(((size_t)2 * B * bins_per_view(H, W) + 3 + B + tiles) * sizeof(int), 256);
-  L.off = align_up((size_t)2 * B * bins_per_view(H, W) * sizeof(int), 256);
-  L.mode = align_up(tiles * sizeof(int), 256) + align_up(tiles * kBandRec * sizeof(int), 256);
-  L.ent = align_up((size_t)2 * 4 * (size_t)(NF > 0 ? NF : 1) * sizeof(int4), 256);
-  L.acc = align_up((size_t)(NF > 0 ? NF : 1) * kAccMax * sizeof(float) + 16, 256);  // rasterize-backward face records + job counter
-  L.base = L.cnt + L.off + L.mode + L.ent + L.acc + 256;
-  return L;
-}
-
-// The 256-byte aligned start of the layout's pieces in workspace `ws`, or nullptr when they do not fit.
-char* layout_origin(const Layout& Lo, void* ws, size_t ws_bytes) {
-  if (!ws) return nullptr;
-  char* p = (char*)align_up((size_t)ws, 256);
-  if (ws_bytes < Lo.base || p + Lo.acc_at() + Lo.acc > (char*)ws + ws_bytes) return nullptr;
-  return p;
-}
-
-size_t pool_block_bytes(int K) {
-  return sizeof(int4) + (size_t)3 * 256 * (size_t)K * sizeof(uint32_t);
-}
-
 int check_dims(int B, int64_t NF, int H, int W) {
   if (B <= 0 || H <= 0 || W <= 0 || NF < 0) return DIBR_B200_EINVAL;
   if (H > DIBR_B200_MAX_IMAGE_DIM || W > DIBR_B200_MAX_IMAGE_DIM || B > 65535) return DIBR_B200_ESIZE;
@@ -2291,16 +2236,17 @@ int check_dims(int B, int64_t NF, int H, int W) {
   return 0;
 }
 
-// knum > 0 enables the hit cache in whatever the workspace holds beyond the minimum.  The face
-// inputs (xy, z, first, validity, given bboxes) are left empty for the caller to fill in.
+// Carves the scene's pieces out of the workspace (workspace_layout.h).  knum > 0 enables the hit
+// cache in whatever the workspace holds beyond the minimum; f64 adds the float scene of a float64
+// call, which f64_bins fills in.  The other face inputs (xy, z, first, validity, given bboxes) are
+// left empty for the caller to fill in.
 int setup_scene(Scene& s, int B, int64_t NF, int F, int H, int W, float multiplier, float margin,
-                int knum, void* ws, size_t ws_bytes) {
+                int knum, bool f64, void* ws, size_t ws_bytes) {
   if (!(multiplier > 0.f)) return DIBR_B200_EINVAL;
   if (!ws) return DIBR_B200_EINVAL;
-  const Layout Lo = layout_for(B, NF, H, W);
-  char* p = layout_origin(Lo, ws, ws_bytes);
-  char* const end = (char*)ws + ws_bytes;
-  if (!p) return DIBR_B200_EWORKSPACE;
+  const WorkspaceLayout L = workspace_layout({B, NF, H, W, knum, f64}, ws, ws_bytes);
+  if (!L.fits) return DIBR_B200_EWORKSPACE;
+  char* const o = (char*)ws + L.origin;
   s.first = nullptr; s.xy = nullptr; s.z = nullptr; s.premultiplied = 0;
   s.fnz = nullptr; s.valid = nullptr; s.bbox_tight = nullptr; s.bbox_large = nullptr;
   s.B = B; s.H = H; s.W = W; s.F = F; s.NF = NF;
@@ -2317,40 +2263,31 @@ int setup_scene(Scene& s, int B, int64_t NF, int F, int H, int W, float multipli
   }
   s.NB = nb;
   if ((int64_t)2 * B * nb >= 0x7fffffffLL) return DIBR_B200_ESIZE;  // counter ids are 32-bit
-  s.cnt = (int*)p;
-  s.pool_ctr = s.cnt + (size_t)2 * B * nb;
-  s.fb_ctr = s.pool_ctr + 1;
-  s.band_ctr = s.pool_ctr + 2;
-  s.view_flag = s.pool_ctr + 3;
-  s.tile_cnt = s.view_flag + B;
-  p += Lo.cnt;
-  s.off = (int*)p; p += Lo.off;
-  s.fb_list = (int*)p;
-  s.band_list = (int*)(p + align_up((size_t)s.ntx[0] * s.nty[0] * B * sizeof(int), 256));
-  p += Lo.mode;
-  s.entries = (int4*)p; p += Lo.ent;
-  p += Lo.acc;   // face records of the rasterize backward (acc_region)
-  s.pool_tiles = 0; s.pool_K = knum > 0 ? knum : 1; s.pool_hdr = nullptr; s.pool_data = nullptr;
-  if (knum > 0) {
-    const size_t left = (size_t)(end - p);
-    const size_t data = (size_t)3 * 256 * (size_t)knum * sizeof(uint32_t);
-    auto need = [&](size_t n) { return align_up(n * sizeof(int4), 256) + n * data; };
-    size_t n = left / pool_block_bytes(knum);
-    const size_t tiles = (size_t)s.ntx[0] * s.nty[0] * B;
-    if (n > tiles) n = tiles;
-    while (n > 0 && need(n) > left) --n;
-    if (n > 0) {
-      s.pool_tiles = (int)n;
-      s.pool_hdr = (int4*)p; p += align_up(n * sizeof(int4), 256);
-      s.pool_data = (uint32_t*)p;
-    }
+  s.cnt = (int*)(o + L.cnt.at);
+  s.pool_ctr = (int*)(o + L.pool_ctr.at);
+  s.fb_ctr = (int*)(o + L.fb_ctr.at);
+  s.band_ctr = (int*)(o + L.band_ctr.at);
+  s.view_flag = (int*)(o + L.view_flag.at);
+  s.tile_cnt = (int*)(o + L.tile_cnt.at);
+  s.off = (int*)(o + L.off.at);
+  s.fb_list = (int*)(o + L.fb_list.at);
+  s.band_list = (int*)(o + L.band_list.at);
+  s.entries = (int4*)(o + L.entries.at);
+  s.pool_tiles = (int)L.cache_tiles; s.pool_K = knum > 0 ? knum : 1;
+  s.pool_hdr = L.cache_tiles ? (int4*)(o + L.cache_hdr.at) : nullptr;
+  s.pool_data = L.cache_tiles ? (uint32_t*)(o + L.cache_data.at) : nullptr;
+  if (f64) {
+    s.xy = (float*)(o + L.xy.at); s.premultiplied = 1;
+    s.bbox_tight = (float*)(o + L.bbox_tight.at);
+    s.bbox_large = (float*)(o + L.bbox_large.at);
+    s.valid = (uint8_t*)(o + L.valid.at);
   }
   return 0;
 }
 
 int build_bins(const Scene& s, int sets, cudaStream_t st) {
-  const size_t zero_ints = (size_t)2 * s.B * s.NB + 3 + s.B + (size_t)s.ntx[0] * s.nty[0] * s.B;
-  cudaError_t e = cudaMemsetAsync(s.cnt, 0, zero_ints * sizeof(int), st);
+  const Piece counters = workspace_layout({s.B, s.NF, s.H, s.W, 0, false}, 0).counters;
+  cudaError_t e = cudaMemsetAsync(s.cnt, 0, counters.bytes, st);
   if (e != cudaSuccess) return (int)e;
   if (s.NF > 0) {
     const bool agg = s.NF / s.B >= (int64_t)32 * s.ntx[0] * s.nty[0];
@@ -2469,18 +2406,10 @@ int launch_raster_bwd(const RasterBwdArgs& a, cudaStream_t st) {
   return (int)cudaGetLastError();
 }
 
-// The face-record region of a workspace (nullptr: none / too small -> warp-reduction kernel).
-float* acc_region(void* ws, size_t ws_bytes, int B, int64_t NF, int H, int W) {
-  const Layout Lo = layout_for(B, NF, H, W);
-  char* p = layout_origin(Lo, ws, ws_bytes);
-  return p ? (float*)(p + Lo.acc_at()) : nullptr;
-}
-
 template <int DT, typename FT>
-int launch_rows_t(const RowBwdArgs& a0, int64_t NF, float* g_xy, float* g_ff, int accumulate_xy, cudaStream_t st) {
-  RowBwdArgs a = a0;
-  a.job_ctr = reinterpret_cast<int*>(a.acc + (size_t)NF * RwCfg<DT>::kAcc);   // kAcc <= 16 < kAccMax: room behind the records
-  cudaError_t e = cudaMemsetAsync(a.acc, 0, (size_t)NF * RwCfg<DT>::kAcc * sizeof(float) + sizeof(int), st);
+int launch_rows_t(const RowBwdArgs& a, int64_t NF, float* g_xy, float* g_ff, int accumulate_xy, cudaStream_t st) {
+  // the face records and the job counter right behind them
+  cudaError_t e = cudaMemsetAsync(a.acc, 0, (size_t)((char*)(a.job_ctr + 1) - (char*)a.acc), st);
   if (e != cudaSuccess) return (int)e;
   {
     Span sp("raster_bwd_rows_kernel", st);
@@ -2498,11 +2427,12 @@ int launch_rows_t(const RowBwdArgs& a0, int64_t NF, float* g_xy, float* g_ff, in
 // Row-walk rasterize backward: one warp per 32 rows x strip columns; the strip is as long as
 // still leaves a few waves of single-warp CTAs (longer strips = fewer cut face runs).
 template <typename FT>
-int launch_raster_bwd_rows(const RasterBwdArgs& r, float* acc, int accumulate_xy, cudaStream_t st) {
+int launch_raster_bwd_rows(const RasterBwdArgs& r, float* acc, int* job_ctr, int accumulate_xy, cudaStream_t st) {
   RowBwdArgs a;
   a.B = r.B; a.H = r.H; a.W = r.W; a.F = r.F;
   a.grad_feat = r.grad_feat; a.idx = r.idx; a.w = r.w; a.xy = r.xy;
-  a.feat = r.feat; a.grid = r.grid; a.rc = r.rc; a.multiplier = r.multiplier; a.acc = acc;
+  a.feat = r.feat; a.grid = r.grid; a.rc = r.rc; a.multiplier = r.multiplier;
+  a.acc = acc; a.job_ctr = job_ctr;
   a.jobs_y = (r.H + 31) / 32;
   int strip = 32;   // H100, c4_shard: strips of 16 / 64 columns 1 % faster / 8 % slower
   while (strip > kRwSlab && (int64_t)r.B * a.jobs_y * ((r.W + strip - 1) / strip) < 8192) strip >>= 1;
@@ -2570,7 +2500,7 @@ int check_backward(bool f64, int B, int F, int H, int W, int D, const void* grad
   if (raster && (!ff || !g_ff || !(output_weights || (!f64 && multiplier > 0.f)))) return DIBR_B200_EINVAL;
   if (!soft_ok) return DIBR_B200_EINVAL;
   if (f64) return raster || grad_soft_mask ? f64_scene(s, B, F, H, W, multiplier, ws, ws_bytes) : 0;
-  return grad_soft_mask ? setup_scene(s, B, NF, F, H, W, multiplier, boxlen_m, knum, ws, ws_bytes) : 0;
+  return grad_soft_mask ? setup_scene(s, B, NF, F, H, W, multiplier, boxlen_m, knum, false, ws, ws_bytes) : 0;
 }
 
 }  // namespace
@@ -2594,7 +2524,7 @@ extern "C" {
 
 size_t dibr_b200_workspace_bytes_f64(int batch, int64_t total_faces, int height, int width) {
   if (check_dims(batch, total_faces, height, width)) return 0;
-  return f64_layout(batch, total_faces, height, width).total;
+  return workspace_layout({batch, total_faces, height, width, 0, true}, 0).bytes;
 }
 
 int dibr_b200_forward_f64(int batch, int num_faces, int height, int width, int feat_dim,
@@ -2698,16 +2628,13 @@ int dibr_b200_version(void) { return 200; }
 
 size_t dibr_b200_workspace_bytes(int batch, int64_t total_faces, int height, int width) {
   if (check_dims(batch, total_faces, height, width)) return 0;
-  return layout_for(batch, total_faces, height, width).base;
+  return workspace_layout({batch, total_faces, height, width, 0, false}, 0).bytes;
 }
 
 size_t dibr_b200_workspace_bytes_cached(int batch, int64_t total_faces, int height, int width,
                                         int knum, int64_t cache_tiles) {
   if (check_dims(batch, total_faces, height, width) || knum <= 0 || cache_tiles < 0) return 0;
-  const int64_t tiles = (int64_t)((width + kTile - 1) / kTile) * ((height + kTile - 1) / kTile) * batch;
-  if (cache_tiles > tiles) cache_tiles = tiles;
-  return layout_for(batch, total_faces, height, width).base + 512 +
-         (size_t)cache_tiles * pool_block_bytes(knum);
+  return workspace_layout({batch, total_faces, height, width, knum, false}, cache_tiles).bytes;
 }
 
 static int forward_impl(int batch, int num_faces, int height, int width, int feat_dim,
@@ -2726,7 +2653,7 @@ static int forward_impl(int batch, int num_faces, int height, int width, int fea
   cudaStream_t st = (cudaStream_t)stream;
   FwdArgs a;
   Scene& s = a.s;
-  rc = setup_scene(s, batch, NF, num_faces, height, width, multiplier, boxlen_m, soft ? knum : 0,
+  rc = setup_scene(s, batch, NF, num_faces, height, width, multiplier, boxlen_m, soft ? knum : 0, false,
                    workspace, workspace_bytes_);
   if (rc) return rc;
   s.xy = face_vertices_image; s.z = face_vertices_z; s.fnz = face_normals_z; s.valid = valid_faces;
@@ -2797,8 +2724,14 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
   float* const g_ff_v = grad_face_features ? grad_face_features + (size_t)view_begin * num_faces * 3 * feat_dim : nullptr;
   // row-walk kernel: fp32 or bf16 features, D <= 4, rows a multiple of 4 px, a workspace with the face records
   float* acc = nullptr;
-  if (run_raster && feat_dim <= 4 && (width % kRwSlab) == 0 && NF > 0)
-    acc = acc_region(workspace, workspace_bytes_, batch, NF, height, width);
+  int* job_ctr = nullptr;
+  if (run_raster && feat_dim <= kRowWalkMaxD && (width % kRwSlab) == 0 && NF > 0) {
+    const WorkspaceLayout L = workspace_layout({batch, NF, height, width, 0, false}, workspace, workspace_bytes_);
+    if (L.fits) {
+      acc = (float*)((char*)workspace + L.origin + L.face_records.at);
+      job_ctr = (int*)((char*)workspace + L.origin + L.job_ctr(NFv, feat_dim).at);
+    }
+  }
   if (!(flags & DIBR_B200_ACCUMULATE) && !acc) {
     e = cudaMemsetAsync(g_xy_v, 0, (size_t)NFv * 6 * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
@@ -2820,8 +2753,8 @@ static int backward_impl(int batch, int num_faces, int height, int width, int fe
     a.grid = make_grid(multiplier, width, height); a.rc = make_raster_const(eps); a.multiplier = multiplier;
     a.grad_xy = g_xy_v;
     a.grad_feat_out = g_ff_v;
-    if (acc) rc = bf16 ? launch_raster_bwd_rows<__nv_bfloat16>(a, acc, (flags & DIBR_B200_ACCUMULATE) ? 1 : 0, st)
-                       : launch_raster_bwd_rows<float>(a, acc, (flags & DIBR_B200_ACCUMULATE) ? 1 : 0, st);
+    if (acc) rc = bf16 ? launch_raster_bwd_rows<__nv_bfloat16>(a, acc, job_ctr, (flags & DIBR_B200_ACCUMULATE) ? 1 : 0, st)
+                       : launch_raster_bwd_rows<float>(a, acc, job_ctr, (flags & DIBR_B200_ACCUMULATE) ? 1 : 0, st);
     else rc = bf16 ? launch_raster_bwd<__nv_bfloat16>(a, st) : launch_raster_bwd<float>(a, st);
     if (rc) return rc;
   }
@@ -2911,7 +2844,7 @@ int dibr_b200_packed_rasterize_forward(int batch, int64_t total_faces, int heigh
   cudaStream_t st = (cudaStream_t)stream;
   FwdArgs a;
   Scene& s = a.s;
-  rc = setup_scene(s, batch, total_faces, 0, height, width, multiplier, 0.f, 0, workspace, workspace_bytes_);
+  rc = setup_scene(s, batch, total_faces, 0, height, width, multiplier, 0.f, 0, false, workspace, workspace_bytes_);
   if (rc) return rc;
   s.first = first_idx_face_per_mesh; s.xy = face_vertices_image; s.z = face_vertices_z;
   s.premultiplied = 1; s.bbox_tight = face_bboxes;
@@ -2959,7 +2892,7 @@ int dibr_b200_soft_mask_forward(int batch, int num_faces, int height, int width,
   cudaStream_t st = (cudaStream_t)stream;
   FwdArgs a;
   Scene& s = a.s;
-  rc = setup_scene(s, batch, NF, num_faces, height, width, multiplier, 0.f, 0, workspace, workspace_bytes_);
+  rc = setup_scene(s, batch, NF, num_faces, height, width, multiplier, 0.f, 0, false, workspace, workspace_bytes_);
   if (rc) return rc;
   s.xy = face_vertices_image; s.premultiplied = 1; s.bbox_large = face_large_bboxes;
   rc = build_bins(s, 2, st);

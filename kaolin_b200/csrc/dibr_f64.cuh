@@ -188,34 +188,12 @@ __global__ void __launch_bounds__(kThreads) dibr_f64_kernel(const __grid_constan
   }
 }
 
-struct F64Layout { size_t base, xyf, bt, bl, valid, total; };
-F64Layout f64_layout(int B, int64_t NF, int H, int W) {
-  F64Layout L;
-  const size_t n = (size_t)(NF > 0 ? NF : 1);
-  L.base = align_up(layout_for(B, NF, H, W).base, 256);
-  L.xyf = align_up(n * 6 * sizeof(float), 256);
-  L.bt = align_up(n * 4 * sizeof(float), 256);
-  L.bl = L.bt;
-  L.valid = align_up(n, 256);
-  L.total = L.base + L.xyf + L.bt + L.bl + L.valid + 256;
-  return L;
-}
-
 // Lays out the float scene of a double call (scaled vertices, conservative bboxes, validity) in the
-// workspace.  Host only: nothing is enqueued.  `multiplier` is the C float the reference's kernels
-// take: it places the pixel centres.
+// workspace, after setup_scene's pieces; a null workspace is too small.  Host only: nothing is
+// enqueued.  `multiplier` is the C float the reference's kernels take: it places the pixel centres.
 int f64_scene(Scene& s, int B, int F, int H, int W, float multiplier, void* ws, size_t ws_bytes) {
-  const int64_t NF = (int64_t)B * F;
-  const F64Layout L = f64_layout(B, NF, H, W);
-  char* p = (char*)align_up((size_t)ws, 256);
-  if (!ws || ws_bytes < L.total || p + L.total - 256 > (char*)ws + ws_bytes) return DIBR_B200_EWORKSPACE;
-  int rc = setup_scene(s, B, NF, F, H, W, multiplier, 0.f, 0, p, L.base);
-  if (rc) return rc;
-  s.xy = (float*)(p + L.base); s.premultiplied = 1;
-  s.bbox_tight = (float*)(p + L.base + L.xyf);
-  s.bbox_large = (float*)(p + L.base + L.xyf + L.bt);
-  s.valid = (uint8_t*)(p + L.base + L.xyf + L.bt + L.bl);
-  return 0;
+  if (!ws) return DIBR_B200_EWORKSPACE;
+  return setup_scene(s, B, (int64_t)B * F, F, H, W, multiplier, 0.f, 0, true, ws, ws_bytes);
 }
 
 // Fills the float scene laid out by f64_scene from the double inputs, scaled by the double
