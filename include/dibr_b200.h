@@ -365,6 +365,45 @@ int dibr_b200_deftet_sparse_render_backward(
     float* grad_face_vertices_image, float* grad_face_features, dibr_b200_stream_t stream);
 
 /*
+ * Point-in-mesh test (kaolin/ops/mesh/check_sign.py:45-57,104-155; kaolin_b200/csrc/check_sign.cu).
+ * Operator: kaolin::unbatched_mesh_intersection_cuda (kaolin/csrc/ops/mesh/mesh_intersection.cpp:32-65,
+ * kernel mesh_intersection_cuda.cu:105-219; registered at bindings.cpp:49).  A face counts for a point q
+ * when q's (y, z) lies in the face's closed y-z box (float bounds, NaN skipped), the signed volumes of q
+ * and (q.x + 10, q.y, q.z) against it differ in sign, the three 2-D signed areas admit q and the
+ * edge/vertex tie-break accepts it; every step is rounded as the reference's compiled kernel rounds it.
+ * `dtype` is DIBR_B200_DTYPE_F32 or DIBR_B200_DTYPE_F64 and types every float argument (void*).
+ *
+ * dibr_b200_check_sign_workspace_bytes: the bytes of the build workspace ("mesh") of `batch` views of
+ *   `num_faces` faces, and of the query workspace for `num_points` points per view.  Returns 0, or
+ *   DIBR_B200_EINVAL / DIBR_B200_ESIZE (B*F*16 or B*N not below 2^31 - 1).
+ * dibr_b200_check_sign_build: verts (B, V, 3), faces (F, 3) int64.  Per view, maxlen = max over axes of
+ *   (max - min) over all V vertices, NaN propagating (check_sign.py:138-141); each face's corners
+ *   verts[b][faces[f][k]] / maxlen (correctly rounded) go to one record, its y-z box to the grid of
+ *   the view (G x G cells, G from F).  status (1) int32 is set non-zero when a face index lies outside
+ *   [0, V) (the mesh is then not usable); it is the one value to read back.
+ * dibr_b200_check_sign_query: points (B, N, 3) against a built mesh of the same B and F: points / maxlen,
+ *   then inside (B, N) uint8 = count % 2, fully written, in input order.  No host synchronisation.
+ * dibr_b200_mesh_intersection_count: the raw operator, one view: points (N, 3) and the pre-gathered,
+ *   already normalised corners verts_1, verts_2, verts_3 (F, 3), no index check, no normalisation;
+ *   counts (N) of `dtype`.  workspace >= build_bytes + query_bytes of (1, F, N).
+ * Negative sizes, a bad dtype or a NULL buffer that is used give DIBR_B200_EINVAL; a workspace below its
+ * size DIBR_B200_EWORKSPACE.  F = 0 leaves every point outside.
+ */
+#define DIBR_B200_DTYPE_F32 0
+#define DIBR_B200_DTYPE_F64 1
+int dibr_b200_check_sign_workspace_bytes(int batch, int num_faces, int num_points, int dtype, size_t* build_bytes,
+                                         size_t* query_bytes);
+int dibr_b200_check_sign_build(int batch, int num_vertices, int num_faces, int dtype, const void* verts,
+                               const int64_t* faces, int32_t* status, void* workspace, size_t workspace_bytes,
+                               dibr_b200_stream_t stream);
+int dibr_b200_check_sign_query(int batch, int num_faces, int num_points, int dtype, const void* points,
+                               const void* mesh, size_t mesh_bytes, uint8_t* inside, void* workspace,
+                               size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_mesh_intersection_count(int num_faces, int num_points, int dtype, const void* points,
+                                      const void* verts_1, const void* verts_2, const void* verts_3, void* counts,
+                                      void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
  * Diffuse lighting (kaolin/render/lighting/sg.py, sh.py; kaolin_b200/csrc/lighting.cu).
  *
  * General reduced SG inner product, the operator kaolin::unbatched_reduced_sg_inner_product_

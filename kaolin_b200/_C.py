@@ -1,6 +1,8 @@
 """``kaolin_b200._C.render.mesh`` — the four operators the reference registers in
 kaolin/csrc/bindings.cpp:111-115, with identical names, argument order/meaning,
-return structure and error behaviour, implemented by libdibr_b200.so.
+return structure and error behaviour, implemented by libdibr_b200.so; likewise
+``_C.render.sg``, the DefTet pair and ``_C.ops.mesh.unbatched_mesh_intersection_cuda``
+(bindings.cpp:49), which the reference's ``check_sign.py`` calls.
 
 This is what makes the library a drop-in *below* the reference's own Python
 wrappers: ``kaolin.render.mesh.rasterization`` / ``.dibr`` run unmodified with
@@ -263,6 +265,36 @@ def unbatched_reduced_sg_inner_product_backward_cuda(grad_out, intensity, direct
     _check_sg("unbatched_reduced_sg_inner_product_backward_cuda", args)
     return sg.backward_sg_inner_product(*[t for _, t in args])
 
+
+def unbatched_mesh_intersection_cuda(points, verts_1, verts_2, verts_3):
+    """mesh_intersection.cpp:32-65 -> counts (num_points,) of the points' type: for each point, the faces
+    (verts_1[f], verts_2[f], verts_3[f]) its +x ray crosses, as the reference's kernel counts them
+    (check_sign's corners, gathered and normalised by the caller).  float32 or float64."""
+    fn = "unbatched_mesh_intersection_cuda"
+    named = [("points", points), ("verts_1", verts_1), ("verts_2", verts_2), ("verts_3", verts_3)]
+    dev = _check_all(fn, named, float_dtype=points.dtype)
+    if len({t.dtype for _, t in named}) > 1:
+        raise RuntimeError(f"{fn}: expected all tensors to have the same type, "
+                           f"got {[str(t.dtype) for _, t in named]}")
+    num_points, num_faces = points.shape[0], verts_1.shape[0]
+    _check_size(fn, "points", points, (num_points, 3))
+    for name, t in named[1:]:
+        _check_size(fn, name, t, (num_faces, 3))
+    dtype = {torch.float32: _lib.DTYPE_F32, torch.float64: _lib.DTYPE_F64}.get(points.dtype)
+    if dtype is None:
+        raise RuntimeError(f"{fn} not implemented for '{str(points.dtype).replace('torch.', '')}'")
+    out = torch.empty((num_points,), dtype=points.dtype, device=dev)
+    build, query = _lib.check_sign_workspace_bytes(1, num_faces, num_points, dtype, fn)
+    ws = _lib.scratch(build + query, dev)
+    _lib.call("dibr_b200_mesh_intersection_count", dev, num_faces, num_points, dtype, points, verts_1, verts_2,
+              verts_3, out, ws, ws.numel(), what=fn)
+    return out
+
+
+# kaolin._C.ops.mesh.<op>, as bindings.cpp:43,48-49 lays it out
+ops = types.SimpleNamespace(mesh=types.SimpleNamespace(
+    unbatched_mesh_intersection_cuda=unbatched_mesh_intersection_cuda,
+))
 
 # kaolin._C.render.{mesh,sg}.<op> namespaces, as bindings.cpp:42,111-115,129-133 lays them out
 render = types.SimpleNamespace(sg=types.SimpleNamespace(

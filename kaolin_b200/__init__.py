@@ -11,7 +11,9 @@ compute_vertex_normals}``, ``metrics.trianglemesh.uniform_laplacian_smoothing``,
 subdivision (``ops.mesh.subdivide_trianglemesh`` and ``ops.mesh.LoopSubdivision``, which builds its
 levels once), and DMTet's tet-grid operators (``ops.conversions.marching_tetrahedra``,
 ``ops.conversions.MarchingTetrahedra``, which builds the grid's topology once, and
-``ops.mesh.subdivide_tetmesh``); see DESIGN.md for scope.  There is no CPU fallback: every entry point
+``ops.mesh.subdivide_tetmesh``), and the point-in-mesh test (``ops.mesh.check_sign``,
+``ops.mesh.CheckSign``, which builds the mesh once, and ``_C.ops.mesh.unbatched_mesh_intersection_cuda``);
+see DESIGN.md for scope.  There is no CPU fallback: every entry point
 raises if the CUDA library (kaolin_b200/csrc, built in-tree) is missing or the
 tensors are not on a CUDA device.
 """

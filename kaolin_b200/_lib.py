@@ -16,9 +16,11 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libdibr_b200.so")
 SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline.cu"),
            os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
-           os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu")]
+           os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu"),
+           os.path.join(CSRC, "check_sign.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
+           os.path.join(CSRC, "grid_bins.cuh"),
            os.path.join(_HERE, "..", "include", "dibr_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -27,6 +29,7 @@ EINVAL, EWORKSPACE, ESIZE = -1, -3, -4
 RASTER, SOFT_MASK = 1, 2
 LIGHT_SG_INNER_PRODUCT, LIGHT_SG_FITTED, LIGHT_SH9 = 0, 1, 2     # dibr_b200_diffuse_* models
 BINS_VALID, ACCUMULATE = 1, 2      # dibr_b200_backward flags
+DTYPE_F32, DTYPE_F64 = 0, 1        # dibr_b200_check_sign_* and dibr_b200_mesh_intersection_count
 
 _lock = threading.Lock()
 _lib = None
@@ -124,6 +127,11 @@ SIGNATURES = {
     "dibr_b200_marching_tets_backward": (_i, [_i, _i, _i] + [_vp] * 9 + [_vp]),
     "dibr_b200_tet_subdivide_forward": (_i, [_i, _i, _i, _i64, _i] + [_vp] * 8 + [_vp]),
     "dibr_b200_tet_subdivide_backward": (_i, [_i, _i, _i, _i] + [_vp] * 7 + [_vp]),
+    # point-in-mesh test (ops.mesh.check_sign, CheckSign, _C.ops.mesh; csrc/check_sign.cu)
+    "dibr_b200_check_sign_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz), ctypes.POINTER(_sz)]),
+    "dibr_b200_check_sign_build": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dibr_b200_check_sign_query": (_i, [_i, _i, _i, _i, _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
+    "dibr_b200_mesh_intersection_count": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 
@@ -227,6 +235,14 @@ def marching_tets_case_table():
     out = (ctypes.c_int32 * (16 * 12))()
     check(lib().dibr_b200_marching_tets_case_table(out), "marching_tets_case_table")
     return list(out)
+
+
+def check_sign_workspace_bytes(batch, num_faces, num_points, dtype, what):
+    """(build bytes, query bytes) of ``dibr_b200_check_sign_workspace_bytes``; raises on its status."""
+    build, query = _sz(0), _sz(0)
+    check(lib().dibr_b200_check_sign_workspace_bytes(batch, num_faces, num_points, dtype, ctypes.byref(build),
+                                                     ctypes.byref(query)), what)
+    return build.value, query.value
 
 
 def scratch(nbytes, device):

@@ -11,8 +11,8 @@
 // the rest of the (B,P,K) arrays is -1 / 0.  The reference scans ALL faces for every point
 // (O(P*F) bbox tests, one warp per point).  Here:
 //   * the faces of a view are binned once into a uniform G x G grid laid over the bounding box of
-//     the query points (count -> scan -> fill; faces that cover more than kMaxCells cells go to a
-//     short per-view "wide" list instead);
+//     the query points (grid_bins.cuh: count -> scan -> fill; faces that cover more than kMaxCells
+//     cells go to a short per-view "wide" list instead);
 //   * one warp per point reads only its cell's faces + the wide list, 32 candidates per step, the
 //     hits are compacted with a ballot into shared memory, sorted by face index (they are few) and
 //     written in that order — the reference's order;
@@ -32,24 +32,15 @@
 
 #include "../../include/dibr_b200.h"
 #include "dibr_math.cuh"
+#include "grid_bins.cuh"
 
 namespace {
 
 using namespace dibr;
 
-constexpr int kMaxCells = 16;     // cells a face may be inserted in; wider faces -> the view's wide list
 constexpr int kHitCap = 128;      // hits a point can collect before it takes the ordered scan
 constexpr int kWarps = 8;         // points per CTA
 constexpr unsigned kFull = 0xffffffffu;
-
-struct Grid {
-  int B, F, P, G;
-  const float* bounds;   // [B][4] xmin, ymin, 1/cell_w, 1/cell_h
-  int* cnt;              // [B][G*G + 1] (last: wide list length)
-  int* off;              // [B][G*G + 1]
-  int* entries;          // [B][F*kMaxCells]
-  int* wide;             // [B][F]
-};
 
 __global__ void deftet_bounds_kernel(int B, int P, int G, const float* __restrict__ pix, float* __restrict__ bounds) {
   const int b = blockIdx.x;
@@ -75,78 +66,6 @@ __global__ void deftet_bounds_kernel(int B, int P, int G, const float* __restric
     const float wx = fmaxf(x1 - x0, 1e-20f), wy = fmaxf(y1 - y0, 1e-20f);
     float* o = bounds + 4 * b;
     o[0] = x0; o[1] = y0; o[2] = (float)G / wx; o[3] = (float)G / wy;
-  }
-}
-
-__device__ __forceinline__ int cell_of(float v, float lo, float inv, int G) {
-  const float c = (v - lo) * inv;
-  // NaN -> 0; the clamp keeps points on the upper border (and anything outside) in range
-  return (int)fminf(fmaxf(c, 0.f), (float)(G - 1));
-}
-
-// cells whose points can pass the half-open bbox test  x0 >= xmin && x0 < xmax  (conservative)
-__device__ __forceinline__ bool face_cells(const Grid& g, int b, int64_t face, const float* bbox, int& cx0, int& cx1,
-                                           int& cy0, int& cy1) {
-  const float4 bb = __ldg(reinterpret_cast<const float4*>(bbox) + face);
-  const float* bd = g.bounds + 4 * b;
-  if (!(bb.z > bb.x) || !(bb.w > bb.y)) return false;   // empty or NaN box: no point can be inside
-  cx0 = cell_of(bb.x, bd[0], bd[2], g.G); cx1 = cell_of(bb.z, bd[0], bd[2], g.G);
-  cy0 = cell_of(bb.y, bd[1], bd[3], g.G); cy1 = cell_of(bb.w, bd[1], bd[3], g.G);
-  return true;
-}
-
-template <bool FILL>
-__global__ void __launch_bounds__(256) deftet_bin_kernel(Grid g, const float* __restrict__ bbox) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (int64_t)g.B * g.F) return;
-  const int b = (int)(i / g.F), f = (int)(i - (int64_t)b * g.F);
-  int cx0, cx1, cy0, cy1;
-  if (!face_cells(g, b, i, bbox, cx0, cx1, cy0, cy1)) return;
-  const int ncell = g.G * g.G;
-  int* cnt = g.cnt + (size_t)b * (ncell + 1);
-  if ((cx1 - cx0 + 1) * (cy1 - cy0 + 1) > kMaxCells) {
-    const int pos = atomicAdd(cnt + ncell, 1);
-    if (FILL) g.wide[(size_t)b * g.F + pos] = f;
-    return;
-  }
-  for (int cy = cy0; cy <= cy1; ++cy)
-    for (int cx = cx0; cx <= cx1; ++cx) {
-      const int c = cy * g.G + cx;
-      const int pos = atomicAdd(cnt + c, 1);
-      if (FILL) g.entries[(size_t)b * g.F * kMaxCells + g.off[(size_t)b * (ncell + 1) + c] + pos] = f;
-    }
-}
-
-// exclusive scan of the G*G cell counters of one view (the wide-list counter is only reset)
-__global__ void __launch_bounds__(1024) deftet_scan_kernel(Grid g) {
-  __shared__ int warp_sums[32];
-  __shared__ int carry;
-  const int ncell = g.G * g.G;
-  int* cnt = g.cnt + (size_t)blockIdx.x * (ncell + 1);
-  int* off = g.off + (size_t)blockIdx.x * (ncell + 1);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) { carry = 0; off[ncell] = cnt[ncell]; cnt[ncell] = 0; }   // off[ncell] keeps the wide length
-  __syncthreads();
-  for (int base = 0; base < ncell; base += 1024) {
-    const int i = base + tid;
-    const int v = i < ncell ? cnt[i] : 0;
-    int x = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(kFull, x, d); if (lane >= d) x += y; }
-    if (lane == 31) warp_sums[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-      int w = warp_sums[lane];
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(kFull, w, d); if (lane >= d) w += y; }
-      warp_sums[lane] = w;
-    }
-    __syncthreads();
-    const int excl = carry + (warp ? warp_sums[warp - 1] : 0) + x - v;
-    if (i < ncell) { off[i] = excl; cnt[i] = 0; }
-    __syncthreads();
-    if (tid == 1023) carry = excl + v;
-    __syncthreads();
   }
 }
 
@@ -301,12 +220,6 @@ __global__ void __launch_bounds__(256) deftet_backward_kernel(const __grid_const
   atomicAdd(gx + 2, make_float2(v[4], v[5]));
 }
 
-int grid_side(int F) {
-  int G = 8;
-  while (G < 256 && (int64_t)G * G < F) G += 8;   // ~1 face per cell before overlaps
-  return G;
-}
-
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 struct Layout { size_t bounds, cnt, off, entries, wide, total; };
@@ -359,9 +272,9 @@ int dibr_b200_deftet_sparse_render_forward(int batch, int num_faces, int num_pix
   deftet_bounds_kernel<<<batch, 256, 0, st>>>(batch, num_pixels, g.G, pixel_coords, const_cast<float*>(g.bounds));
   const int64_t nf = (int64_t)batch * num_faces;
   if (nf > 0) {
-    deftet_bin_kernel<false><<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(g, face_bboxes);
-    deftet_scan_kernel<<<batch, 1024, 0, st>>>(g);
-    deftet_bin_kernel<true><<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(g, face_bboxes);
+    grid_bin_kernel<false, false><<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(g, face_bboxes);
+    grid_scan_kernel<<<batch, 1024, 0, st>>>(g);
+    grid_bin_kernel<false, true><<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(g, face_bboxes);
   } else {
     e = cudaMemsetAsync(g.off, 0, L.off, st);
     if (e != cudaSuccess) return (int)e;

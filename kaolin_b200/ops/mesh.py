@@ -22,6 +22,13 @@ once and applies them with autograd to the vertices and a learnable per-vertex a
 
 ``subdivide_tetmesh`` (tetmesh.py:85-181) refines a tet grid on the topology of its tets, which
 marching tetrahedra (``kaolin_b200.ops.conversions``) shares.
+
+``check_sign`` (check_sign.py) labels points inside or outside a watertight mesh, equal to the
+reference's CUDA operator bit for bit, with its faces binned on a y-z grid instead of tested against
+every point (csrc/check_sign.cu); ``CheckSign`` builds the mesh once for many point sets::
+
+    S = CheckSign(verts, faces)               # Simplicits, occupancy sampling: many point sets, one mesh
+    inside = S(points)                        # (B, N) bool, no host synchronisation
 """
 import torch
 
@@ -29,7 +36,8 @@ from .. import _lib
 from ..render.mesh import _host
 
 __all__ = ["adjacency_matrix", "uniform_laplacian", "compute_vertex_normals", "average_face_vertex_features",
-           "UniformLaplacian", "subdivide_trianglemesh", "LoopSubdivision", "subdivide_tetmesh"]
+           "UniformLaplacian", "subdivide_trianglemesh", "LoopSubdivision", "subdivide_tetmesh", "check_sign",
+           "CheckSign"]
 
 
 def _check(func, typed):
@@ -454,3 +462,135 @@ def subdivide_tetmesh(vertices, tetrahedrons, features=None):
     f = vertices.new_empty((B, V, 0)) if features is None else features.contiguous()
     y, yf = _TetSubdivide.apply(vertices.contiguous(), f, topo, new_tets)
     return (y, new_tets) if features is None else (y, new_tets, yf)
+
+
+_CHECK_SIGN_DTYPES = {torch.float32: _lib.DTYPE_F32, torch.float64: _lib.DTYPE_F64}
+
+
+def _check_sign_args(verts, faces, points, hash_resolution):
+    """check_sign.py:104-136, in its order, with its types and messages (``points`` None: CheckSign)."""
+    if points is not None:
+        assert verts.device == points.device
+        assert faces.device == points.device
+    else:
+        assert faces.device == verts.device
+    if not faces.dtype == torch.int64:
+        raise TypeError(f"Expected faces entries to be torch.int64 "
+                        f"but got {faces.dtype}.")
+    if not isinstance(hash_resolution, int):
+        raise TypeError(f"Expected hash_resolution to be int "
+                        f"but got {type(hash_resolution)}.")
+    if verts.ndim != 3:
+        raise ValueError(f"Expected verts to have 3 dimensions "
+                         f"but got {verts.ndim} dimensions.")
+    if faces.ndim != 2:
+        raise ValueError(f"Expected faces to have 2 dimensions "
+                         f"but got {faces.ndim} dimensions.")
+    if points is not None and points.ndim != 3:
+        raise ValueError(f"Expected points to have 3 dimensions "
+                         f"but got {points.ndim} dimensions.")
+    if verts.shape[2] != 3:
+        raise ValueError(f"Expected verts to have 3 coordinates "
+                         f"but got {verts.shape[2]} coordinates.")
+    if faces.shape[1] != 3:
+        raise ValueError(f"Expected faces to have 3 vertices "
+                         f"but got {faces.shape[1]} vertices.")
+    if points is not None and points.shape[2] != 3:
+        raise ValueError(f"Expected points to have 3 coordinates "
+                         f"but got {points.shape[2]} coordinates.")
+
+
+def _check_sign_dtype(func, dtype, named):
+    """CUDA tensors of one type, float32 or float64: the reference's operator takes verts and points of
+    one type (at::checkAllSameType)."""
+    _host.check_tensors(func, named, dtype=None)
+    if dtype not in _CHECK_SIGN_DTYPES:
+        raise RuntimeError(f"\"{func}\" not implemented for '{str(dtype).replace('torch.', '')}' "
+                           "(kaolin_b200 takes verts and points as float32 or float64)")
+    for name, t in named:
+        if t.dtype != dtype:
+            raise RuntimeError(f"{func}: expected {name} of type {dtype}, got {t.dtype}")
+
+
+class CheckSign:
+    r"""The point-in-mesh test of one (batched) mesh, built once.
+
+    ``S = CheckSign(verts, faces)`` normalises the mesh and bins its faces; ``S(points)`` then returns
+    ``check_sign(verts, faces, points)`` without a host synchronisation, for labelling many point sets
+    against one mesh (uniform samples in its box, occupancy and SDF pre-training)::
+
+        S = CheckSign(verts, faces)               # one device-to-host read: the face-index check
+        inside = S(points)                        # (B, N) bool, as check_sign(verts, faces, points)
+
+    ``verts`` (B, V, 3) float32 or float64 and ``faces`` (F, 3) int64 on one CUDA device; the points
+    must have the verts' type and batch size.  The reference normalises by each mesh's extent on every
+    call; the mesh is fixed here at build, so the result is the same.  Later changes to ``verts`` do not
+    reach ``S``.  The argument errors are ``check_sign``'s; a face index outside [0, V) raises
+    ``IndexError``.
+    """
+
+    def __init__(self, verts, faces):
+        func = "CheckSign"
+        _check_sign_args(verts, faces, None, 0)
+        _check_sign_dtype(func, verts.dtype, [("verts", verts)])
+        _check(func, [("faces", faces, torch.int64)])
+        self.dtype, self.device = verts.dtype, verts.device
+        B, V, _ = verts.shape
+        F = faces.shape[0]
+        self.batch_size, self.num_vertices, self.num_faces = B, V, F
+        if B == 0:
+            return
+        dtype = _CHECK_SIGN_DTYPES[verts.dtype]
+        nbytes, _ = _lib.check_sign_workspace_bytes(B, F, 0, dtype, func)
+        self._mesh = _lib.scratch(nbytes, verts.device)
+        status = torch.empty(1, dtype=torch.int32, device=verts.device)
+        _lib.call("dibr_b200_check_sign_build", verts.device, B, V, F, dtype, verts.contiguous(),
+                  faces.contiguous(), status, self._mesh, self._mesh.numel(), what=func)
+        if status.item():                                 # the build's one device-to-host read
+            raise IndexError(f"{func}: faces holds an index outside [0, {V})")
+
+    def __call__(self, points):
+        func = "CheckSign"
+        if points.ndim != 3 or points.shape[2] != 3:
+            raise ValueError(f"{func}: expected points of shape (B, N, 3), got {list(points.shape)}")
+        _check_sign_dtype(func, self.dtype, [("points", points)])
+        if points.device != self.device:
+            raise RuntimeError(f"{func}: expected points on {self.device}, got {points.device}")
+        B, N = self.batch_size, points.shape[1]
+        if points.shape[0] != B:
+            raise ValueError(f"{func}: expected points of batch size {B}, got {points.shape[0]}")
+        out = torch.empty((B, N), dtype=torch.bool, device=points.device)
+        if B == 0 or N == 0:
+            return out
+        dtype = _CHECK_SIGN_DTYPES[self.dtype]
+        _, nbytes = _lib.check_sign_workspace_bytes(B, self.num_faces, N, dtype, func)
+        ws = _lib.scratch(nbytes, points.device)
+        _lib.call("dibr_b200_check_sign_query", points.device, B, self.num_faces, N, dtype, points.contiguous(),
+                  self._mesh, self._mesh.numel(), out, ws, ws.numel(), what=func)
+        return out
+
+
+def check_sign(verts, faces, points, hash_resolution=512):
+    r"""kaolin.ops.mesh.check_sign: whether each point lies inside a watertight triangle mesh.
+
+    ``verts`` (B, V, 3), ``faces`` (F, 3) int64 and ``points`` (B, N, 3) -> (B, N) bool.  Per view, the
+    vertices and points are divided by the mesh's largest extent over all V vertices, and a ray from
+    each point along +x is tested against every face; a point is inside when it crosses an odd number of
+    faces.  Equal to the reference's CUDA operator bit for bit in float32 and float64: every comparison
+    follows its compiled arithmetic, including the edge and vertex tie-breaking.  The faces are binned
+    on a y-z grid, so each point is tested against its cell's faces only.  The mesh is built on every
+    call, as the reference does (one device-to-host read, the face-index check); ``CheckSign`` builds it
+    once.  ``hash_resolution`` is type-checked as in the reference and otherwise unused (the reference
+    uses it on its CPU path only).  The argument errors are the reference's, in its order.
+
+    Deliberate deviations: ``verts`` and ``points`` must be float32 or float64 CUDA tensors of one type
+    and one batch size (there is no CPU path); F = 0 gives all ``False`` (the reference's launch fails);
+    B = 0 gives a (0, N) tensor (the reference's ``torch.stack([])`` raises); a face index outside
+    [0, V) raises ``IndexError`` (the reference's ``index_select`` faults on the device).
+    """
+    _check_sign_args(verts, faces, points, hash_resolution)
+    _check_sign_dtype("check_sign", verts.dtype, [("verts", verts), ("points", points)])
+    if verts.shape[0] != points.shape[0]:
+        raise ValueError(f"check_sign: expected verts and points of one batch size, "
+                         f"got {verts.shape[0]} and {points.shape[0]}")
+    return CheckSign(verts, faces)(points)
