@@ -391,6 +391,7 @@ int dibr_b200_deftet_sparse_render_backward(
  */
 #define DIBR_B200_DTYPE_F32 0
 #define DIBR_B200_DTYPE_F64 1
+#define DIBR_B200_DTYPE_U8 2     /* marching cubes: uint8 (and bool) grids */
 int dibr_b200_check_sign_workspace_bytes(int batch, int num_faces, int num_points, int dtype, size_t* build_bytes,
                                          size_t* query_bytes);
 int dibr_b200_check_sign_build(int batch, int num_vertices, int num_faces, int dtype, const void* verts,
@@ -713,6 +714,46 @@ int dibr_b200_marching_tets_backward(int batch, int num_vertices, int num_edges,
                                      const int32_t* adj, const int32_t* adj_edge, const float* vertices,
                                      const float* sdf, const int32_t* vid, const float* grad_out,
                                      float* grad_vertices, float* grad_sdf, dibr_b200_stream_t stream);
+
+/*
+ * Marching cubes (kaolin/ops/conversions/voxelgrid.py:158-246, the reference's unbatched_mcube) for B
+ * views of a grid (B, X, Y, Z) at `grid` with element strides stride_b..stride_z, float32
+ * (DIBR_B200_DTYPE_F32) or uint8 / bool (DIBR_B200_DTYPE_U8).  The grid is padded by `pad` (1: a
+ * virtual border of zeros, as the reference's wrapper pads; 0: none, as its raw operator takes an
+ * already-padded grid) into a lattice of N = (X+2pad)(Y+2pad)(Z+2pad) points, each the corner of a
+ * cube whose far corners are clamped to the lattice's far border.  csrc/marching_cubes.cu describes
+ * the case, vertex and face order, which are the reference's.
+ *   dibr_b200_marching_cubes_count: writes cases (B*N) uint8, the case of every cube; scan
+ *     (2*(B*N + 1)) int32, the exclusive scans of the per-cube triangle counts and owned-vertex
+ *     counts, each with its total; and totals (B, 2) int32 {faces, vertices} per view: the one value
+ *     to read back to size the outputs.  Workspace >= dibr_b200_marching_cubes_workspace_bytes.
+ *   dibr_b200_marching_cubes_emit: writes, all views in one array each, view after view,
+ *     out_vertices (sum nv, 3) f32 and out_faces (sum nf, 3) int64 (vertex ids per view; -1 only with
+ *     pad 0, where an edge on the lattice's border has no owning cube).
+ *   dibr_b200_marching_cubes_backward (pad 1, float32 grid): grad_out (sum nv, 3) -> grad_grid
+ *     (B, X, Y, Z) contiguous, one thread per input value over its <= 6 sign-change edges, no atomics.
+ * Memory per cube, all views: 1 byte of cases + 8 of scans, kept from count to backward, plus 8 of
+ * workspace (the counts) during count: 17 bytes, and 4 bytes per 4096 cubes of scan tile sums.
+ * B*N must be at most (2^31 - 1) / 5, so that the worst case of 5 triangles per cube is indexable by
+ * int (else DIBR_B200_ESIZE); a non-positive dimension, a pad other than 0 or 1, a bad dtype or a
+ * NULL buffer that is used give DIBR_B200_EINVAL.
+ * dibr_b200_marching_cubes_case_table (host): pairs (256, 5, 3, 2) int32, the corners (i, j) of the
+ * edge of each vertex of each triangle of each case, -1 past the case's triangles.
+ */
+int dibr_b200_marching_cubes_case_table(int32_t* pairs);
+int dibr_b200_marching_cubes_workspace_bytes(int batch, int X, int Y, int Z, int pad, size_t* workspace_bytes);
+int dibr_b200_marching_cubes_count(int batch, int X, int Y, int Z, int pad, int dtype, const void* grid, int64_t stride_b,
+                                   int64_t stride_x, int64_t stride_y, int64_t stride_z, float iso, uint8_t* cases,
+                                   int32_t* scan, int32_t* totals, void* workspace, size_t workspace_bytes,
+                                   dibr_b200_stream_t stream);
+int dibr_b200_marching_cubes_emit(int batch, int X, int Y, int Z, int pad, int dtype, const void* grid, int64_t stride_b,
+                                  int64_t stride_x, int64_t stride_y, int64_t stride_z, float iso, const uint8_t* cases,
+                                  const int32_t* scan, float* out_vertices, int64_t* out_faces,
+                                  dibr_b200_stream_t stream);
+int dibr_b200_marching_cubes_backward(int batch, int X, int Y, int Z, int pad, const float* grid, int64_t stride_b,
+                                      int64_t stride_x, int64_t stride_y, int64_t stride_z, float iso,
+                                      const uint8_t* cases, const int32_t* scan, const float* grad_out,
+                                      float* grad_grid, dibr_b200_stream_t stream);
 
 /*
  * subdivide_tetmesh (kaolin/ops/mesh/tetmesh.py:85-181) on the tet topology: vertices (B, V, 3) and

@@ -1,8 +1,9 @@
 """``kaolin_b200._C.render.mesh`` — the four operators the reference registers in
 kaolin/csrc/bindings.cpp:111-115, with identical names, argument order/meaning,
 return structure and error behaviour, implemented by libdibr_b200.so; likewise
-``_C.render.sg``, the DefTet pair and ``_C.ops.mesh.unbatched_mesh_intersection_cuda``
-(bindings.cpp:49), which the reference's ``check_sign.py`` calls.
+``_C.render.sg``, the DefTet pair, ``_C.ops.mesh.unbatched_mesh_intersection_cuda``
+(bindings.cpp:49), which the reference's ``check_sign.py`` calls, and
+``_C.ops.conversions.unbatched_mcube_forward_cuda``, which its ``voxelgrids_to_trianglemeshes`` calls.
 
 This is what makes the library a drop-in *below* the reference's own Python
 wrappers: ``kaolin.render.mesh.rasterization`` / ``.dibr`` run unmodified with
@@ -291,9 +292,18 @@ def unbatched_mesh_intersection_cuda(points, verts_1, verts_2, verts_3):
     return out
 
 
-# kaolin._C.ops.mesh.<op>, as bindings.cpp:43,48-49 lays it out
+def unbatched_mcube_forward_cuda(voxelgrid, iso_value):
+    """unbatched_mcube.cpp -> [vertices (nv, 3) float32, faces (nf, 3) int32]: marching cubes on one
+    already-padded grid (X, Y, Z) float32, as ``voxelgrids_to_trianglemeshes`` calls it per view."""
+    from .ops.conversions.voxelgrid import unbatched_mcube_forward
+    return unbatched_mcube_forward(voxelgrid, iso_value)
+
+
+# kaolin._C.ops.{mesh,conversions}.<op>, as bindings.cpp lays them out
 ops = types.SimpleNamespace(mesh=types.SimpleNamespace(
     unbatched_mesh_intersection_cuda=unbatched_mesh_intersection_cuda,
+), conversions=types.SimpleNamespace(
+    unbatched_mcube_forward_cuda=unbatched_mcube_forward_cuda,
 ))
 
 # kaolin._C.render.{mesh,sg}.<op> namespaces, as bindings.cpp:42,111-115,129-133 lays them out

@@ -17,10 +17,10 @@ LIB_PATH = os.path.join(CSRC, "libdibr_b200.so")
 SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline.cu"),
            os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
            os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu"),
-           os.path.join(CSRC, "check_sign.cu")]
+           os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
-           os.path.join(CSRC, "grid_bins.cuh"),
+           os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
            os.path.join(_HERE, "..", "include", "dibr_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -30,6 +30,7 @@ RASTER, SOFT_MASK = 1, 2
 LIGHT_SG_INNER_PRODUCT, LIGHT_SG_FITTED, LIGHT_SH9 = 0, 1, 2     # dibr_b200_diffuse_* models
 BINS_VALID, ACCUMULATE = 1, 2      # dibr_b200_backward flags
 DTYPE_F32, DTYPE_F64 = 0, 1        # dibr_b200_check_sign_* and dibr_b200_mesh_intersection_count
+DTYPE_U8 = 2                       # dibr_b200_marching_cubes_* (uint8 and bool grids)
 
 _lock = threading.Lock()
 _lib = None
@@ -132,6 +133,12 @@ SIGNATURES = {
     "dibr_b200_check_sign_build": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dibr_b200_check_sign_query": (_i, [_i, _i, _i, _i, _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dibr_b200_mesh_intersection_count": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    # marching cubes (ops.conversions.voxelgrids_to_trianglemeshes, _C.ops.conversions; csrc/marching_cubes.cu)
+    "dibr_b200_marching_cubes_case_table": (_i, [_vp]),
+    "dibr_b200_marching_cubes_workspace_bytes": (_i, [_i] * 5 + [ctypes.POINTER(_sz)]),
+    "dibr_b200_marching_cubes_count": (_i, [_i] * 6 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dibr_b200_marching_cubes_emit": (_i, [_i] * 6 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _vp]),
+    "dibr_b200_marching_cubes_backward": (_i, [_i] * 5 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _vp]),
 }
 
 
@@ -235,6 +242,21 @@ def marching_tets_case_table():
     out = (ctypes.c_int32 * (16 * 12))()
     check(lib().dibr_b200_marching_tets_case_table(out), "marching_tets_case_table")
     return list(out)
+
+
+def marching_cubes_case_table():
+    """The library's marching-cubes case table (a host query, no device work): 256 * 5 * 3 * 2 corner
+    indices, -1 past a case's triangles (include/dibr_b200.h)."""
+    out = (ctypes.c_int32 * (256 * 30))()
+    check(lib().dibr_b200_marching_cubes_case_table(out), "marching_cubes_case_table")
+    return list(out)
+
+
+def marching_cubes_workspace_bytes(batch, X, Y, Z, pad, what):
+    """The workspace bytes of ``dibr_b200_marching_cubes_count``; raises on its status."""
+    out = _sz(0)
+    check(lib().dibr_b200_marching_cubes_workspace_bytes(batch, X, Y, Z, pad, ctypes.byref(out)), what)
+    return out.value
 
 
 def check_sign_workspace_bytes(batch, num_faces, num_points, dtype, what):

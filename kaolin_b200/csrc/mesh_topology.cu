@@ -23,6 +23,7 @@
 #include <stdint.h>
 
 #include "../../include/dibr_b200.h"
+#include "scan.cuh"
 
 // launch tracing (dibr_b200_trace_begin / _end), kept in dibr_b200.cu
 namespace dibr_b200_detail {
@@ -39,8 +40,11 @@ struct Span {
   ~Span() { if (on) dibr_b200_detail::span_close(st); }
 };
 
+using dibr_b200_detail::exclusive_scan;
+using dibr_b200_detail::kScanTile;
+
 constexpr int kScanThreads = 1024;
-constexpr int kScanTile = kScanThreads * 4;   // elements per CTA of the scan
+static_assert(kScanTile == kScanThreads * 4, "scan_*_kernel: four elements per thread");
 constexpr int kShortRow = 32;                 // rows of at most this many corners are sorted by one thread
 constexpr int kLongCtas = 132;                // CTAs that share out the long rows
 constexpr int kThreads = 256;
@@ -124,7 +128,9 @@ __global__ void __launch_bounds__(kScanThreads) scan_apply_kernel(const int* __r
   }
 }
 
-int exclusive_scan(const int* in, int n, int* sums, int* out, cudaStream_t st) {
+}  // namespace
+
+int dibr_b200_detail::exclusive_scan(const int* in, int n, int* sums, int* out, cudaStream_t st) {
   if (n == 0) return (int)cudaMemsetAsync(out, 0, sizeof(int), st);
   const int tiles = (int)((n + kScanTile - 1) / kScanTile);
   { Span s("scan_reduce_kernel", st); scan_reduce_kernel<<<tiles, kScanThreads, 0, st>>>(in, n, sums); }
@@ -132,6 +138,8 @@ int exclusive_scan(const int* in, int n, int* sums, int* out, cudaStream_t st) {
   { Span s("scan_apply_kernel", st); scan_apply_kernel<<<tiles, kScanThreads, 0, st>>>(in, n, sums, out); }
   return (int)cudaGetLastError();
 }
+
+namespace {
 
 // ---------------------------------------------------------------------------------------------
 // Build.
