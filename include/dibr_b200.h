@@ -21,7 +21,8 @@
  * which calls dibr_b200_backward) must be 16-byte aligned; otherwise the call
  * returns DIBR_B200_EINVAL.  The kernels make 16-byte vector accesses on them.
  * A fresh allocation is aligned; a contiguous view at an element offset may not be
- * (the Python layer copies such inputs).  The workspace needs no alignment.
+ * (the Python layer copies such inputs).  The workspace needs no alignment: every entry point rounds
+ * its pointer up to 256 bytes, and every size query includes those bytes.
  *
  * The four "operator" entry points replace, one for one, the functions the
  * reference registers in kaolin/csrc/bindings.cpp:111-115; the two "fused"
@@ -431,10 +432,10 @@ int dibr_b200_mesh_intersection_count(int num_faces, int num_points, int dtype, 
  *
  * Light gradients are bit-reproducible: no float atomics; per-CTA partials summed in a fixed order
  * in fp64.  The workspace does not depend on N: 264 CTA slots x 7 floats per light (SH9: 9 floats)
- * = 7.4 KB per light.  Per-point data is read once for any L (kept in registers while the lights
- * are streamed through shared memory); with only light gradients requested the backward reads
- * grad_out, normal and albedo and writes nothing per point.  Clamp gradients pass where the input is
- * >= 0, as torch.clamp's do.
+ * = 7.4 KB per light, and 256 bytes.  Per-point data is read once for any L (kept in registers
+ * while the lights are streamed through shared memory); with only light gradients requested the
+ * backward reads grad_out, normal and albedo and writes nothing per point.  Clamp gradients pass
+ * where the input is >= 0, as torch.clamp's do.
  * The formulas are the reference's, literally, in fp32.  Where the reference itself produces inf or
  * NaN the result is unspecified: um = 0 (opposite directions of equal sharpness), sharpness 0, and
  * sharpness so small that sqrt(1 - scale) is 0 in the fitted model.
@@ -482,9 +483,9 @@ int dibr_b200_diffuse_backward(
  * (N,3), grad_spec_albedo (N,3) and the light gradients; a NULL gradient is not computed, and with
  * only light gradients requested nothing is written per point.  Clamp gradients pass where
  * min <= x <= max, as torch.clamp's do.  Light gradients need workspace >=
- * dibr_b200_specular_workspace_bytes(L) = 264 CTA slots x 7 floats = 7.4 KB per light, independent
- * of N; they are bit-reproducible, as the diffuse models' are.  L = 0 gives zero output and zero
- * per-point gradients (the reference's empty sum); N = 0 does nothing per point.
+ * dibr_b200_specular_workspace_bytes(L) = 264 CTA slots x 7 floats = 7.4 KB per light and 256 bytes,
+ * independent of N; they are bit-reproducible, as the diffuse models' are.  L = 0 gives zero output
+ * and zero per-point gradients (the reference's empty sum); N = 0 does nothing per point.
  * Unspecified, as the reference itself gives inf or NaN there: roughness 0, and w + v = 0 (a unit
  * normal exactly perpendicular to the view).
  */
@@ -521,8 +522,8 @@ int dibr_b200_specular_backward(
  * grad_normals (through the normalisation) and the light gradients; a NULL gradient is not
  * computed, and with only light gradients requested nothing is written per pixel.  The camera gets
  * no gradient.  Light gradients need workspace >= dibr_b200_sg_shade_workspace_bytes(L) = 7.4 KB per
- * light, independent of the pixel count, and are bit-reproducible.  H or W above 16384 gives
- * DIBR_B200_ESIZE; negative sizes or a NULL input that is read give DIBR_B200_EINVAL, before any
+ * light and 256 bytes, independent of the pixel count, and are bit-reproducible.  H or W above 16384
+ * gives DIBR_B200_ESIZE; negative sizes or a NULL input that is read give DIBR_B200_EINVAL, before any
  * CUDA call.  Unspecified, where the reference itself gives inf or NaN: a covered pixel of roughness 0,
  * or whose unit normal is exactly perpendicular to its view (w + v = 0).
  */
@@ -733,7 +734,8 @@ int dibr_b200_marching_tets_backward(int batch, int num_vertices, int num_edges,
  *   dibr_b200_marching_cubes_backward (pad 1, float32 grid): grad_out (sum nv, 3) -> grad_grid
  *     (B, X, Y, Z) contiguous, one thread per input value over its <= 6 sign-change edges, no atomics.
  * Memory per cube, all views: 1 byte of cases + 8 of scans, kept from count to backward, plus 8 of
- * workspace (the counts) during count: 17 bytes, and 4 bytes per 4096 cubes of scan tile sums.
+ * workspace (the counts) during count: 17 bytes, and 4 bytes per 4096 cubes of scan tile sums and
+ * under 512 bytes of alignment.
  * B*N must be at most (2^31 - 1) / 5, so that the worst case of 5 triangles per cube is indexable by
  * int (else DIBR_B200_ESIZE); a non-positive dimension, a pad other than 0 or 1, a bad dtype or a
  * NULL buffer that is used give DIBR_B200_EINVAL.

@@ -20,7 +20,7 @@ SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline
            os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
-           os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
+           os.path.join(CSRC, "op_layouts.h"), os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
            os.path.join(_HERE, "..", "include", "dibr_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]

@@ -46,6 +46,9 @@
 
 namespace {
 
+using dibr_layout::carve;
+using dibr_layout::piece;
+
 constexpr int kQueryThreads = 256;
 
 // Correctly rounded operations, never contracted: the predicate spells out every FMA itself.
@@ -298,57 +301,27 @@ __global__ void __launch_bounds__(kQueryThreads) cs_query_kernel(const __grid_co
   if (a.counts) a.counts[i] = (T)n;
 }
 
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-// The build workspace: status-independent pieces a query reads, in this order.
-struct BuildLayout { size_t maxlen, bounds, cnt, off, entries, wide, boxes, records, total; };
-BuildLayout build_layout(int B, int F, size_t tsize) {
-  const int G = grid_side(F);
-  const size_t nf = (size_t)B * (size_t)(F > 0 ? F : 1);
-  BuildLayout L;
-  L.maxlen = align_up((size_t)B * tsize, 256);
-  L.bounds = align_up((size_t)B * 4 * sizeof(float), 256);
-  L.cnt = align_up((size_t)B * (G * G + 1) * sizeof(int), 256);
-  L.off = L.cnt;
-  L.entries = align_up(nf * kMaxCells * sizeof(int), 256);
-  L.wide = align_up(nf * sizeof(int), 256);
-  L.boxes = align_up(nf * sizeof(float4), 256);
-  L.records = align_up(nf * 9 * tsize, 256);
-  L.total = L.maxlen + L.bounds + L.cnt + L.off + L.entries + L.wide + L.boxes + L.records + 256;
-  return L;
-}
-
-struct QueryLayout { size_t cnt, off, pcell, order, total; };
-QueryLayout query_layout(int B, int F, int N) {
-  const int G = grid_side(F);
-  const size_t np = (size_t)B * (size_t)(N > 0 ? N : 1);
-  QueryLayout L;
-  L.cnt = align_up((size_t)B * (G * G + 1) * sizeof(int), 256);
-  L.off = L.cnt;
-  L.pcell = align_up(np * sizeof(int), 256);
-  L.order = L.pcell;
-  L.total = L.cnt + L.off + L.pcell + L.order + 256;
-  return L;
-}
-
 struct Mesh {   // the build workspace carved
   Grid g;
+  void* counters; size_t counters_bytes;   // the grid's cnt and off
   void* maxlen; void* records; float4* boxes;
 };
 
 int carve_build(int B, int F, size_t tsize, void* ws, size_t bytes, Mesh& m) {
-  const BuildLayout L = build_layout(B, F, tsize);
-  char* p = (char*)align_up((size_t)ws, 256);
-  if (bytes < L.total || p + L.total - 256 > (char*)ws + bytes) return DIBR_B200_EWORKSPACE;
+  const dibr_layout::CheckSignBuildLayout L = dibr_layout::check_sign_build_layout(B, F, tsize);
+  char* o = carve(ws, bytes, L.bytes);
+  if (!o) return DIBR_B200_EWORKSPACE;
   m.g.B = B; m.g.F = F; m.g.P = 0; m.g.G = grid_side(F);
-  m.maxlen = p; p += L.maxlen;
-  m.g.bounds = (float*)p; p += L.bounds;
-  m.g.cnt = (int*)p; p += L.cnt;
-  m.g.off = (int*)p; p += L.off;
-  m.g.entries = (int*)p; p += L.entries;
-  m.g.wide = (int*)p; p += L.wide;
-  m.boxes = (float4*)p; p += L.boxes;
-  m.records = p;
+  m.g.bounds = piece<float>(o, L.grid.bounds);
+  m.g.cnt = piece<int>(o, L.grid.cnt);
+  m.g.off = piece<int>(o, L.grid.off);
+  m.g.entries = piece<int>(o, L.grid.entries);
+  m.g.wide = piece<int>(o, L.grid.wide);
+  m.counters = piece<char>(o, L.grid.counters);
+  m.counters_bytes = L.grid.counters.bytes;
+  m.maxlen = piece<char>(o, L.maxlen);
+  m.boxes = piece<float4>(o, L.boxes);
+  m.records = piece<char>(o, L.records);
   return 0;
 }
 
@@ -364,8 +337,7 @@ template <typename T>
 int build(int B, int V, int F, const T* verts, const int64_t* faces, const T* v1, const T* v2, const T* v3,
           int32_t* status, const Mesh& m, cudaStream_t st) {
   Grid g = m.g;
-  const BuildLayout L = build_layout(B, F, sizeof(T));
-  cudaError_t e = cudaMemsetAsync(g.cnt, 0, L.cnt + L.off, st);
+  cudaError_t e = cudaMemsetAsync(m.counters, 0, m.counters_bytes, st);
   if (e != cudaSuccess) return (int)e;
   if (status) {
     e = cudaMemsetAsync(status, 0, sizeof(int32_t), st);
@@ -389,17 +361,17 @@ template <typename T>
 int query(int N, const T* points, const T* maxlen, const Mesh& m, uint8_t* inside, T* counts, void* ws, size_t bytes,
           cudaStream_t st) {
   const int B = m.g.B, F = m.g.F;
-  const QueryLayout L = query_layout(B, F, N);
-  char* p = (char*)align_up((size_t)ws, 256);
-  if (bytes < L.total || p + L.total - 256 > (char*)ws + bytes) return DIBR_B200_EWORKSPACE;
+  const dibr_layout::CheckSignQueryLayout L = dibr_layout::check_sign_query_layout(B, F, N);
+  char* o = carve(ws, bytes, L.bytes);
+  if (!o) return DIBR_B200_EWORKSPACE;
   if (N == 0) return 0;
   Grid pg = m.g;          // the same cells, counting points
   pg.P = N;
-  pg.cnt = (int*)p; p += L.cnt;
-  pg.off = (int*)p; p += L.off;
-  int* pcell = (int*)p; p += L.pcell;
-  int* order = (int*)p;
-  cudaError_t e = cudaMemsetAsync(pg.cnt, 0, L.cnt, st);
+  pg.cnt = piece<int>(o, L.cnt);
+  pg.off = piece<int>(o, L.off);
+  int* pcell = piece<int>(o, L.pcell);
+  int* order = piece<int>(o, L.order);
+  cudaError_t e = cudaMemsetAsync(pg.cnt, 0, L.cnt.bytes, st);
   if (e != cudaSuccess) return (int)e;
   const int64_t np = (int64_t)B * N;
   cs_point_cell_kernel<T><<<blocks(np, 256), 256, 0, st>>>(pg, points, maxlen, pcell);
@@ -426,8 +398,8 @@ int dibr_b200_check_sign_workspace_bytes(int batch, int num_faces, int num_point
   const size_t ts = tsize_of(dtype);
   if (batch <= 0 || num_faces < 0 || num_points < 0 || ts == 0) return DIBR_B200_EINVAL;
   if (int r = check_sizes(batch, num_faces, num_points)) return r;
-  if (build_bytes) *build_bytes = build_layout(batch, num_faces, ts).total;
-  if (query_bytes) *query_bytes = query_layout(batch, num_faces, num_points).total;
+  if (build_bytes) *build_bytes = dibr_layout::check_sign_build_layout(batch, num_faces, ts).bytes;
+  if (query_bytes) *query_bytes = dibr_layout::check_sign_query_layout(batch, num_faces, num_points).bytes;
   return 0;
 }
 
@@ -472,8 +444,9 @@ int dibr_b200_mesh_intersection_count(int num_faces, int num_points, int dtype, 
   if (num_points > 0 && (!points || !counts)) return DIBR_B200_EINVAL;
   if (num_faces > 0 && (!verts_1 || !verts_2 || !verts_3)) return DIBR_B200_EINVAL;
   if (int r = check_sizes(1, num_faces, num_points)) return r;
-  const size_t nb = build_layout(1, num_faces, ts).total;
-  if (workspace_bytes < nb + query_layout(1, num_faces, num_points).total) return DIBR_B200_EWORKSPACE;
+  const size_t nb = dibr_layout::check_sign_build_layout(1, num_faces, ts).bytes;
+  if (workspace_bytes < nb + dibr_layout::check_sign_query_layout(1, num_faces, num_points).bytes)
+    return DIBR_B200_EWORKSPACE;
   Mesh m;
   if (int r = carve_build(1, num_faces, ts, workspace, nb, m)) return r;
   cudaStream_t st = (cudaStream_t)stream;

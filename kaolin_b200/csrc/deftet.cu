@@ -37,6 +37,8 @@
 namespace {
 
 using namespace dibr;
+using dibr_layout::carve;
+using dibr_layout::piece;
 
 constexpr int kHitCap = 128;      // hits a point can collect before it takes the ordered scan
 constexpr int kWarps = 8;         // points per CTA
@@ -220,28 +222,13 @@ __global__ void __launch_bounds__(256) deftet_backward_kernel(const __grid_const
   atomicAdd(gx + 2, make_float2(v[4], v[5]));
 }
 
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-struct Layout { size_t bounds, cnt, off, entries, wide, total; };
-Layout layout_for(int B, int F) {
-  const int G = grid_side(F);
-  Layout L;
-  L.bounds = align_up((size_t)B * 4 * sizeof(float), 256);
-  L.cnt = align_up((size_t)B * (G * G + 1) * sizeof(int), 256);
-  L.off = L.cnt;
-  L.entries = align_up((size_t)B * (size_t)(F > 0 ? F : 1) * kMaxCells * sizeof(int), 256);
-  L.wide = align_up((size_t)B * (size_t)(F > 0 ? F : 1) * sizeof(int), 256);
-  L.total = L.bounds + L.cnt + L.off + L.entries + L.wide + 256;
-  return L;
-}
-
 }  // namespace
 
 extern "C" {
 
 size_t dibr_b200_deftet_workspace_bytes(int batch, int num_faces) {
   if (batch <= 0 || num_faces < 0) return 0;
-  return layout_for(batch, num_faces).total;
+  return dibr_layout::deftet_layout(batch, num_faces).bytes;
 }
 
 int dibr_b200_deftet_sparse_render_forward(int batch, int num_faces, int num_pixels, int knum,
@@ -254,20 +241,20 @@ int dibr_b200_deftet_sparse_render_forward(int batch, int num_faces, int num_pix
   if (!pixel_coords || !render_ranges || !face_idx || !pixel_depth || !w0 || !w1 || !workspace) return DIBR_B200_EINVAL;
   if (num_faces > 0 && (!face_vertices_z || !face_vertices_image || !face_bboxes)) return DIBR_B200_EINVAL;
   if ((int64_t)batch * num_pixels * knum >= (int64_t)1 << 40 || (int64_t)num_faces * kMaxCells >= 0x7fffffffLL) return DIBR_B200_ESIZE;
-  const Layout L = layout_for(batch, num_faces);
-  char* p = (char*)align_up((size_t)workspace, 256);
-  if (workspace_bytes < L.total || p + L.total - 256 > (char*)workspace + workspace_bytes) return DIBR_B200_EWORKSPACE;
+  const dibr_layout::DeftetLayout L = dibr_layout::deftet_layout(batch, num_faces);
+  char* o = carve(workspace, workspace_bytes, L.bytes);
+  if (!o) return DIBR_B200_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   if (num_pixels == 0) return 0;
   FwdArgs a;
   Grid& g = a.g;
   g.B = batch; g.F = num_faces; g.P = num_pixels; g.G = grid_side(num_faces);
-  g.bounds = (float*)p; p += L.bounds;
-  g.cnt = (int*)p; p += L.cnt;
-  g.off = (int*)p; p += L.off;
-  g.entries = (int*)p; p += L.entries;
-  g.wide = (int*)p;
-  cudaError_t e = cudaMemsetAsync(g.cnt, 0, L.cnt, st);
+  g.bounds = piece<float>(o, L.grid.bounds);
+  g.cnt = piece<int>(o, L.grid.cnt);
+  g.off = piece<int>(o, L.grid.off);
+  g.entries = piece<int>(o, L.grid.entries);
+  g.wide = piece<int>(o, L.grid.wide);
+  cudaError_t e = cudaMemsetAsync(g.cnt, 0, L.grid.cnt.bytes, st);
   if (e != cudaSuccess) return (int)e;
   deftet_bounds_kernel<<<batch, 256, 0, st>>>(batch, num_pixels, g.G, pixel_coords, const_cast<float*>(g.bounds));
   const int64_t nf = (int64_t)batch * num_faces;
@@ -276,7 +263,7 @@ int dibr_b200_deftet_sparse_render_forward(int batch, int num_faces, int num_pix
     grid_scan_kernel<<<batch, 1024, 0, st>>>(g);
     grid_bin_kernel<false, true><<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(g, face_bboxes);
   } else {
-    e = cudaMemsetAsync(g.off, 0, L.off, st);
+    e = cudaMemsetAsync(g.off, 0, L.grid.off.bytes, st);
     if (e != cudaSuccess) return (int)e;
   }
   a.knum = knum; a.eps = eps; a.fvz = face_vertices_z; a.fvi = face_vertices_image; a.bbox = face_bboxes;

@@ -16,9 +16,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "op_layouts.h"
+
 namespace {
 
-constexpr int kMaxCells = 16;     // cells a face may be inserted in; wider faces -> the view's wide list
+using dibr_layout::grid_side;     // the grid's side for F faces per view
+using dibr_layout::kMaxCells;     // cells a face may be inserted in; wider faces -> the view's wide list
 constexpr unsigned kGridFull = 0xffffffffu;
 
 struct Grid {
@@ -101,12 +104,6 @@ __global__ void __launch_bounds__(1024) grid_scan_kernel(Grid g) {
     if (tid == 1023) carry = excl + v;
     __syncthreads();
   }
-}
-
-int grid_side(int F) {
-  int G = 8;
-  while (G < 256 && (int64_t)G * G < F) G += 8;   // ~1 face per cell before overlaps
-  return G;
 }
 
 }  // namespace

@@ -27,6 +27,7 @@
 #include <stdint.h>
 
 #include "../../include/dibr_b200.h"
+#include "op_layouts.h"
 
 namespace {
 
@@ -708,7 +709,14 @@ int launch_bwd(const Args& a, cudaStream_t st) {
   return (int)cudaGetLastError();
 }
 
-size_t partial_bytes(int slots, int lights) { return (size_t)kBwdCtas * (size_t)lights * (size_t)slots * sizeof(float); }
+// The workspace of a backward whose light gradients take `floats` partial sums per light.
+dibr_layout::LightingLayout partials(int floats, int lights) { return dibr_layout::lighting_layout(kBwdCtas, floats, lights); }
+
+// The partial sums of l in the workspace, or NULL when it does not fit.
+float* carve_partials(const dibr_layout::LightingLayout& l, void* workspace, size_t workspace_bytes) {
+  char* o = dibr_layout::carve(workspace, workspace_bytes, l.bytes);
+  return o ? dibr_layout::piece<float>(o, l.partial) : nullptr;
+}
 
 // ---------------------------------------------------------------------------------------------
 // SHADE (sg_shade of kaolin/render/easy_render/mesh.py): deferred shading of a (B, H, W) G-buffer, one
@@ -1008,7 +1016,7 @@ int launch_shade_bwd(const ShadeArgs& s, cudaStream_t st) {
 extern "C" {
 
 size_t dibr_b200_sg_inner_product_workspace_bytes(int num_other) {
-  return num_other < 0 ? 0 : partial_bytes(Cfg<GENERAL>::kAcc, num_other);
+  return num_other < 0 ? 0 : partials(Cfg<GENERAL>::kAcc, num_other).bytes;
 }
 
 int dibr_b200_sg_inner_product_forward(int64_t num_sg, int num_other, const float* amplitude, const float* direction,
@@ -1046,8 +1054,8 @@ int dibr_b200_sg_inner_product_backward(int64_t num_sg, int num_other, const flo
   a.gl_amp = grad_other_amplitude; a.gl_dir = grad_other_direction; a.gl_sharp = grad_other_sharpness;
   if (num_other > 0 && (a.gl_amp || a.gl_dir || a.gl_sharp)) {
     if (!workspace) return DIBR_B200_EINVAL;
-    if (workspace_bytes < partial_bytes(Cfg<GENERAL>::kAcc, num_other)) return DIBR_B200_EWORKSPACE;
-    a.partial = (float*)workspace;
+    a.partial = carve_partials(partials(Cfg<GENERAL>::kAcc, num_other), workspace, workspace_bytes);
+    if (!a.partial) return DIBR_B200_EWORKSPACE;
   }
   cudaStream_t st = (cudaStream_t)stream;
   if (num_other == 0) {   // empty sum: every sg-side gradient is zero
@@ -1060,12 +1068,20 @@ int dibr_b200_sg_inner_product_backward(int64_t num_sg, int num_other, const flo
   return launch_bwd<GENERAL>(a, st);
 }
 
+// The workspace of a diffuse backward with light gradients; SH9 has one light of 9 coefficients.
+static dibr_layout::LightingLayout diffuse_partials(int model, int num_lights) {
+  switch (model) {
+    case DIBR_B200_LIGHT_SG_INNER_PRODUCT: return partials(Cfg<LOBE>::kAcc, num_lights);
+    case DIBR_B200_LIGHT_SG_FITTED: return partials(Cfg<FITTED>::kAcc, num_lights);
+    default: return partials(Cfg<SH9>::kAcc, 1);
+  }
+}
+
 size_t dibr_b200_diffuse_workspace_bytes(int model, int num_lights) {
   if (num_lights < 0) return 0;
   switch (model) {
-    case DIBR_B200_LIGHT_SG_INNER_PRODUCT: return partial_bytes(Cfg<LOBE>::kAcc, num_lights);
-    case DIBR_B200_LIGHT_SG_FITTED: return partial_bytes(Cfg<FITTED>::kAcc, num_lights);
-    case DIBR_B200_LIGHT_SH9: return partial_bytes(Cfg<SH9>::kAcc, 1);
+    case DIBR_B200_LIGHT_SG_INNER_PRODUCT: case DIBR_B200_LIGHT_SG_FITTED: case DIBR_B200_LIGHT_SH9:
+      return diffuse_partials(model, num_lights).bytes;
     default: return 0;
   }
 }
@@ -1124,8 +1140,8 @@ int dibr_b200_diffuse_backward(int model, int64_t num_points, int num_lights, co
   if (model != DIBR_B200_LIGHT_SH9) { a.gl_dir = grad_light_direction; a.gl_sharp = grad_light_sharpness; }
   if (num_lights > 0 && (a.gl_amp || a.gl_dir || a.gl_sharp)) {
     if (!workspace) return DIBR_B200_EINVAL;
-    if (workspace_bytes < dibr_b200_diffuse_workspace_bytes(model, num_lights)) return DIBR_B200_EWORKSPACE;
-    a.partial = (float*)workspace;
+    a.partial = carve_partials(diffuse_partials(model, num_lights), workspace, workspace_bytes);
+    if (!a.partial) return DIBR_B200_EWORKSPACE;
   }
   cudaStream_t st = (cudaStream_t)stream;
   if (num_lights == 0) {   // empty sum: zero irradiance, zero per-point gradients
@@ -1142,7 +1158,7 @@ int dibr_b200_diffuse_backward(int model, int64_t num_points, int num_lights, co
 }
 
 size_t dibr_b200_specular_workspace_bytes(int num_lights) {
-  return num_lights < 0 ? 0 : partial_bytes(Cfg<SPECULAR>::kAcc, num_lights);
+  return num_lights < 0 ? 0 : partials(Cfg<SPECULAR>::kAcc, num_lights).bytes;
 }
 
 static int specular_args(Args& a, int64_t num_points, int num_lights, const float* light_amplitude,
@@ -1188,8 +1204,8 @@ int dibr_b200_specular_backward(int64_t num_points, int num_lights, const float*
   a.gl_amp = grad_light_amplitude; a.gl_dir = grad_light_direction; a.gl_sharp = grad_light_sharpness;
   if (num_lights > 0 && (a.gl_amp || a.gl_dir || a.gl_sharp)) {
     if (!workspace) return DIBR_B200_EINVAL;
-    if (workspace_bytes < dibr_b200_specular_workspace_bytes(num_lights)) return DIBR_B200_EWORKSPACE;
-    a.partial = (float*)workspace;
+    a.partial = carve_partials(partials(Cfg<SPECULAR>::kAcc, num_lights), workspace, workspace_bytes);
+    if (!a.partial) return DIBR_B200_EWORKSPACE;
   }
   cudaStream_t st = (cudaStream_t)stream;
   if (num_lights == 0) {   // empty sum: zero output, zero per-point gradients
@@ -1204,7 +1220,7 @@ int dibr_b200_specular_backward(int64_t num_points, int num_lights, const float*
 }
 
 size_t dibr_b200_sg_shade_workspace_bytes(int num_lights) {
-  return num_lights < 0 ? 0 : partial_bytes(Cfg<SHADE>::kAcc, num_lights);
+  return num_lights < 0 ? 0 : partials(Cfg<SHADE>::kAcc, num_lights).bytes;
 }
 
 static int shade_args(ShadeArgs& s, int batch, int height, int width, int num_lights, const float* camera,
@@ -1258,8 +1274,8 @@ int dibr_b200_sg_shade_backward(int batch, int height, int width, int num_lights
   const bool want_light = num_lights > 0 && (s.a.gl_amp || s.a.gl_dir || s.a.gl_sharp);
   if (want_light) {
     if (!workspace) return DIBR_B200_EINVAL;
-    if (workspace_bytes < dibr_b200_sg_shade_workspace_bytes(num_lights)) return DIBR_B200_EWORKSPACE;
-    s.a.partial = (float*)workspace;
+    s.a.partial = carve_partials(partials(Cfg<SHADE>::kAcc, num_lights), workspace, workspace_bytes);
+    if (!s.a.partial) return DIBR_B200_EWORKSPACE;
   }
   if (!want_light && !grad_albedo && !grad_spec_albedo && !grad_roughness && !grad_normals) return 0;
   return launch_shade_bwd(s, (cudaStream_t)stream);

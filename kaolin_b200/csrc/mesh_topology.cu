@@ -42,14 +42,14 @@ struct Span {
 
 using dibr_b200_detail::exclusive_scan;
 using dibr_b200_detail::kScanTile;
+using dibr_layout::carve;
+using dibr_layout::piece;
 
 constexpr int kScanThreads = 1024;
 static_assert(kScanTile == kScanThreads * 4, "scan_*_kernel: four elements per thread");
 constexpr int kShortRow = 32;                 // rows of at most this many corners are sorted by one thread
 constexpr int kLongCtas = 132;                // CTAs that share out the long rows
 constexpr int kThreads = 256;
-
-__host__ __device__ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 inline unsigned grid_for(int64_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
@@ -291,22 +291,6 @@ __global__ void __launch_bounds__(kThreads) topo_compact_kernel(Topo t) {
   for (int i = lane; i < n; i += 32) t.adj[b + i] = src[i];
 }
 
-struct TopoLayout {
-  size_t count, raw, sums, long_rows, long_count, bytes;
-};
-
-TopoLayout topo_layout(int V, int64_t corners, int R) {
-  TopoLayout l;
-  const size_t tiles = (size_t)(V + kScanTile - 1) / kScanTile + 1;
-  l.count = 0;
-  l.raw = align_up(l.count + sizeof(int) * (size_t)V, 256);
-  l.sums = align_up(l.raw + sizeof(int) * R * (size_t)corners, 256);
-  l.long_rows = align_up(l.sums + sizeof(int) * tiles, 256);
-  l.long_count = align_up(l.long_rows + sizeof(int) * (size_t)V, 256);
-  l.bytes = l.long_count + 256;
-  return l;
-}
-
 // 0, or the error: V must leave room for V + 1 offsets, and the R*F*S raw neighbour entries (so
 // every offset and every key k*F + f) must fit a 32-bit int.
 int topo_dims(int V, int64_t F, int S, int R = 2) {
@@ -315,10 +299,10 @@ int topo_dims(int V, int64_t F, int S, int R = 2) {
   return 0;
 }
 
-// The build of both CSRs, with the layout l in ws; arguments checked by the caller.
-int topo_build(Topo& t, char* ws, const TopoLayout& l, cudaStream_t st) {
-  t.count = (int*)(ws + l.count); t.raw = (int*)(ws + l.raw); t.sums = (int*)(ws + l.sums);
-  t.long_rows = (int*)(ws + l.long_rows); t.long_count = (int*)(ws + l.long_count);
+// The build of both CSRs, with the pieces l at the workspace origin o; arguments checked by the caller.
+int topo_build(Topo& t, char* o, const dibr_layout::TopoPieces& l, cudaStream_t st) {
+  t.count = piece<int>(o, l.count); t.raw = piece<int>(o, l.raw); t.sums = piece<int>(o, l.sums);
+  t.long_rows = piece<int>(o, l.long_rows); t.long_count = piece<int>(o, l.long_count);
   const int V = t.V;
   const int64_t FS = (int64_t)t.F * t.S;
   if (cudaMemsetAsync(t.status, 0, 2 * sizeof(int), st) != cudaSuccess) return (int)cudaGetLastError();
@@ -571,19 +555,6 @@ __global__ void __launch_bounds__(kThreads) subdiv_faces_kernel(Subdiv s) {
   for (int u = 0; u < 12; ++u) out[u] = v[kChild[u]];
 }
 
-struct SubdivLayout {
-  size_t count, sums, bytes;
-};
-
-SubdivLayout subdiv_layout(int V) {
-  SubdivLayout l;
-  const size_t tiles = (size_t)(V + kScanTile - 1) / kScanTile + 1;
-  l.count = 0;
-  l.sums = align_up(sizeof(int) * (size_t)V, 256);
-  l.bytes = l.sums + align_up(sizeof(int) * tiles, 256);
-  return l;
-}
-
 // The reference's default weight of a vertex of n neighbours, _get_alpha(n) * n, in its fp32 steps:
 // torch evaluates 2*pi / n as reciprocal(n) * 2*pi.  n = 0 gives NaN.
 __device__ __forceinline__ float default_alpha(int deg) {
@@ -752,24 +723,6 @@ __global__ void __launch_bounds__(kThreads) tet_edges_kernel(Subdiv s) {
     const int64_t a = v[kTetPairA[u]], b = v[kTetPairB[u]];
     s.face_edge[6 * (int64_t)t + u] = ok ? edge_id(s, (int)(a < b ? a : b), (int)(a < b ? b : a)) : -1;
   }
-}
-
-struct TetLayout {
-  TopoLayout topo;
-  size_t corner_ptr, corners, degree, weight, status, edge_ptr, bytes;
-};
-
-TetLayout tet_layout(int V, int64_t T) {
-  TetLayout l;
-  l.topo = topo_layout(V, 4 * T, 3);
-  l.corner_ptr = align_up(l.topo.bytes, 256);
-  l.corners = align_up(l.corner_ptr + sizeof(int) * ((size_t)V + 1), 256);
-  l.degree = align_up(l.corners + sizeof(int) * 4 * (size_t)T, 256);
-  l.weight = align_up(l.degree + sizeof(int) * (size_t)V, 256);
-  l.status = align_up(l.weight + sizeof(float) * (size_t)V, 256);
-  l.edge_ptr = l.status + 256;
-  l.bytes = align_up(l.edge_ptr + sizeof(int) * ((size_t)V + 1), 256);
-  return l;
 }
 
 // Marching tetrahedra.  occ(v) = sdf(v) > 0 (0 and NaN are outside).  A tet's case is
@@ -1028,7 +981,7 @@ extern "C" {
 
 size_t dibr_b200_mesh_topology_workspace_bytes(int num_vertices, int64_t num_faces, int face_size) {
   if (topo_dims(num_vertices, num_faces, face_size)) return 0;
-  return topo_layout(num_vertices, num_faces * face_size, 2).bytes;
+  return dibr_layout::mesh_topology_layout(num_vertices, num_faces, face_size).bytes;
 }
 
 int dibr_b200_mesh_topology_build(int num_vertices, int64_t num_faces, int face_size, const int64_t* faces,
@@ -1040,13 +993,14 @@ int dibr_b200_mesh_topology_build(int num_vertices, int64_t num_faces, int face_
   if (!corner_ptr || !adj_ptr || !status || !workspace) return DIBR_B200_EINVAL;
   if (FS > 0 && (!faces || !corners || !adj)) return DIBR_B200_EINVAL;
   if (num_vertices > 0 && (!degree || !weight)) return DIBR_B200_EINVAL;
-  const TopoLayout l = topo_layout(num_vertices, FS, 2);
-  if (workspace_bytes < l.bytes) return DIBR_B200_EWORKSPACE;
+  const dibr_layout::MeshTopologyLayout l = dibr_layout::mesh_topology_layout(num_vertices, num_faces, face_size);
+  char* o = carve(workspace, workspace_bytes, l.bytes);
+  if (!o) return DIBR_B200_EWORKSPACE;
   Topo t;
   t.V = num_vertices; t.S = face_size; t.R = 2; t.F = (int)num_faces; t.faces = faces;
   t.corner_ptr = corner_ptr; t.corners = corners; t.adj_ptr = adj_ptr; t.adj = adj; t.degree = degree;
   t.weight = weight; t.status = status;
-  return topo_build(t, (char*)workspace, l, (cudaStream_t)stream);
+  return topo_build(t, o, l.topo, (cudaStream_t)stream);
 }
 
 int dibr_b200_laplacian_apply(int batch, int num_vertices, int channels, const int32_t* adj_ptr, const int32_t* adj,
@@ -1143,7 +1097,7 @@ int dibr_b200_adjacency_coo(int num_vertices, int64_t num_edges, const int32_t* 
 
 size_t dibr_b200_loop_subdivision_workspace_bytes(int num_vertices, int64_t num_faces) {
   if (topo_dims(num_vertices, num_faces, 3)) return 0;
-  return subdiv_layout(num_vertices).bytes;
+  return dibr_layout::subdivision_layout(num_vertices).bytes;
 }
 
 int dibr_b200_loop_subdivision_build(int num_vertices, int64_t num_faces, const int64_t* faces,
@@ -1155,18 +1109,18 @@ int dibr_b200_loop_subdivision_build(int num_vertices, int64_t num_faces, const 
   if (!corner_ptr || !adj_ptr || !edge_ptr || !status || !workspace) return DIBR_B200_EINVAL;
   if (num_faces > 0 && (!faces || !corners || !adj || !adj_edge || !face_edge || !edges || !new_faces))
     return DIBR_B200_EINVAL;
-  const SubdivLayout l = subdiv_layout(num_vertices);
-  if (workspace_bytes < l.bytes) return DIBR_B200_EWORKSPACE;
-  char* ws = (char*)workspace;
+  const dibr_layout::SubdivisionLayout l = dibr_layout::subdivision_layout(num_vertices);
+  char* o = carve(workspace, workspace_bytes, l.bytes);
+  if (!o) return DIBR_B200_EWORKSPACE;
   Subdiv s;
   s.V = num_vertices; s.F = (int)num_faces; s.faces = faces;
   s.corner_ptr = corner_ptr; s.corners = corners; s.adj_ptr = adj_ptr; s.adj = adj;
-  s.count = (int*)(ws + l.count); s.edge_ptr = edge_ptr; s.adj_edge = adj_edge; s.face_edge = face_edge;
+  s.count = piece<int>(o, l.count); s.edge_ptr = edge_ptr; s.adj_edge = adj_edge; s.face_edge = face_edge;
   s.edges = (int4*)edges; s.new_faces = new_faces;
   cudaStream_t st = (cudaStream_t)stream;
   const int V = num_vertices;
   if (V > 0) { Span sp("subdiv_count_kernel", st); subdiv_count_kernel<<<grid_for(V, kThreads), kThreads, 0, st>>>(s); }
-  if (int e = exclusive_scan(s.count, V, (int*)(ws + l.sums), edge_ptr, st)) return e;
+  if (int e = exclusive_scan(s.count, V, piece<int>(o, l.sums), edge_ptr, st)) return e;
   if (num_faces > 0) {
     const int64_t capacity = 6 * num_faces;       // the adjacency holds at most 2 * F * 3 entries
     { Span sp("subdiv_edges_kernel", st); subdiv_edges_kernel<true><<<grid_for(capacity, kThreads), kThreads, 0, st>>>(s, capacity); }
@@ -1233,7 +1187,7 @@ int dibr_b200_loop_subdivision_backward(int batch, int num_vertices, int num_edg
 
 size_t dibr_b200_tet_topology_workspace_bytes(int num_vertices, int64_t num_tets) {
   if (topo_dims(num_vertices, num_tets, 4, 3)) return 0;
-  return tet_layout(num_vertices, num_tets).bytes;
+  return dibr_layout::tet_topology_layout(num_vertices, num_tets).bytes;
 }
 
 int dibr_b200_tet_topology_build(int num_vertices, int64_t num_tets, const int64_t* tets, int32_t* adj_ptr,
@@ -1242,21 +1196,21 @@ int dibr_b200_tet_topology_build(int num_vertices, int64_t num_tets, const int64
   if (const int e = topo_dims(num_vertices, num_tets, 4, 3)) return e;
   if (!adj_ptr || !status || !workspace) return DIBR_B200_EINVAL;
   if (num_tets > 0 && (!tets || !adj || !edges || !adj_edge || !tet_edge)) return DIBR_B200_EINVAL;
-  const TetLayout l = tet_layout(num_vertices, num_tets);
-  if (workspace_bytes < l.bytes) return DIBR_B200_EWORKSPACE;
-  char* ws = (char*)workspace;
+  const dibr_layout::TetTopologyLayout l = dibr_layout::tet_topology_layout(num_vertices, num_tets);
+  char* o = carve(workspace, workspace_bytes, l.bytes);
+  if (!o) return DIBR_B200_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int V = num_vertices;
   Topo t;
   t.V = V; t.S = 4; t.R = 3; t.F = (int)num_tets; t.faces = tets;
-  t.corner_ptr = (int*)(ws + l.corner_ptr); t.corners = (int*)(ws + l.corners); t.adj_ptr = adj_ptr; t.adj = adj;
-  t.degree = (int*)(ws + l.degree); t.weight = (float*)(ws + l.weight); t.status = (int*)(ws + l.status);
-  if (int e = topo_build(t, ws, l.topo, st)) return e;
+  t.corner_ptr = piece<int>(o, l.corner_ptr); t.corners = piece<int>(o, l.corners); t.adj_ptr = adj_ptr; t.adj = adj;
+  t.degree = piece<int>(o, l.degree); t.weight = piece<float>(o, l.weight); t.status = piece<int>(o, l.status);
+  if (int e = topo_build(t, o, l.topo, st)) return e;
   // the topology's count (all zero again) and scan partials serve the edge numbering
   Subdiv s;
   s.V = V; s.F = (int)num_tets; s.faces = tets;
   s.corner_ptr = t.corner_ptr; s.corners = t.corners; s.adj_ptr = adj_ptr; s.adj = adj;
-  s.count = t.count; s.edge_ptr = (int*)(ws + l.edge_ptr); s.adj_edge = adj_edge; s.face_edge = tet_edge;
+  s.count = t.count; s.edge_ptr = piece<int>(o, l.edge_ptr); s.adj_edge = adj_edge; s.face_edge = tet_edge;
   s.edges = nullptr; s.new_faces = nullptr; s.pairs = (int2*)edges;
   if (V > 0) { Span sp("subdiv_count_kernel", st); subdiv_count_kernel<<<grid_for(V, kThreads), kThreads, 0, st>>>(s); }
   if (int e = exclusive_scan(s.count, V, t.sums, s.edge_ptr, st)) return e;
@@ -1294,9 +1248,7 @@ static int mt_dims(int batch, int V, int E, int64_t T) {
 
 size_t dibr_b200_marching_tets_workspace_bytes(int batch, int num_edges, int64_t num_tets) {
   if (mt_dims(batch, 0, num_edges, num_tets)) return 0;
-  const int64_t n = (int64_t)batch * (num_edges + 2 * num_tets);
-  const size_t tiles = (size_t)(n + kScanTile - 1) / kScanTile + 1;
-  return align_up(sizeof(int) * (size_t)n, 256) + align_up(sizeof(int) * tiles, 256);
+  return dibr_layout::marching_tets_layout(batch, num_edges, num_tets).bytes;
 }
 
 int dibr_b200_marching_tets_count(int batch, int num_vertices, int num_edges, int64_t num_tets, const int32_t* edges,
@@ -1308,12 +1260,14 @@ int dibr_b200_marching_tets_count(int batch, int num_vertices, int num_edges, in
   if (num_edges > 0 && !edges) return DIBR_B200_EINVAL;
   if (num_tets > 0 && !tets) return DIBR_B200_EINVAL;
   if (batch > 0 && num_vertices > 0 && !sdf) return DIBR_B200_EINVAL;
-  if (workspace_bytes < dibr_b200_marching_tets_workspace_bytes(batch, num_edges, num_tets)) return DIBR_B200_EWORKSPACE;
+  const dibr_layout::MarchingTetsLayout l = dibr_layout::marching_tets_layout(batch, num_edges, num_tets);
+  char* o = carve(workspace, workspace_bytes, l.bytes);
+  if (!o) return DIBR_B200_EWORKSPACE;
   MTets m = {};
   m.B = batch; m.V = num_vertices; m.E = num_edges; m.T = (int)num_tets;
-  m.edges = (const int2*)edges; m.tets = tets; m.sdf = sdf; m.flags = (int*)workspace; m.scan = scan;
+  m.edges = (const int2*)edges; m.tets = tets; m.sdf = sdf; m.flags = piece<int>(o, l.flags); m.scan = scan;
   const int64_t n = (int64_t)batch * (num_edges + 2 * num_tets);
-  int* sums = (int*)((char*)workspace + align_up(sizeof(int) * (size_t)n, 256));
+  int* sums = piece<int>(o, l.sums);
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t classify = (int64_t)batch * (num_edges + num_tets);
   if (classify > 0) { Span s("mt_classify_kernel", st); mt_classify_kernel<<<grid_for(classify, kThreads), kThreads, 0, st>>>(m); }

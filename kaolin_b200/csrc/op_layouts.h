@@ -1,0 +1,224 @@
+// op_layouts.h — where every operator outside the rasterizer keeps its scratch in the caller's workspace.
+//
+// One function per operator family returns its pieces and its total; the family's size query returns
+// that total and its entry points carve with the same function, so the two cannot disagree.  Plain
+// C++ without CUDA, so that tests/host_math can compile it on a CPU and check each piece's place.
+//
+// Every family follows one rule (the rasterizer's workspace_layout.h uses the same origin and fit):
+//   - pieces go back to back from the origin, each starting on a multiple of kAlign;
+//   - the origin is the workspace pointer rounded up to kAlign, so a workspace of any alignment works;
+//   - the total is the end of the last piece plus kAlign, which covers that rounding; the workspace
+//     fits when it is not NULL and holds the total.
+// A memset that clears several counters clears one piece that holds them all.
+#pragma once
+#include <stddef.h>
+#include <stdint.h>
+
+namespace dibr_layout {
+
+constexpr size_t kAlign = 256;
+constexpr int kScanTile = 4096;   // elements per CTA of the exclusive scan (scan.cuh)
+constexpr int kMaxCells = 16;     // grid cells a face may be inserted in; wider faces go to the view's wide list
+
+inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+struct Piece { size_t at, bytes; };
+
+// Places pieces back to back, each rounded up to kAlign; total() adds kAlign of slack for the origin.
+struct Placer {
+  size_t at = 0, end = 0;
+  Piece put(size_t bytes) {
+    const Piece p = {at, bytes};
+    end = at + bytes;
+    at += align_up(bytes, kAlign);
+    return p;
+  }
+  size_t total() const { return end + kAlign; }
+};
+
+// Bytes from the workspace pointer to the origin.
+inline size_t origin_offset(const void* ws) {
+  const uintptr_t p = (uintptr_t)ws;
+  return align_up(p, kAlign) - p;
+}
+
+inline bool fits(const void* ws, size_t ws_bytes, size_t bytes) { return ws && ws_bytes >= bytes; }
+
+// The origin of a workspace that fits a layout of `bytes`, or NULL.
+inline char* carve(void* ws, size_t ws_bytes, size_t bytes) {
+  return fits(ws, ws_bytes, bytes) ? (char*)ws + origin_offset(ws) : nullptr;
+}
+
+template <typename T>
+T* piece(char* origin, Piece p) { return reinterpret_cast<T*>(origin + p.at); }
+
+// The exclusive scan's tile sums for n elements (one int per tile and one spare).
+inline size_t scan_sums_bytes(int64_t n) { return sizeof(int) * (size_t)((n + kScanTile - 1) / kScanTile + 1); }
+
+// ---------------------------------------------------------------------------------------------
+// The per-view face grid of grid_bins.cuh, shared by DefTet and the check_sign build.
+
+// G x G cells for F faces per view: about one face per cell before overlaps.
+inline int grid_side(int F) {
+  int G = 8;
+  while (G < 256 && (int64_t)G * G < F) G += 8;
+  return G;
+}
+
+// counters holds cnt and off, [B][G*G + 1] int each and each from a multiple of kAlign: the check_sign
+// build clears both with one memset.
+struct GridBins { Piece bounds, counters, cnt, off, entries, wide; };
+
+inline GridBins grid_bins(Placer& p, int B, int F) {
+  const size_t G = (size_t)grid_side(F), nf = (size_t)B * (size_t)(F > 0 ? F : 1);
+  const size_t cells = (size_t)B * (G * G + 1) * sizeof(int), room = align_up(cells, kAlign);
+  GridBins g;
+  g.bounds = p.put((size_t)B * 4 * sizeof(float));
+  g.counters = p.put(2 * room);
+  g.cnt = {g.counters.at, cells};
+  g.off = {g.counters.at + room, cells};
+  g.entries = p.put(nf * kMaxCells * sizeof(int));
+  g.wide = p.put(nf * sizeof(int));
+  return g;
+}
+
+struct DeftetLayout { GridBins grid; size_t bytes; };
+
+inline DeftetLayout deftet_layout(int B, int F) {
+  Placer p;
+  DeftetLayout L;
+  L.grid = grid_bins(p, B, F);
+  L.bytes = p.total();
+  return L;
+}
+
+// The check_sign build ("mesh"), which its queries read: the normalising scale maxlen [B] T, the grid,
+// the face boxes [B][F] float4 and the face records [B][F][9] T, for T of tsize bytes.
+struct CheckSignBuildLayout { Piece maxlen; GridBins grid; Piece boxes, records; size_t bytes; };
+
+inline CheckSignBuildLayout check_sign_build_layout(int B, int F, size_t tsize) {
+  const size_t nf = (size_t)B * (size_t)(F > 0 ? F : 1);
+  Placer p;
+  CheckSignBuildLayout L;
+  L.maxlen = p.put((size_t)B * tsize);
+  L.grid = grid_bins(p, B, F);
+  L.boxes = p.put(nf * 4 * sizeof(float));
+  L.records = p.put(nf * 9 * tsize);
+  L.bytes = p.total();
+  return L;
+}
+
+// A check_sign query of N points per view: the points binned on the build's grid (cnt, off as in the
+// grid) and each point's cell and place in cell order.
+struct CheckSignQueryLayout { Piece cnt, off, pcell, order; size_t bytes; };
+
+inline CheckSignQueryLayout check_sign_query_layout(int B, int F, int N) {
+  const size_t G = (size_t)grid_side(F), np = (size_t)B * (size_t)(N > 0 ? N : 1);
+  const size_t cells = (size_t)B * (G * G + 1) * sizeof(int);
+  Placer p;
+  CheckSignQueryLayout L;
+  L.cnt = p.put(cells);
+  L.off = p.put(cells);
+  L.pcell = p.put(np * sizeof(int));
+  L.order = p.put(np * sizeof(int));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
+// mesh_topology.cu
+
+// The CSR build of V vertices and `corners` corners with R raw neighbours each: per-vertex counts, the
+// raw neighbours, the scan's tile sums, the long-row list and its counter.
+struct TopoPieces { Piece count, raw, sums, long_rows, long_count; };
+
+inline TopoPieces topo_pieces(Placer& p, int V, int64_t corners, int R) {
+  TopoPieces t;
+  t.count = p.put(sizeof(int) * (size_t)V);
+  t.raw = p.put(sizeof(int) * (size_t)R * (size_t)corners);
+  t.sums = p.put(scan_sums_bytes(V));
+  t.long_rows = p.put(sizeof(int) * (size_t)V);
+  t.long_count = p.put(sizeof(int));
+  return t;
+}
+
+struct MeshTopologyLayout { TopoPieces topo; size_t bytes; };
+
+inline MeshTopologyLayout mesh_topology_layout(int V, int64_t F, int S) {
+  Placer p;
+  MeshTopologyLayout L;
+  L.topo = topo_pieces(p, V, F * S, 2);
+  L.bytes = p.total();
+  return L;
+}
+
+// Loop subdivision's edge numbering: per-vertex counts and the scan's tile sums.
+struct SubdivisionLayout { Piece count, sums; size_t bytes; };
+
+inline SubdivisionLayout subdivision_layout(int V) {
+  Placer p;
+  SubdivisionLayout L;
+  L.count = p.put(sizeof(int) * (size_t)V);
+  L.sums = p.put(scan_sums_bytes(V));
+  L.bytes = p.total();
+  return L;
+}
+
+// The tet-mesh topology: the CSR build of T tets (R = 3), then the corner CSR, degrees, weights and the
+// build's two status words, which the caller does not keep, and the edge offsets [V + 1].
+struct TetTopologyLayout { TopoPieces topo; Piece corner_ptr, corners, degree, weight, status, edge_ptr; size_t bytes; };
+
+inline TetTopologyLayout tet_topology_layout(int V, int64_t T) {
+  Placer p;
+  TetTopologyLayout L;
+  L.topo = topo_pieces(p, V, 4 * T, 3);
+  L.corner_ptr = p.put(sizeof(int) * ((size_t)V + 1));
+  L.corners = p.put(sizeof(int) * 4 * (size_t)T);
+  L.degree = p.put(sizeof(int) * (size_t)V);
+  L.weight = p.put(sizeof(float) * (size_t)V);
+  L.status = p.put(2 * sizeof(int));
+  L.edge_ptr = p.put(sizeof(int) * ((size_t)V + 1));
+  L.bytes = p.total();
+  return L;
+}
+
+// Marching tets: one flag per (view, edge) and two per (view, tet), and the scan's tile sums.
+struct MarchingTetsLayout { Piece flags, sums; size_t bytes; };
+
+inline MarchingTetsLayout marching_tets_layout(int B, int E, int64_t T) {
+  const int64_t n = (int64_t)B * (E + 2 * T);
+  Placer p;
+  MarchingTetsLayout L;
+  L.flags = p.put(sizeof(int) * (size_t)n);
+  L.sums = p.put(scan_sums_bytes(n));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
+// marching_cubes.cu: the triangle and owned-vertex counts of `cubes` cubes (all views), one after the
+// other, and the scan's tile sums.
+struct MarchingCubesLayout { Piece counts, sums; size_t bytes; };
+
+inline MarchingCubesLayout marching_cubes_layout(int64_t cubes) {
+  Placer p;
+  MarchingCubesLayout L;
+  L.counts = p.put(2 * sizeof(int) * (size_t)cubes);
+  L.sums = p.put(scan_sums_bytes(cubes));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
+// lighting.cu: the light gradients' partial sums, `floats` per light in each of `slots` CTA slots.
+struct LightingLayout { Piece partial; size_t bytes; };
+
+inline LightingLayout lighting_layout(int slots, int floats, int lights) {
+  Placer p;
+  LightingLayout L;
+  L.partial = p.put((size_t)slots * (size_t)lights * (size_t)floats * sizeof(float));
+  L.bytes = p.total();
+  return L;
+}
+
+}  // namespace dibr_layout

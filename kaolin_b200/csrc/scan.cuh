@@ -3,12 +3,14 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "op_layouts.h"
+
 namespace dibr_b200_detail {
 
-constexpr int kScanTile = 4096;   // elements per CTA: `sums` holds ceil(n / kScanTile) ints
+using dibr_layout::kScanTile;   // elements per CTA
 
 // Exclusive scan in[n] -> out[n + 1] (out[n] = the total), enqueued on st; `in` and `out` must not
-// overlap.  Returns a cudaError_t.
+// overlap, and `sums` holds dibr_layout::scan_sums_bytes(n).  Returns a cudaError_t.
 int exclusive_scan(const int* in, int n, int* sums, int* out, cudaStream_t st);
 
 }  // namespace dibr_b200_detail

@@ -23,19 +23,18 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "op_layouts.h"
+
 namespace dibr_layout {
 
 constexpr int kTile = 16;         // px per side of a screen tile, the finest bin
 constexpr int kMaxLevels = 6;     // 16 * 4^5 = 16384 px
 constexpr int kBandRec = 24;      // ints per record of the soft-mask work list
 constexpr int kRowWalkMaxD = 4;   // the largest feature dim the row-walk rasterize backward takes
-constexpr size_t kAlign = 256;
 constexpr size_t kInt4Bytes = 4 * sizeof(int);
 
 // Floats per face record of the row-walk backward: 6 vertex-gradient and 3*D feature sums, padded to float4.
 constexpr int face_record_floats(int D) { return (6 + 3 * D + 3) & ~3; }
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 inline int levels_for(int H, int W) {
   int L = 1;
@@ -52,8 +51,6 @@ inline int bins_per_view(int H, int W) {
   }
   return nb;
 }
-
-struct Piece { size_t at, bytes; };
 
 struct LayoutShape {
   int B;          // views
@@ -141,8 +138,8 @@ inline WorkspaceLayout workspace_layout(const LayoutShape& s, int64_t cache_tile
 // the hit cache takes as many tiles, up to all of them, as the rest of the workspace holds.
 inline WorkspaceLayout workspace_layout(const LayoutShape& s, const void* ws, size_t ws_bytes) {
   WorkspaceLayout L = workspace_layout(s, 0);
-  L.origin = align_up((size_t)(uintptr_t)ws, kAlign) - (size_t)(uintptr_t)ws;
-  L.fits = ws && ws_bytes >= L.min_bytes;
+  L.origin = origin_offset(ws);
+  L.fits = fits(ws, ws_bytes, L.min_bytes);
   if (L.fits && s.knum > 0) {
     const size_t room = ws_bytes - L.origin;   // from the origin to the workspace's end
     size_t n = (room - L.cache_hdr.at) / (kInt4Bytes + cache_tile_data_bytes(s.knum));

@@ -78,7 +78,7 @@ class _Topology:
         own = status is None
         if own:
             status = torch.empty(2, **i32)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        ws = _lib.scratch(nbytes, dev)
         _lib.call("dibr_b200_mesh_topology_build", dev,
                   V, F, S, faces, self.corner_ptr, self.corners, self.adj_ptr, self._adj, self.degree, self.weight,
                   status, ws, nbytes, what=func)

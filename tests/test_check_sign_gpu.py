@@ -239,3 +239,23 @@ def test_raw_operator_argument_checks():
     with pytest.raises(RuntimeError):
         op(p.half(), v.half(), v.half(), v.half())                     # dispatch: float and double only
     assert op(p, v, v, v).dtype == torch.float32 and not op(p, v, v, v).any()
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    s = SCENES["batch3"]
+    verts, faces, points = t(s["verts"]), t(s["faces"]), t(s["points"])
+    raw = SCENES["raw_soup"]
+    args = [t(raw[k]) for k in ("points", "verts_1", "verts_2", "verts_3")]
+
+    def run():
+        return [check_sign(verts, faces, points), CheckSign(verts, faces)(points),
+                _C.ops.mesh.unbatched_mesh_intersection_cuda(*args)]
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

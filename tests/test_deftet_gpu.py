@@ -11,6 +11,7 @@ import torch
 
 from oracle import deftet as DT
 from kaolin_b200 import _C as b200_C
+from kaolin_b200 import _lib
 from kaolin_b200.render.mesh import deftet_sparse_render
 
 pytestmark = pytest.mark.gpu
@@ -93,3 +94,20 @@ def test_deftet_public_api_and_gradients_vs_torch_restatement():
     (feat * gw).sum().backward(); (r_feat * gw).sum().backward()
     close(t_ff.grad, r_ff.grad, 1e-5)
     close(t_fvi.grad, r_fvi.grad, 1e-4)
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    fvi, fvz, ff, pix, rr = _scene(2, 1500, 700, 0.8, 0.25, 9)
+    bb = np.concatenate([fvi.min(2), fvi.max(2)], -1)
+
+    def run():
+        return b200_C.render.mesh.deftet_sparse_render_forward_cuda(T(fvz), T(fvi), T(bb), T(pix), T(rr), 24, 1e-8)
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

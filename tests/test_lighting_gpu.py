@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from oracle import lighting as OL
-from kaolin_b200 import synthetic
+from kaolin_b200 import _lib, synthetic
 from kaolin_b200.render import lighting
 from kaolin_b200.render.mesh import rasterize, texture_mapping
 
@@ -245,3 +245,31 @@ def test_operator_shim_error_wording():
     nc = torch.rand(3, 4, device=DEV).t()
     close(lighting.unbatched_reduced_sg_inner_product(cu[0], nc, *cu[2:]),
           lighting.unbatched_reduced_sg_inner_product(cu[0], nc.contiguous(), *cu[2:]), 0.0)
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    gen = torch.Generator(device=DEV); gen.manual_seed(9)
+    N = 10_001
+    n = torch.nn.functional.normalize(torch.randn((N, 3), device=DEV, generator=gen), dim=-1)
+    al = torch.rand((N, 3), device=DEV, generator=gen)
+    w = torch.rand((N, 3), device=DEV, generator=gen)
+    lights, sh = list(_lights(8, gen)), [torch.rand((9,), device=DEV, generator=gen) - 0.5]
+    general = [al, n, torch.rand((N,), device=DEV, generator=gen) * 5 + 0.5, *_lights(5, gen)]
+
+    def run():
+        outs = []
+        for fn, ins, wi in ((MODELS["diff_ip"][0], lights + [n, al], w), (MODELS["fitted"][0], lights + [n, al], w),
+                            (lighting.sh9_irradiance, sh + [n], w[:, 0]),
+                            (lighting.unbatched_reduced_sg_inner_product, general, w)):
+            o, grads = _run(fn, ins, wi)
+            outs += [o, *grads]
+        return outs
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

@@ -91,12 +91,13 @@ def _ws(B, X, Y, Z, pad):
     return _lib.lib().dibr_b200_marching_cubes_workspace_bytes(B, X, Y, Z, pad, ctypes.byref(out)), out.value
 
 
-def test_workspace_bytes_and_size_limits():
+def test_aligned_workspace_bytes_and_size_limits():
     status, nbytes = _ws(2, 256, 256, 256, 1)
     cubes = 2 * 258 ** 3
     align = lambda v: (v + 255) // 256 * 256
-    assert status == 0 and nbytes == align(8 * cubes) + align(4 * (-(-cubes // 4096) + 1))
-    assert _ws(0, 3, 3, 3, 1) == (0, 256)
+    # the counts, the scan's tile sums from the next 256-byte boundary, and 256 bytes to align the pointer
+    assert status == 0 and nbytes == align(8 * cubes) + 4 * (-(-cubes // 4096) + 1) + 256
+    assert _ws(0, 3, 3, 3, 1) == (0, 4 + 256)
     for args in ((-1, 2, 2, 2, 1), (1, 0, 2, 2, 1), (1, 2, -3, 2, 0), (1, 2, 2, 2, 2)):
         assert _ws(*args)[0] == _lib.EINVAL, args
     # B * (X + 2)^3 must not exceed (2^31 - 1) // 5 = 429 496 729: 754^3 fits, 755^3 does not

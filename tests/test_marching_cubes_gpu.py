@@ -12,7 +12,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from kaolin_b200 import _C
+from kaolin_b200 import _C, _lib
 from kaolin_b200.ops import conversions
 from oracle import build_ref_mcube, ref_golden_mcube
 from oracle import marching_cubes as O
@@ -299,3 +299,20 @@ def test_256_cubed_two_views_in_bounded_memory():
         v1, f1 = mc(grid[b:b + 1])
         assert torch.equal(verts[b], v1[0]) and torch.equal(faces[b], f1[0])
         assert int(faces[b].min()) == 0 and int(faces[b].max()) == verts[b].shape[0] - 1
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    grid = torch.from_numpy(np.stack([occupancy(24, 23), occupancy(24, 24)])).to(DEV)
+
+    def run():
+        verts, faces = mc(grid)
+        return [torch.cat(verts), torch.cat(faces)]
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

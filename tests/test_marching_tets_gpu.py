@@ -429,3 +429,23 @@ def test_dmtet_tutorial_step_matches_the_oracle():
     assert torch.equal(ff, rff)
     for k in (slice(0, 1), slice(1, 4)):          # the sdf and the deformation
         assert float((g[:, k].double() - rg[:, k]).abs().max()) <= 1e-5 * float(rg[:, k].abs().max())
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    verts, tets_np = grid(16, 3)
+    v, s = sphere_sdf(verts, 3, 4)
+    feats = torch.randn((3, len(verts), 2), device=DEV)
+    tets = T_(tets_np)
+
+    def run():
+        verts_out, faces, tet_idx = conversions.MarchingTetrahedra(len(verts), tets)(v, s, True)
+        return [torch.cat(verts_out), torch.cat(faces), torch.cat(tet_idx), *mesh.subdivide_tetmesh(v, tets, feats)]
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

@@ -289,3 +289,24 @@ def test_tutorial_step_matches_the_dense_laplacian():
     rv, rt = step(lambda d: torch.matmul(Ld, d))
     assert float((gv - rv).abs().max()) <= 1e-5 * float(rv.abs().max())
     assert float((gt - rt).abs().max()) <= 1e-5 * float(rt.abs().max())
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    V, f = synthetic.icosphere(3)
+    faces_np = np.concatenate([np.asarray(f), fan(300)[1]])            # a long row among short ones
+    V = max(len(V), 302)
+    faces = T(faces_np)
+    x = torch.randn((2, V, 3), generator=torch.Generator(device="cpu").manual_seed(2)).to(DEV)
+
+    def run():
+        L = mesh.UniformLaplacian(V, faces)
+        return [L @ x, L.to_dense(), mesh.adjacency_matrix(V, faces)._indices()]
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

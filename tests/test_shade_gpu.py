@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from oracle import shade as OSH
+from kaolin_b200 import _lib
 from kaolin_b200.render import easy_render, lighting
 
 pytestmark = pytest.mark.gpu
@@ -240,3 +241,20 @@ def test_edge_sizes(B, H, W, L, cov):
         close(o, r)
     for gr, r in zip(grads, rg):
         close(gr, r)
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    cam, face_idx, ins, ws = batch(2, 32, 40, 5, seed=13)
+
+    def shade():
+        outs, grads = run(easy_render.sg_shade, cam, face_idx, ins, ws)
+        return [*outs, *grads]
+
+    want = shade()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = shade()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

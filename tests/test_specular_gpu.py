@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle import specular as OS
-from kaolin_b200 import synthetic
+from kaolin_b200 import _lib, synthetic
 from kaolin_b200.render import lighting
 from kaolin_b200.render.mesh import rasterize, texture_mapping
 
@@ -213,3 +213,22 @@ def test_float64_inputs_are_rejected():
     ins = _lights(2, gen) + _points(5, gen)
     with pytest.raises(RuntimeError, match="not implemented for 'float64'"):
         lighting.sg_warp_specular_term(*[t.double() for t in ins])
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    gen = torch.Generator(device=DEV); gen.manual_seed(9)
+    N = 10_001
+    ins, w = _lights(8, gen) + _points(N, gen), torch.rand((N, 3), device=DEV, generator=gen)
+
+    def run():
+        o, grads = _run(lighting.sg_warp_specular_term, ins, w)
+        return [o, *grads]
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)

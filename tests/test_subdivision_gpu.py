@@ -384,3 +384,22 @@ def test_tutorial_step_matches_the_oracle_subdivision():
     rv, ra = step(oracle_step)
     assert float((gv - rv).abs().max()) <= 1e-5 * float(rv.abs().max())
     assert float((ga - ra).abs().max()) <= 1e-5 * float(ra.abs().max())
+
+
+def test_workspace_at_an_odd_address(monkeypatch):
+    """Every workspace starting at byte 1 of a larger buffer: the outputs of an aligned one."""
+    v, f = synthetic.icosphere(3)
+    faces = T(np.asarray(f, np.int64))
+    x = torch.randn((2, len(v), 3), generator=torch.Generator(device="cpu").manual_seed(3)).to(DEV)
+
+    def run():
+        S = mesh.LoopSubdivision(len(v), faces, 2)
+        return [S(x), S.faces]
+
+    want = run()
+    scratch, odd = _lib.scratch, []
+    monkeypatch.setattr(_lib, "scratch", lambda n, device: odd.append(n) or scratch(int(n) + 1, device)[1:])
+    got = run()
+    assert odd
+    for a, b in zip(want, got):
+        assert torch.equal(a, b)
