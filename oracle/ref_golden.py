@@ -8,9 +8,14 @@ output or a face of a gradient output; half of the sample is drawn from the rows
 (covered pixels, faces with a gradient), half from all rows, plus the row of the largest magnitude.
 Outputs named in ``full=``, and outputs of at most 2 * SAMPLE_ROWS rows, are stored whole.
 
+A test may keep its cases in a store file of its own (``path=``), with fewer sampled rows
+(``sample_rows=``) and, for outputs it only compares bit for bit (``digest_only=``), nothing but the
+digest and the shape: the float32 binning matrix keeps thousands of outputs in
+``tests/golden/ref_cuda_binning.npz`` that way.
+
 Regenerate on a GPU with oracle/_ref built (``oracle/build_ref.py``) by running the GPU tests with
-``KAOLIN_REF_CUDA_RECORD=1``: every ``reference()`` call then runs the reference and the file is
-rewritten when the process exits.
+``KAOLIN_REF_CUDA_RECORD=1``: every ``reference()`` call then runs the reference and each store it
+recorded into is rewritten when the process exits.
 """
 import atexit
 import hashlib
@@ -24,8 +29,8 @@ RECORD = os.environ.get("KAOLIN_REF_CUDA_RECORD") == "1"
 SAMPLE_ROWS = 256         # outputs of at most 2 * SAMPLE_ROWS rows are stored whole
 _PIXEL_DIMS = 3          # (B, H, W[, D]) image outputs; everything else is (B, F, ...) per face
 
-_stored = None
-_recorded = {}
+_stored = {}       # path -> {case: {name: {field: array}}}
+_recorded = {}     # path -> {case: ...}, the cases recorded by this process
 
 
 def _numpy(t):
@@ -46,20 +51,22 @@ def _row_view(name, a):
     return a.reshape(int(np.prod(a.shape[:lead])), -1)
 
 
-def _compact(case, name, t, full):
+def _compact(case, name, t, full, sample_rows=SAMPLE_ROWS, digest_only=False):
     a = _numpy(t)
+    e = {"sha": np.array(_digest(a)), "shape": np.array(a.shape, np.int64)}
+    if digest_only:
+        return e
     rows = _row_view(name, a)
     mag = np.abs(rows.astype(np.float64))
-    e = {"sha": np.array(_digest(a)), "shape": np.array(a.shape, np.int64),
-         "scale": np.array(mag.max() if mag.size else 0.0)}
-    if full or rows.shape[0] <= 2 * SAMPLE_ROWS:
+    e["scale"] = np.array(mag.max() if mag.size else 0.0)
+    if full or rows.shape[0] <= 2 * sample_rows:
         e["values"] = rows
         return e
     rng = np.random.default_rng(int(hashlib.sha256(f"{case}.{name}".encode()).hexdigest()[:8], 16))
     marked = np.flatnonzero((rows != -1).any(1) if name == "face_idx" else (rows != 0).any(1))
-    n = min(SAMPLE_ROWS // 2, marked.size)
+    n = min(sample_rows // 2, marked.size)
     pick = [marked[rng.choice(marked.size, n, replace=False)] if n else np.zeros(0, np.int64),
-            rng.choice(rows.shape[0], SAMPLE_ROWS // 2, replace=False)]
+            rng.choice(rows.shape[0], sample_rows // 2, replace=False)]
     if mag.size:
         pick.append(np.array([np.unravel_index(np.argmax(mag), mag.shape)[0]]))
     e["rows"] = np.unique(np.concatenate(pick)).astype(np.int32)
@@ -70,12 +77,12 @@ def _compact(case, name, t, full):
 class Reference:
     """The stored outputs of one case."""
 
-    def __init__(self, case, entries):
-        self.case, self.e = case, entries
+    def __init__(self, case, entries, path=PATH):
+        self.case, self.e, self.path = case, entries, path
 
     def _entry(self, name):
         if name not in self.e:
-            raise KeyError(f"{self.case}: no stored reference output {name!r} in {PATH}")
+            raise KeyError(f"{self.case}: no stored reference output {name!r} in {self.path}")
         return self.e[name]
 
     def equal(self, name, ours):
@@ -97,39 +104,41 @@ class Reference:
         return _row_view(name, a)[self.rows(name)], e["values"]
 
 
-def _load():
-    global _stored
-    if _stored is None:
-        _stored = {}
-        if os.path.exists(PATH):
-            with np.load(PATH) as z:
+def _load(path):
+    if path not in _stored:
+        _stored[path] = {}
+        if os.path.exists(path):
+            with np.load(path) as z:
                 for k in z.files:
                     case, name, field = k.rsplit(".", 2)
-                    _stored.setdefault(case, {}).setdefault(name, {})[field] = z[k]
-    return _stored
+                    _stored[path].setdefault(case, {}).setdefault(name, {})[field] = z[k]
+    return _stored[path]
 
 
 def _save():
-    if not _recorded:
-        return
-    merged = {c: dict(v) for c, v in _load().items()}
-    merged.update(_recorded)
-    flat = {f"{c}.{n}.{f}": v for c, names in merged.items() for n, fields in names.items()
-            for f, v in fields.items()}
-    np.savez_compressed(PATH, **flat)
+    for path, recorded in _recorded.items():
+        merged = {c: dict(v) for c, v in _load(path).items()}
+        merged.update(recorded)
+        flat = {f"{c}.{n}.{f}": v for c, names in merged.items() for n, fields in names.items()
+                for f, v in fields.items()}
+        np.savez_compressed(path, **flat)
 
 
-def reference(case, live, names=("face_idx", "features", "soft_mask", "grad_fvi", "grad_ff"), full=()):
-    """The reference's outputs ``names`` for ``case``.  ``live()`` runs the reference (oracle/_ref) and
-    returns {name: tensor}; it is called only when recording."""
+def reference(case, live, names=("face_idx", "features", "soft_mask", "grad_fvi", "grad_ff"), full=(),
+              path=PATH, sample_rows=SAMPLE_ROWS, digest_only=()):
+    """The reference's outputs ``names`` for ``case`` in the store ``path``.  ``live()`` runs the
+    reference (oracle/_ref) and returns {name: tensor}; it is called only when recording.  Outputs in
+    ``full`` are stored whole, those in ``digest_only`` as their digest and shape alone, the others
+    whole up to 2 * sample_rows rows and as a sample of sample_rows rows above that."""
     case = case.replace(".", "p")
     if RECORD:
         if not _recorded:
             atexit.register(_save)
         out = {k: v for k, v in live().items() if k in names}
-        _recorded[case] = {k: _compact(case, k, v, k in full) for k, v in out.items()}
-        return Reference(case, _recorded[case])
-    stored = _load()
+        entries = {k: _compact(case, k, v, k in full, sample_rows, k in digest_only) for k, v in out.items()}
+        _recorded.setdefault(path, {})[case] = entries
+        return Reference(case, entries, path)
+    stored = _load(path)
     if case not in stored:
-        raise KeyError(f"no stored reference outputs for {case!r} in {PATH}")
-    return Reference(case, stored[case])
+        raise KeyError(f"no stored reference outputs for {case!r} in {path}")
+    return Reference(case, stored[case], path)
