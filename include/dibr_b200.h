@@ -406,6 +406,36 @@ int dibr_b200_mesh_intersection_count(int num_faces, int num_points, int dtype, 
                                       void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
 
 /*
+ * Point-to-mesh distance (kaolin/metrics/trianglemesh.py:20-99, 125-149; kaolin_b200/csrc/point_mesh_distance.cu).
+ * points (batch, N, 3) and face_vertices (batch, F, 3, 3), both of `dtype` (DIBR_B200_DTYPE_F32 or _F64),
+ * contiguous; each view's points against that view's faces.
+ * dibr_b200_point_mesh_distance_workspace_bytes: the workspace of the forward and of the backward.
+ * dibr_b200_point_mesh_distance_forward: per point, the squared distance `dist` (batch, N) `dtype` to the
+ *   nearest face, its index `face_idx` (batch, N) int64 within the view and its type `dist_type` (batch, N)
+ *   int32 (0 face, 1-3 vertex v1-v3, 4-6 edge v1v2, v2v3, v3v1), every pair evaluated with the reference
+ *   kernel's arithmetic; the smallest distance wins, the lowest face index among equals.  dist is rounded
+ *   to float in both dtypes, as the reference's double kernel does.  A face whose distance is NaN wins
+ *   only when every face is NaN for the point; then face 0 and its distance and type are written.
+ *   With F = 0 the outputs are left as they are.
+ * dibr_b200_point_mesh_distance_backward: grad_dist (batch, N) -> grad_points (batch, N, 3), WRITTEN, and
+ *   grad_face_vertices (batch, F, 3, 3), ADDED TO: each face's points add their terms in ascending point
+ *   order (no float atomics; in float32 each addition flushes subnormals, as the reference's atomicAdd
+ *   does).  Either output may be NULL.  A point whose face_idx is outside [0, F) contributes nothing and
+ *   its grad_points row is not written.  The reference's per-type expressions, grad_out = 2 * grad_dist.
+ * B*N and B*F must be below 2^31 - 1 (else DIBR_B200_ESIZE); workspace >= the size query (any alignment,
+ * else DIBR_B200_EWORKSPACE).  Neither call reads anything back to the host.
+ */
+int dibr_b200_point_mesh_distance_workspace_bytes(int batch, int num_points, int num_faces, int dtype,
+                                                  size_t* forward_bytes, size_t* backward_bytes);
+int dibr_b200_point_mesh_distance_forward(int batch, int num_points, int num_faces, int dtype, const void* points,
+                                          const void* face_vertices, void* dist, int64_t* face_idx, int32_t* dist_type,
+                                          void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_point_mesh_distance_backward(int batch, int num_points, int num_faces, int dtype, const void* grad_dist,
+                                           const void* points, const void* face_vertices, const int64_t* face_idx,
+                                           const int32_t* dist_type, void* grad_points, void* grad_face_vertices,
+                                           void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
  * Diffuse lighting (kaolin/render/lighting/sg.py, sh.py; kaolin_b200/csrc/lighting.cu).
  *
  * General reduced SG inner product, the operator kaolin::unbatched_reduced_sg_inner_product_

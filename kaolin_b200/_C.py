@@ -3,7 +3,8 @@ kaolin/csrc/bindings.cpp:111-115, with identical names, argument order/meaning,
 return structure and error behaviour, implemented by libdibr_b200.so; likewise
 ``_C.render.sg``, the DefTet pair, ``_C.ops.mesh.unbatched_mesh_intersection_cuda``
 (bindings.cpp:49), which the reference's ``check_sign.py`` calls, and
-``_C.ops.conversions.unbatched_mcube_forward_cuda``, which its ``voxelgrids_to_trianglemeshes`` calls.
+``_C.ops.conversions.unbatched_mcube_forward_cuda``, which its ``voxelgrids_to_trianglemeshes`` calls, and
+``_C.metrics.unbatched_triangle_distance_{forward,backward}_cuda``, which its ``point_to_mesh_distance`` calls.
 
 This is what makes the library a drop-in *below* the reference's own Python
 wrappers: ``kaolin.render.mesh.rasterization`` / ``.dibr`` run unmodified with
@@ -298,6 +299,75 @@ def unbatched_mcube_forward_cuda(voxelgrid, iso_value):
     from .ops.conversions.voxelgrid import unbatched_mcube_forward
     return unbatched_mcube_forward(voxelgrid, iso_value)
 
+
+def _check_triangle_distance(fn, named, sizes):
+    """CHECK_CUDA, then CHECK_CONTIGUOUS, then CHECK_SIZES (unbatched_triangle_distance.cpp), in its order."""
+    for name, t in named:
+        if not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor")
+    for name, t in named:
+        if not t.is_contiguous():
+            raise RuntimeError(f"{name} must be contiguous")
+    for name, t in named:
+        if tuple(t.shape) != tuple(sizes[name]):
+            raise RuntimeError(f"{name} must of size {{{', '.join(str(s) for s in sizes[name])}}}")
+    dev = named[0][1].device
+    for name, t in named:
+        if t.device != dev:
+            raise RuntimeError(f"{fn}: expected all tensors on one device; {name} is on {t.device}")
+
+
+def _check_types(fn, named):
+    for name, t, dtype in named:
+        if t.dtype != dtype:
+            raise RuntimeError(f"{fn}: expected {name} of type {dtype}, got {t.dtype}")
+
+
+def unbatched_triangle_distance_forward_cuda(points, face_vertices, dist, face_idx, dist_type):
+    """unbatched_triangle_distance.cpp:43-72: points (N, 3), face_vertices (F, 3, 3) -> written into
+    dist (N), face_idx (N) int64 and dist_type (N) int32; float32 or float64.  With F = 0 the outputs are
+    left as they are, as in the reference."""
+    from .metrics.trianglemesh import _dtype_flag, _pmd_forward
+    fn = "unbatched_triangle_distance_forward_cuda"
+    named = [("points", points), ("face_vertices", face_vertices), ("dist", dist), ("face_idx", face_idx),
+             ("dist_type", dist_type)]
+    N, F = points.shape[0], face_vertices.shape[0]
+    _check_triangle_distance(fn, named, {"points": (N, 3), "face_vertices": (F, 3, 3), "dist": (N,),
+                                         "face_idx": (N,), "dist_type": (N,)})
+    _dtype_flag(fn, points.dtype)
+    _check_types(fn, [("face_vertices", face_vertices, points.dtype), ("dist", dist, points.dtype),
+                      ("face_idx", face_idx, torch.int64), ("dist_type", dist_type, torch.int32)])
+    with torch.cuda.device(points.device):
+        _pmd_forward(points[None], face_vertices[None], dist, face_idx, dist_type)
+
+
+def unbatched_triangle_distance_backward_cuda(grad_dist, points, face_vertices, face_idx, dist_type, grad_points,
+                                              grad_face_vertices):
+    """unbatched_triangle_distance.cpp:74-114: grad_points (N, 3) written, grad_face_vertices (F, 3, 3)
+    added to, in ascending point order per face (no float atomics)."""
+    from .metrics.trianglemesh import _dtype_flag, _pmd_backward
+    fn = "unbatched_triangle_distance_backward_cuda"
+    named = [("grad_dist", grad_dist), ("points", points), ("face_vertices", face_vertices), ("face_idx", face_idx),
+             ("dist_type", dist_type), ("grad_points", grad_points), ("grad_face_vertices", grad_face_vertices)]
+    N, F = points.shape[0], face_vertices.shape[0]
+    _check_triangle_distance(fn, named, {"grad_dist": (N,), "points": (N, 3), "face_vertices": (F, 3, 3),
+                                         "face_idx": (N,), "dist_type": (N,), "grad_points": (N, 3),
+                                         "grad_face_vertices": (F, 3, 3)})
+    _dtype_flag(fn, points.dtype)
+    _check_types(fn, [("grad_dist", grad_dist, points.dtype), ("face_vertices", face_vertices, points.dtype),
+                      ("face_idx", face_idx, torch.int64), ("dist_type", dist_type, torch.int32),
+                      ("grad_points", grad_points, points.dtype),
+                      ("grad_face_vertices", grad_face_vertices, points.dtype)])
+    with torch.cuda.device(points.device):
+        _pmd_backward(grad_dist[None], points[None], face_vertices[None], face_idx, dist_type, grad_points,
+                      grad_face_vertices)
+
+
+# kaolin._C.metrics.<op>, as bindings.cpp lays it out
+metrics = types.SimpleNamespace(
+    unbatched_triangle_distance_forward_cuda=unbatched_triangle_distance_forward_cuda,
+    unbatched_triangle_distance_backward_cuda=unbatched_triangle_distance_backward_cuda,
+)
 
 # kaolin._C.ops.{mesh,conversions}.<op>, as bindings.cpp lays them out
 ops = types.SimpleNamespace(mesh=types.SimpleNamespace(

@@ -14,7 +14,8 @@ levels once), and DMTet's tet-grid operators (``ops.conversions.marching_tetrahe
 ``ops.mesh.subdivide_tetmesh``), and the point-in-mesh test (``ops.mesh.check_sign``,
 ``ops.mesh.CheckSign``, which builds the mesh once, and ``_C.ops.mesh.unbatched_mesh_intersection_cuda``),
 and marching cubes (``ops.conversions.voxelgrids_to_trianglemeshes``, every view in one call, and
-``_C.ops.conversions.unbatched_mcube_forward_cuda``);
+``_C.ops.conversions.unbatched_mcube_forward_cuda``), and the point-to-mesh distance
+(``metrics.trianglemesh.point_to_mesh_distance``, every view in one call, and ``_C.metrics``);
 see DESIGN.md for scope.  There is no CPU fallback: every entry point
 raises if the CUDA library (kaolin_b200/csrc, built in-tree) is missing or the
 tensors are not on a CUDA device.

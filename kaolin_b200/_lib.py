@@ -17,10 +17,12 @@ LIB_PATH = os.path.join(CSRC, "libdibr_b200.so")
 SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline.cu"),
            os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
            os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu"),
-           os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu")]
+           os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu"),
+           os.path.join(CSRC, "point_mesh_distance.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
            os.path.join(CSRC, "op_layouts.h"), os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
+           os.path.join(CSRC, "row_sort.cuh"),
            os.path.join(_HERE, "..", "include", "dibr_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -29,7 +31,7 @@ EINVAL, EWORKSPACE, ESIZE = -1, -3, -4
 RASTER, SOFT_MASK = 1, 2
 LIGHT_SG_INNER_PRODUCT, LIGHT_SG_FITTED, LIGHT_SH9 = 0, 1, 2     # dibr_b200_diffuse_* models
 BINS_VALID, ACCUMULATE = 1, 2      # dibr_b200_backward flags
-DTYPE_F32, DTYPE_F64 = 0, 1        # dibr_b200_check_sign_* and dibr_b200_mesh_intersection_count
+DTYPE_F32, DTYPE_F64 = 0, 1        # check_sign, mesh_intersection_count and point_mesh_distance
 DTYPE_U8 = 2                       # dibr_b200_marching_cubes_* (uint8 and bool grids)
 
 _lock = threading.Lock()
@@ -139,6 +141,10 @@ SIGNATURES = {
     "dibr_b200_marching_cubes_count": (_i, [_i] * 6 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dibr_b200_marching_cubes_emit": (_i, [_i] * 6 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _vp]),
     "dibr_b200_marching_cubes_backward": (_i, [_i] * 5 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _vp]),
+    # point-to-mesh distance (metrics.trianglemesh.point_to_mesh_distance, _C.metrics; csrc/point_mesh_distance.cu)
+    "dibr_b200_point_mesh_distance_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz), ctypes.POINTER(_sz)]),
+    "dibr_b200_point_mesh_distance_forward": (_i, [_i, _i, _i, _i] + [_vp] * 5 + [_vp, _sz, _vp]),
+    "dibr_b200_point_mesh_distance_backward": (_i, [_i, _i, _i, _i] + [_vp] * 7 + [_vp, _sz, _vp]),
 }
 
 
@@ -265,6 +271,15 @@ def check_sign_workspace_bytes(batch, num_faces, num_points, dtype, what):
     check(lib().dibr_b200_check_sign_workspace_bytes(batch, num_faces, num_points, dtype, ctypes.byref(build),
                                                      ctypes.byref(query)), what)
     return build.value, query.value
+
+
+def point_mesh_distance_workspace_bytes(batch, num_points, num_faces, dtype, what):
+    """(forward bytes, backward bytes) of ``dibr_b200_point_mesh_distance_workspace_bytes``; raises on its
+    status."""
+    fwd, bwd = _sz(0), _sz(0)
+    check(lib().dibr_b200_point_mesh_distance_workspace_bytes(batch, num_points, num_faces, dtype, ctypes.byref(fwd),
+                                                              ctypes.byref(bwd)), what)
+    return fwd.value, bwd.value
 
 
 def scratch(nbytes, device):

@@ -23,6 +23,7 @@
 #include <stdint.h>
 
 #include "../../include/dibr_b200.h"
+#include "row_sort.cuh"
 #include "scan.cuh"
 
 // launch tracing (dibr_b200_trace_begin / _end), kept in dibr_b200.cu
@@ -185,15 +186,6 @@ __global__ void __launch_bounds__(kThreads) topo_fill_kernel(Topo t) {
   }
 }
 
-__device__ __forceinline__ void insertion_sort(int* a, int n) {
-  for (int i = 1; i < n; ++i) {
-    const int x = a[i];
-    int j = i - 1;
-    while (j >= 0 && a[j] > x) { a[j + 1] = a[j]; --j; }
-    a[j + 1] = x;
-  }
-}
-
 __device__ __forceinline__ void finish_row(const Topo& t, int v, int unique) {
   t.degree[v] = unique;
   t.weight[v] = unique ? 1.0f / (float)unique : 0.0f;   // IEEE division: torch.div(A, num_neighbour)
@@ -223,27 +215,6 @@ __global__ void __launch_bounds__(kThreads) topo_sort_rows_kernel(Topo t) {
   for (int i = 0; i < t.R * n; ++i)
     if (i == 0 || nb[i] != nb[u - 1]) nb[u++] = nb[i];
   finish_row(t, v, u);
-}
-
-// Ascending bitonic network over a[0, n) in global memory, one CTA, any n: the "flip" form sorts
-// every block of size k ascending, so a missing partner (index >= n) stands for +inf and is skipped.
-__device__ void block_bitonic_sort(int* a, int64_t n) {
-  int64_t n2 = 1;
-  while (n2 < n) n2 <<= 1;
-  for (int64_t k = 2; k <= n2; k <<= 1) {
-    for (int64_t s = k >> 1; s > 0; s >>= 1) {
-      for (int64_t p = threadIdx.x; p < (n2 >> 1); p += blockDim.x) {
-        const int64_t blk = p / s, off = p - blk * s;
-        const int64_t i = blk * 2 * s + off;
-        const int64_t j = s == (k >> 1) ? blk * 2 * s + 2 * s - 1 - off : i + s;
-        if (j < n) {
-          const int x = a[i], y = a[j];
-          if (x > y) { a[i] = y; a[j] = x; }
-        }
-      }
-      __syncthreads();
-    }
-  }
 }
 
 __global__ void __launch_bounds__(kScanThreads) topo_sort_long_kernel(Topo t) {

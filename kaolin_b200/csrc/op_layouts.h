@@ -210,6 +210,44 @@ inline MarchingCubesLayout marching_cubes_layout(int64_t cubes) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// point_mesh_distance.cu, for B views of N points and F faces, T of tsize bytes.
+// Forward: one record of kFaceRecord T per (view, face) and one 64-bit search key per (view, point).
+// Backward: the nine face terms per (view, point), then the points grouped by (view, closest face):
+// counts [B*F], offsets [B*F + 1], the scan's tile sums, the point ids [B*N], the long-row list
+// [B*F] and its counter.
+constexpr int kFaceRecord = 33;   // v1, v2, v3, e12, e23, e31, three edge normals, unit normal, |e|^2 x 3
+
+struct PointMeshForwardLayout { Piece records, keys; size_t bytes; };
+
+inline PointMeshForwardLayout point_mesh_forward_layout(int B, int N, int F, size_t tsize) {
+  const size_t nf = (size_t)B * (size_t)(F > 0 ? F : 1), np = (size_t)B * (size_t)(N > 0 ? N : 1);
+  Placer p;
+  PointMeshForwardLayout L;
+  L.records = p.put(nf * kFaceRecord * tsize);
+  L.keys = p.put(np * sizeof(unsigned long long));
+  L.bytes = p.total();
+  return L;
+}
+
+struct PointMeshBackwardLayout { Piece terms, count, off, sums, ids, long_rows, long_count; size_t bytes; };
+
+inline PointMeshBackwardLayout point_mesh_backward_layout(int B, int N, int F, size_t tsize) {
+  const int64_t nf = (int64_t)B * F;
+  const size_t np = (size_t)B * (size_t)(N > 0 ? N : 1);
+  Placer p;
+  PointMeshBackwardLayout L;
+  L.terms = p.put(np * 9 * tsize);
+  L.count = p.put(sizeof(int) * (size_t)(nf > 0 ? nf : 1));
+  L.off = p.put(sizeof(int) * ((size_t)nf + 1));
+  L.sums = p.put(scan_sums_bytes(nf));
+  L.ids = p.put(np * sizeof(int));
+  L.long_rows = p.put(sizeof(int) * (size_t)(nf > 0 ? nf : 1));
+  L.long_count = p.put(sizeof(int));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
 // lighting.cu: the light gradients' partial sums, `floats` per light in each of `slots` CTA slots.
 struct LightingLayout { Piece partial; size_t bytes; };
 
