@@ -278,13 +278,19 @@ bin_faces_kernel(Scene s, int sets) {
     __syncthreads();
   }
   int64_t i = (int64_t)blockIdx.x * kBinThreads + tid;
-  const bool live = i < s.NF;
-  if (!live) i = s.NF - 1;
+  const bool in_range = i < s.NF;
+  if (!in_range) i = s.NF - 1;
   int b; int64_t fbase;
   face_view(s, i, b, fbase);
   const int f = (int)(i - fbase);
   float v[6];
   load_xy(s, i, v);
+  // A face with a NaN among its nine coordinates goes into neither set: it never wins a pixel and
+  // is never a soft-mask candidate, so every later step sees the scene without it (DESIGN.md, NaN
+  // vertices).  The min / max below drop a NaN, and the per-pixel tests pass one.
+  bool tainted = isnan(v[0]) || isnan(v[1]) || isnan(v[2]) || isnan(v[3]) || isnan(v[4]) || isnan(v[5]);
+  if (s.z) tainted = tainted || isnan(__ldg(s.z + 3 * i)) || isnan(__ldg(s.z + 3 * i + 1)) || isnan(__ldg(s.z + 3 * i + 2));
+  const bool live = in_range && !tainted;
   bool valid = live;
   if (s.fnz) valid = valid && __ldg(s.fnz + i) >= 0.f;
   if (s.valid) valid = valid && (__ldg(s.valid + i) != 0);
@@ -2543,7 +2549,7 @@ int dibr_b200_forward_f64(int batch, int num_faces, int height, int width, int f
   F64Args a;
   rc = f64_scene(a.s, batch, num_faces, height, width, multiplier_f, workspace, workspace_bytes_);
   if (rc) return rc;
-  rc = f64_bins(a.s, face_vertices_image, face_normals_z, valid_faces, multiplier, boxlen_m,
+  rc = f64_bins(a.s, face_vertices_image, face_vertices_z, face_normals_z, valid_faces, multiplier, boxlen_m,
                 (raster ? 1 : 0) | (soft ? 2 : 0), st);
   if (rc) return rc;
   a.D = feat_dim; a.K = knum; a.mode = mode; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier_f;
@@ -2580,7 +2586,7 @@ int dibr_b200_backward_f64(int batch, int num_faces, int height, int width, int 
   if (NF == 0 || (!run_raster && !grad_soft_mask)) return 0;
   // the soft-mask branch needs the enlarged bins: forward's (BINS_VALID) or rebuilt here
   if (grad_soft_mask && !(flags & DIBR_B200_BINS_VALID)) {
-    rc = f64_bins(a.s, face_vertices_image, nullptr, nullptr, multiplier, boxlen_m, 2, st);
+    rc = f64_bins(a.s, face_vertices_image, nullptr, nullptr, nullptr, multiplier, boxlen_m, 2, st);
     if (rc) return rc;
   }
   a.D = feat_dim; a.K = knum; a.mode = 0; a.eps = eps; a.sigmainv = sigmainv; a.multiplier = multiplier_f;

@@ -29,15 +29,19 @@ struct F64Args {
   double* g_xy; double* g_ff;
 };
 
-__global__ void __launch_bounds__(256) f64_prep_kernel(int64_t NF, const double* __restrict__ xy, const double* __restrict__ fnz,
+__global__ void __launch_bounds__(256) f64_prep_kernel(int64_t NF, const double* __restrict__ xy, const double* __restrict__ z,
+                                                       const double* __restrict__ fnz,
                                                        const uint8_t* __restrict__ valid_in, double m, double margin,
                                                        float* __restrict__ xyf, float* __restrict__ bt, float* __restrict__ bl,
                                                        uint8_t* __restrict__ valid) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= NF) return;
   double v[6];
+  // a NaN depth makes the face's float vertices NaN: the binning then drops it from both sets, as it
+  // drops a face with a NaN in face_vertices_image (bin_faces_kernel)
+  const bool nan_z = z && (isnan(z[i * 3]) || isnan(z[i * 3 + 1]) || isnan(z[i * 3 + 2]));
 #pragma unroll
-  for (int k = 0; k < 6; ++k) { v[k] = __dmul_rn(xy[i * 6 + k], m); xyf[i * 6 + k] = (float)v[k]; }
+  for (int k = 0; k < 6; ++k) { v[k] = __dmul_rn(xy[i * 6 + k], m); xyf[i * 6 + k] = nan_z ? NAN : (float)v[k]; }
   const double xmin = fmin(fmin(v[0], v[2]), v[4]), ymin = fmin(fmin(v[1], v[3]), v[5]);
   const double xmax = fmax(fmax(v[0], v[2]), v[4]), ymax = fmax(fmax(v[1], v[3]), v[5]);
   reinterpret_cast<float4*>(bt)[i] = make_float4(__double2float_rd(xmin), __double2float_rd(ymin),
@@ -198,12 +202,12 @@ int f64_scene(Scene& s, int B, int F, int H, int W, float multiplier, void* ws, 
 
 // Fills the float scene laid out by f64_scene from the double inputs, scaled by the double
 // multiplier `scale` (face_vertices_image * multiplier in torch, rasterization.py:320, dibr.py:32),
-// and bins it.
-int f64_bins(const Scene& s, const double* fvi, const double* fnz, const uint8_t* valid, double scale, double margin,
-             int sets, cudaStream_t st) {
+// and bins it.  `fvz` (nullable) only marks faces with a NaN depth, which are binned in no set.
+int f64_bins(const Scene& s, const double* fvi, const double* fvz, const double* fnz, const uint8_t* valid,
+             double scale, double margin, int sets, cudaStream_t st) {
   if (s.NF > 0)
     f64_prep_kernel<<<(unsigned)((s.NF + 255) / 256), 256, 0, st>>>(
-        s.NF, fvi, fnz, valid, scale, margin, const_cast<float*>(s.xy), const_cast<float*>(s.bbox_tight),
+        s.NF, fvi, fvz, fnz, valid, scale, margin, const_cast<float*>(s.xy), const_cast<float*>(s.bbox_tight),
         const_cast<float*>(s.bbox_large), const_cast<uint8_t*>(s.valid));
   return build_bins(s, sets, st);     // with no faces: zeroed counters, every pixel takes the empty path
 }

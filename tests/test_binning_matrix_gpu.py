@@ -43,7 +43,8 @@ gradients on its stored rows wherever the reference is within 1e-5 of the oracle
 than ORACLE_MAX_PIXELS pixels (one levels case) are held to the reference's gradients alone, at that
 bar: the C oracle walks every face for every pixel.  Reruns give byte-identical outputs.
 
-Known divergence, not tested: NaN vertices (DESIGN.md).
+NaN vertices, which make a face absent from every set, are held to the scene without them in
+test_nan_vertices_gpu.py.
 """
 import collections
 import functools

@@ -40,8 +40,9 @@ The bbox test is half-open, and a pixel centre is a float: a double xmax equal t
 itself, so the binning already drops that pixel and `x0 >= xmax` in the double test cannot be told from
 `x0 > xmax` by any input.
 
-Known divergence, not tested: NaN vertices.  fmin / fmax drop a NaN where torch.min propagates it,
-and the reference's result then depends on the order it visits faces in.
+NaN vertices make a face absent (f64_prep_kernel and the binning drop it), where the reference's result
+depends on the order it visits faces in; test_nan_vertices_gpu.py holds the float64 path to the scene
+without such faces.
 """
 import collections
 import functools
