@@ -266,6 +266,45 @@ __device__ __forceinline__ void bin_insert(const Scene& s, BinSmem& sm, int set,
   }
 }
 
+// Face i's multiplied xy, and in which sets it may go.  A face with a NaN among its nine
+// coordinates goes into neither set (live = false): it never wins a pixel and is never a soft-mask
+// candidate, so every later step sees the scene without it (DESIGN.md, NaN vertices).  The min / max
+// of face_set_span drop a NaN, and the per-pixel tests pass one.  valid: live and not culled.
+struct FaceState { float v[6]; bool live, valid; };
+
+__device__ __forceinline__ FaceState face_state(const Scene& s, int64_t i, bool in_range) {
+  FaceState fs;
+  float* v = fs.v;
+  load_xy(s, i, v);
+  bool tainted = isnan(v[0]) || isnan(v[1]) || isnan(v[2]) || isnan(v[3]) || isnan(v[4]) || isnan(v[5]);
+  if (s.z) tainted = tainted || isnan(__ldg(s.z + 3 * i)) || isnan(__ldg(s.z + 3 * i + 1)) || isnan(__ldg(s.z + 3 * i + 2));
+  fs.live = in_range && !tainted;
+  fs.valid = fs.live;
+  if (s.fnz) fs.valid = fs.valid && __ldg(s.fnz + i) >= 0.f;
+  if (s.valid) fs.valid = fs.valid && (__ldg(s.valid + i) != 0);
+  return fs;
+}
+
+// The pixel rectangle r and bin span sp of face i in set 0 (tight) or 1 (enlarged).
+__device__ __forceinline__ void face_set_span(const Scene& s, int64_t i, int set, const FaceState& fs, PixRect& r,
+                                              BinSpan& sp) {
+  const float* v = fs.v;
+  float xmin, ymin, xmax, ymax;
+  const float* given = set ? s.bbox_large : s.bbox_tight;
+  if (given) {
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(given) + i);
+    xmin = bb.x; ymin = bb.y; xmax = bb.z; ymax = bb.w;
+  } else {
+    // tight: torch.min / torch.max over the 3 vertices (rasterization.py:325-327);
+    // large: [min - boxlen*m, max + boxlen*m] in fp32 (dibr.py:33-39)
+    xmin = fminf(fminf(v[0], v[2]), v[4]); ymin = fminf(fminf(v[1], v[3]), v[5]);
+    xmax = fmaxf(fmaxf(v[0], v[2]), v[4]); ymax = fmaxf(fmaxf(v[1], v[3]), v[5]);
+    if (set) { xmin = fsub(xmin, s.margin); ymin = fsub(ymin, s.margin); xmax = fadd(xmax, s.margin); ymax = fadd(ymax, s.margin); }
+  }
+  r = bbox_to_rect(s.grid, xmin, ymin, xmax, ymax);
+  sp = bin_span(s, r, set ? fs.live : fs.valid);
+}
+
 // AGG = false (sparse meshes, a few faces per tile): plain atomics, no table.
 template <bool FILL, bool AGG>
 __global__ void __launch_bounds__(AGG ? kBinThreadsAgg : kBinThreadsPlain, AGG ? 2 : 4)
@@ -283,17 +322,8 @@ bin_faces_kernel(Scene s, int sets) {
   int b; int64_t fbase;
   face_view(s, i, b, fbase);
   const int f = (int)(i - fbase);
-  float v[6];
-  load_xy(s, i, v);
-  // A face with a NaN among its nine coordinates goes into neither set: it never wins a pixel and
-  // is never a soft-mask candidate, so every later step sees the scene without it (DESIGN.md, NaN
-  // vertices).  The min / max below drop a NaN, and the per-pixel tests pass one.
-  bool tainted = isnan(v[0]) || isnan(v[1]) || isnan(v[2]) || isnan(v[3]) || isnan(v[4]) || isnan(v[5]);
-  if (s.z) tainted = tainted || isnan(__ldg(s.z + 3 * i)) || isnan(__ldg(s.z + 3 * i + 1)) || isnan(__ldg(s.z + 3 * i + 2));
-  const bool live = in_range && !tainted;
-  bool valid = live;
-  if (s.fnz) valid = valid && __ldg(s.fnz + i) >= 0.f;
-  if (s.valid) valid = valid && (__ldg(s.valid + i) != 0);
+  const FaceState fs = face_state(s, i, in_range);
+  const bool live = fs.live;
   PixRect r[2];
   BinSpan sp[2];
   int where[2][4];
@@ -301,20 +331,7 @@ bin_faces_kernel(Scene s, int sets) {
   for (int set = 0; set < 2; ++set) {
     sp[set].has = false;
     if (!((sets >> set) & 1)) continue;
-    float xmin, ymin, xmax, ymax;
-    const float* given = set ? s.bbox_large : s.bbox_tight;
-    if (given) {
-      const float4 bb = __ldg(reinterpret_cast<const float4*>(given) + i);
-      xmin = bb.x; ymin = bb.y; xmax = bb.z; ymax = bb.w;
-    } else {
-      // tight: torch.min / torch.max over the 3 vertices (rasterization.py:325-327);
-      // large: [min - boxlen*m, max + boxlen*m] in fp32 (dibr.py:33-39)
-      xmin = fminf(fminf(v[0], v[2]), v[4]); ymin = fminf(fminf(v[1], v[3]), v[5]);
-      xmax = fmaxf(fmaxf(v[0], v[2]), v[4]); ymax = fmaxf(fmaxf(v[1], v[3]), v[5]);
-      if (set) { xmin = fsub(xmin, s.margin); ymin = fsub(ymin, s.margin); xmax = fadd(xmax, s.margin); ymax = fadd(ymax, s.margin); }
-    }
-    r[set] = bbox_to_rect(s.grid, xmin, ymin, xmax, ymax);
-    sp[set] = bin_span(s, r[set], set ? live : valid);
+    face_set_span(s, i, set, fs, r[set], sp[set]);
     bool aggregated = false;
     if constexpr (AGG) {
       const bool small = sp[set].bx1 - sp[set].bx0 <= 1 && sp[set].by1 - sp[set].by0 <= 1;
@@ -384,6 +401,154 @@ bin_faces_kernel(Scene s, int sets) {
         if (sp[set].has && w >= 0) dst[sm.vals[w >> 16] + (w & 0xffff)] = e;
       }
     }
+  }
+}
+
+// Count pass in view-owned chunks (sparse meshes whose view's counters fit in shared memory): CTA
+// (c, b) counts faces [c * chunk, (c + 1) * chunk) of view b into a shared copy of the view's bin
+// counters and soft-mask tile bitmask words, then flushes one reduction per non-zero counter and word.
+// The hot counters of a screen patch thus see one global reduction per CTA instead of one atomic per
+// face.
+// Shared memory: the requested sets' counters [nsets][NB], then (with the enlarged set) the view's
+// nty * ceil(ntx / 32) bitmask words and its view_flag word.
+constexpr int kBinChunkThreads = 256;
+constexpr int kBinChunkMaxPerThread = 8;            // faces per thread, at most
+constexpr int kBinChunkTargetCtas = 2 * 132;        // two CTAs per SM of an H100 SXM
+constexpr size_t kBinChunkSmemBudget = 48 * 1024;   // no opt-in: several CTAs per SM
+
+__host__ __device__ inline int bin_chunk_words(const Scene& s, int sets) {
+  const int nsets = (sets & 1) + ((sets >> 1) & 1);
+  const int bitmask = (sets & 2) ? s.nty[0] * ((s.ntx[0] + 31) >> 5) + 1 : 0;
+  return nsets * s.NB + bitmask;
+}
+
+__global__ void __launch_bounds__(kBinChunkThreads) bin_count_chunk_kernel(Scene s, int sets, int chunk) {
+  extern __shared__ int bin_sm[];
+  const int tid = threadIdx.x;
+  const int b = blockIdx.y;
+  const int64_t fbase = (int64_t)b * s.F;
+  const int f0 = blockIdx.x * chunk, f1 = min(f0 + chunk, s.F);
+  const int nw = (s.ntx[0] + 31) >> 5;
+  const int nwords = (sets & 2) ? s.nty[0] * nw : 0;
+  const int total = bin_chunk_words(s, sets);
+  int* const words = bin_sm + total - (nwords + 1);       // with the enlarged set only
+  for (int t = tid; t < total; t += kBinChunkThreads) bin_sm[t] = 0;
+  __syncthreads();
+  // the shared counter of (set, bin): the sets are packed, so a single set sits at 0
+  auto counter = [&](int set, const BinSpan& sp, int bx, int by) -> int* {
+    return bin_sm + (sets == 3 ? set * s.NB : 0) + s.bin_base[sp.l] + by * s.ntx[sp.l] + bx;
+  };
+  for (int f = f0 + tid; f < f1; f += kBinChunkThreads) {
+    // both sets' spans before the first shared atomic: interleaving them with the atomics measured
+    // 0.14 ms instead of 0.057 ms at c4_shard (H100 80GB HBM3, 700 W)
+    const int64_t i = fbase + f;
+    const FaceState fs = face_state(s, i, true);
+    PixRect r[2];
+    BinSpan sp[2];
+#pragma unroll
+    for (int set = 0; set < 2; ++set) {
+      sp[set].has = false;
+      if ((sets >> set) & 1) face_set_span(s, i, set, fs, r[set], sp[set]);
+    }
+#pragma unroll
+    for (int set = 0; set < 2; ++set)
+      if (sp[set].has)
+        for (int by = sp[set].by0; by <= sp[set].by1; ++by)
+          for (int bx = sp[set].bx0; bx <= sp[set].bx1; ++bx) atomicAdd(counter(set, sp[set], bx, by), 1);
+    if (nwords && fs.live && r[1].x_hi > r[1].x_lo && r[1].y_hi > r[1].y_lo) {
+      // the rule of bin_faces_kernel: one bit per 16x16 tile under the enlarged rectangle, or the
+      // view's flag when it covers more than 64 (tile row, word) cells
+      const int tx0 = r[1].x_lo >> 4, tx1 = (r[1].x_hi - 1) >> 4, ty0 = r[1].y_lo >> 4, ty1 = (r[1].y_hi - 1) >> 4;
+      const int w0 = tx0 >> 5, w1 = tx1 >> 5;
+      if ((ty1 - ty0 + 1) * (w1 - w0 + 1) <= 64) {
+        for (int w = w0; w <= w1; ++w) {
+          const int lo = max(tx0 - (w << 5), 0), hi = min(tx1 - (w << 5), 31);
+          const int m = (int)((0xffffffffu >> (31 - hi)) & (0xffffffffu << lo));
+          for (int ty = ty0; ty <= ty1; ++ty)
+            if ((words[ty * nw + w] & m) != m) atomicOr(&words[ty * nw + w], m);
+        }
+      } else {
+        words[nwords] = 1;
+      }
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int set = 0; set < 2; ++set) {
+    if (!((sets >> set) & 1)) continue;
+    const int* c = bin_sm + (sets == 3 ? set * s.NB : 0);
+    int* g = s.cnt + ((size_t)set * s.B + b) * s.NB;
+    for (int t = tid; t < s.NB; t += kBinChunkThreads)
+      if (c[t]) atomicAdd(g + t, c[t]);
+  }
+  if (nwords) {
+    int* g = s.tile_cnt + (size_t)b * s.nty[0] * nw;
+    for (int t = tid; t < nwords; t += kBinChunkThreads)
+      if (words[t]) atomicOr(g + t, words[t]);
+    if (tid == 0 && words[nwords]) atomicOr(s.view_flag + b, 1);
+  }
+}
+
+// Fill pass for the shapes of bin_count_chunk_kernel: CTA (c, b) places faces [256 c, 256 c + 256) of
+// view b, one per thread.  Each face takes its rank in each of its bins from a returning shared
+// atomic on the view's counters (kept in registers: <= 4 per set); after a barrier one returning
+// global atomic per non-zero counter claims the CTA's range of the bin, and each face writes its entry
+// at off + claimed + rank.  One face per thread keeps thousands of CTAs in flight, which hides the
+// latency of the claim; the entries of a bin still land in one contiguous run per CTA.  (A fill in
+// the count pass's chunks of up to 2048 faces, which counted again and then handed out slots in a
+// second walk over its faces, measured slower than plain atomics on an H100 80GB HBM3 at 700 W:
+// 0.20 vs 0.16 ms at c4_shard; this kernel measured 0.096 ms there, 0.16 vs 0.23 ms at c3.)
+__global__ void __launch_bounds__(kBinChunkThreads) bin_fill_chunk_kernel(Scene s, int sets) {
+  extern __shared__ int bin_sm[];
+  const int tid = threadIdx.x;
+  const int b = blockIdx.y;
+  const int64_t fbase = (int64_t)b * s.F;
+  const int f = blockIdx.x * kBinChunkThreads + tid;
+  const int ncnt = ((sets & 1) + ((sets >> 1) & 1)) * s.NB;
+  for (int t = tid; t < ncnt; t += kBinChunkThreads) bin_sm[t] = 0;
+  const int64_t i = fbase + min(f, s.F - 1);
+  const FaceState fs = face_state(s, i, f < s.F);
+  PixRect r[2];
+  BinSpan sp[2];
+#pragma unroll
+  for (int set = 0; set < 2; ++set) {
+    sp[set].has = false;
+    if ((sets >> set) & 1) face_set_span(s, i, set, fs, r[set], sp[set]);
+  }
+  __syncthreads();
+  // a span has at most 2x2 bins: the coarsest level's one bin holds the whole image
+  int* c[2][4];
+  int rank[2][4];
+#pragma unroll
+  for (int set = 0; set < 2; ++set)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int bx = sp[set].bx0 + (k & 1), by = sp[set].by0 + (k >> 1);
+      c[set][k] = nullptr;
+      if (sp[set].has && bx <= sp[set].bx1 && by <= sp[set].by1) {
+        c[set][k] = bin_sm + (sets == 3 ? set * s.NB : 0) + s.bin_base[sp[set].l] + by * s.ntx[sp[set].l] + bx;
+        rank[set][k] = atomicAdd(c[set][k], 1);
+      }
+    }
+  __syncthreads();
+#pragma unroll
+  for (int set = 0; set < 2; ++set) {
+    if (!((sets >> set) & 1)) continue;
+    int* cs = bin_sm + (sets == 3 ? set * s.NB : 0);
+    const size_t g = ((size_t)set * s.B + b) * s.NB;
+    for (int t = tid; t < s.NB; t += kBinChunkThreads) {
+      const int n = cs[t];
+      if (n) cs[t] = __ldg(s.off + g + t) + atomicAdd(s.cnt + g + t, n);
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int set = 0; set < 2; ++set) {
+    const int4 e = make_int4(f, r[set].x_lo | (r[set].x_hi << 16), r[set].y_lo | (r[set].y_hi << 16), 0);
+    int4* dst = s.entries + (size_t)set * 4 * s.NF + 4 * fbase;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (c[set][k]) dst[*c[set][k] + rank[set][k]] = e;
   }
 }
 
@@ -2296,14 +2461,29 @@ int build_bins(const Scene& s, int sets, cudaStream_t st) {
   cudaError_t e = cudaMemsetAsync(s.cnt, 0, counters.bytes, st);
   if (e != cudaSuccess) return (int)e;
   if (s.NF > 0) {
+    // dense meshes (tens of faces per 16x16 tile) hammer a few counters: aggregate per CTA.  Sparse
+    // meshes of equal-sized views whose counters (and bitmask words) fit kBinChunkSmemBudget count and
+    // fill in view-owned chunks (c2, c3, c4_shard); the others (large images, packed batches, whose
+    // view sizes the host does not know) take plain atomics.
     const bool agg = s.NF / s.B >= (int64_t)32 * s.ntx[0] * s.nty[0];
+    const size_t chunk_smem = (size_t)bin_chunk_words(s, sets) * sizeof(int);
+    const bool chunked = !agg && !s.first && chunk_smem <= kBinChunkSmemBudget;
     const int threads = agg ? kBinThreadsAgg : kBinThreadsPlain;
     const unsigned blocks = (unsigned)((s.NF + threads - 1) / threads);
-    // dense meshes (tens of faces per 16x16 tile) hammer a few counters: aggregate per CTA
     {
       Span sp("bin_faces_kernel<count>", st);
-      if (agg) bin_faces_kernel<false, true><<<blocks, threads, 0, st>>>(s, sets);
-      else bin_faces_kernel<false, false><<<blocks, threads, 0, st>>>(s, sets);
+      if (chunked) {
+        // chunks of 256..2048 faces (1..8 per thread), as large as still gives kBinChunkTargetCtas CTAs
+        int64_t per_thread = s.NF / ((int64_t)kBinChunkTargetCtas * kBinChunkThreads);
+        per_thread = per_thread < 1 ? 1 : per_thread > kBinChunkMaxPerThread ? kBinChunkMaxPerThread : per_thread;
+        const int chunk = kBinChunkThreads * (int)per_thread;
+        const dim3 grid((unsigned)((s.F + chunk - 1) / chunk), (unsigned)s.B);
+        bin_count_chunk_kernel<<<grid, kBinChunkThreads, chunk_smem, st>>>(s, sets, chunk);
+      } else if (agg) {
+        bin_faces_kernel<false, true><<<blocks, threads, 0, st>>>(s, sets);
+      } else {
+        bin_faces_kernel<false, false><<<blocks, threads, 0, st>>>(s, sets);
+      }
     }
     {
       Span sp("scan_bins_kernel", st);
@@ -2311,7 +2491,11 @@ int build_bins(const Scene& s, int sets, cudaStream_t st) {
     }
     {
       Span sp("bin_faces_kernel<fill>", st);
-      if (agg) bin_faces_kernel<true, true><<<blocks, threads, 0, st>>>(s, sets);
+      if (chunked) {
+        const dim3 grid((unsigned)((s.F + kBinChunkThreads - 1) / kBinChunkThreads), (unsigned)s.B);
+        const size_t fill_smem = (size_t)((sets & 1) + ((sets >> 1) & 1)) * s.NB * sizeof(int);
+        bin_fill_chunk_kernel<<<grid, kBinChunkThreads, fill_smem, st>>>(s, sets);
+      } else if (agg) bin_faces_kernel<true, true><<<blocks, threads, 0, st>>>(s, sets);
       else bin_faces_kernel<true, false><<<blocks, threads, 0, st>>>(s, sets);
     }
   }
