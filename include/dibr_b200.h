@@ -788,6 +788,41 @@ int dibr_b200_marching_cubes_backward(int batch, int X, int Y, int Z, int pad, c
                                       float* grad_grid, dibr_b200_stream_t stream);
 
 /*
+ * Voxelization (kaolin/ops/conversions/pointcloud.py:22-141, _base_points_to_voxelgrids; and
+ * kaolin/ops/conversions/trianglemesh.py:29-110 with _unbatched_subdivide_vertices,
+ * kaolin/ops/mesh/trianglemesh.py:340-458) of normalised points (batch, num_points, 3) of `dtype`
+ * (DIBR_B200_DTYPE_F32 or _F64), contiguous, into a (batch, res, res, res) occupancy grid; with
+ * faces (num_faces, 3) int64 (shared by every view, indexing the points) the midpoints of the
+ * reference's subdivision of every face are marked too.  csrc/voxelize.cu gives the rounding rules.
+ *   dibr_b200_voxelize_mark: clears the workspace's bit grid and marks every point and midpoint.
+ *     Writes info[4] int64: {flags, first (view * num_faces + face) with an index outside
+ *     [0, num_points) or -1, first such face needing more than DIBR_B200_VOXELIZE_MAX_DEPTH levels of
+ *     subdivision or -1, and with `sparse` the number of set voxels}.  flags is an OR of
+ *     DIBR_B200_VOXELIZE_BAD_INDEX and _TOO_DEEP; when it is not 0 the grid is incomplete.  Faces
+ *     that are not indexed correctly are skipped, never read outside `points`.
+ *   dibr_b200_voxelize_dense: the grid (batch, res, res, res) of `dtype`, 0 or 1, to `out` (16-byte
+ *     aligned).
+ *   dibr_b200_voxelize_sparse (after a mark with `sparse`): out_indices (4, nnz) int64, the (view, x,
+ *     y, z) of every set voxel in grid order, nnz as info[3] gave it (at most 2^31 - 1).
+ * All three carve the same workspace (>= dibr_b200_voxelize_workspace_bytes, any alignment, else
+ * DIBR_B200_EWORKSPACE): res^3 / 8 bytes per view of bit grid, 8 bytes per (view, face) and 8 bytes
+ * per 32768 voxels.  batch * num_faces and batch * res^3 / 1024 must be below 2^31 - 1, res at most
+ * 2^20 (else DIBR_B200_ESIZE); negative sizes, res < 1, a bad dtype or a NULL buffer that is used give
+ * DIBR_B200_EINVAL.  No call reads anything back to the host.
+ */
+#define DIBR_B200_VOXELIZE_MAX_DEPTH 24   /* levels of subdivision below a face */
+#define DIBR_B200_VOXELIZE_BAD_INDEX 1
+#define DIBR_B200_VOXELIZE_TOO_DEEP 2
+int dibr_b200_voxelize_workspace_bytes(int batch, int64_t num_faces, int resolution, size_t* workspace_bytes);
+int dibr_b200_voxelize_mark(int batch, int64_t num_points, int64_t num_faces, int resolution, int dtype,
+                            const void* points, const int64_t* faces, int sparse, int64_t* info, void* workspace,
+                            size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_voxelize_dense(int batch, int64_t num_faces, int resolution, int dtype, void* out, void* workspace,
+                             size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_voxelize_sparse(int batch, int64_t num_faces, int resolution, int64_t nnz, int64_t* out_indices,
+                              void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
  * subdivide_tetmesh (kaolin/ops/mesh/tetmesh.py:85-181) on the tet topology: vertices (B, V, 3) and
  * features (B, V, channels) or NULL -> out_vertices (B, V + E, 3), out_features: rows < V copied, row
  * V + e the midpoint (y_a + y_b) * 0.5 of edge e; out_tets (8T, 4) int64 or NULL: child k of tet t at

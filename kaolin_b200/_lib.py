@@ -18,7 +18,7 @@ SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline
            os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
            os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu"),
            os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu"),
-           os.path.join(CSRC, "point_mesh_distance.cu")]
+           os.path.join(CSRC, "point_mesh_distance.cu"), os.path.join(CSRC, "voxelize.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
            os.path.join(CSRC, "op_layouts.h"), os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
@@ -145,6 +145,11 @@ SIGNATURES = {
     "dibr_b200_point_mesh_distance_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz), ctypes.POINTER(_sz)]),
     "dibr_b200_point_mesh_distance_forward": (_i, [_i, _i, _i, _i] + [_vp] * 5 + [_vp, _sz, _vp]),
     "dibr_b200_point_mesh_distance_backward": (_i, [_i, _i, _i, _i] + [_vp] * 7 + [_vp, _sz, _vp]),
+    # voxelization (ops.conversions.trianglemeshes_to_voxelgrids, pointclouds_to_voxelgrids; csrc/voxelize.cu)
+    "dibr_b200_voxelize_workspace_bytes": (_i, [_i, _i64, _i, ctypes.POINTER(_sz)]),
+    "dibr_b200_voxelize_mark": (_i, [_i, _i64, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _sz, _vp]),
+    "dibr_b200_voxelize_dense": (_i, [_i, _i64, _i, _i, _vp, _vp, _sz, _vp]),
+    "dibr_b200_voxelize_sparse": (_i, [_i, _i64, _i, _i64, _vp, _vp, _sz, _vp]),
 }
 
 
@@ -280,6 +285,13 @@ def point_mesh_distance_workspace_bytes(batch, num_points, num_faces, dtype, wha
     check(lib().dibr_b200_point_mesh_distance_workspace_bytes(batch, num_points, num_faces, dtype, ctypes.byref(fwd),
                                                               ctypes.byref(bwd)), what)
     return fwd.value, bwd.value
+
+
+def voxelize_workspace_bytes(batch, num_faces, resolution, what):
+    """The workspace bytes of the ``dibr_b200_voxelize_*`` calls; raises on its status."""
+    out = _sz(0)
+    check(lib().dibr_b200_voxelize_workspace_bytes(batch, num_faces, resolution, ctypes.byref(out)), what)
+    return out.value
 
 
 def scratch(nbytes, device):

@@ -248,6 +248,25 @@ inline PointMeshBackwardLayout point_mesh_backward_layout(int B, int N, int F, s
 }
 
 // ---------------------------------------------------------------------------------------------
+// voxelize.cu: the bit grid of `nwords` 32-bit words, the work items of `faces` (view, face) pairs and
+// their exclusive scan, the set bits of each chunk of 32 words and their exclusive scan, and the tile
+// sums of whichever scan is longer (the two run one after the other).
+struct VoxelizeLayout { Piece bits, counts, scan, chunk_counts, chunk_scan, sums; size_t bytes; };
+
+inline VoxelizeLayout voxelize_layout(int64_t nwords, int64_t faces, int64_t nchunks) {
+  Placer p;
+  VoxelizeLayout L;
+  L.bits = p.put(sizeof(uint32_t) * (size_t)nwords);
+  L.counts = p.put(sizeof(int) * (size_t)faces);
+  L.scan = p.put(sizeof(int) * ((size_t)faces + 1));
+  L.chunk_counts = p.put(sizeof(int) * (size_t)nchunks);
+  L.chunk_scan = p.put(sizeof(int) * ((size_t)nchunks + 1));
+  L.sums = p.put(scan_sums_bytes(faces > nchunks ? faces : nchunks));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
 // lighting.cu: the light gradients' partial sums, `floats` per light in each of `slots` CTA slots.
 struct LightingLayout { Piece partial; size_t bytes; };
 
