@@ -823,6 +823,59 @@ int dibr_b200_voxelize_sparse(int batch, int64_t num_faces, int resolution, int6
                               void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
 
 /*
+ * Face areas and surface sampling (kaolin/ops/mesh/trianglemesh.py:30-311; kaolin_b200/csrc/sample_points.cu,
+ * which states the random stream and the rounding).  `batch` views of `dtype` (DIBR_B200_DTYPE_F32 or
+ * _F64) share one face array of total_faces faces: view b owns faces g in [face_off[b], face_off[b + 1])
+ * (face_off [batch + 1] int64, device, non-decreasing from 0 to total_faces), reads face row
+ * g - b * fstride of faces (rows, 3) int64 and vertex b * vstride + index of vertices (rows, 3); an
+ * index must lie in [0, num_vertices).  Dense (batch, V, 3) with shared faces (F, 3): fstride = F,
+ * vstride = V; packed vertices with merged faces: fstride = vstride = 0.
+ *   dibr_b200_face_areas_forward: areas [total_faces] of `dtype`; *status = 0 or
+ *     DIBR_B200_SAMPLE_BAD_INDEX (such a face's area is NaN, nothing is read outside `vertices`).
+ *   dibr_b200_face_areas_backward: grad_areas [total_faces] -> grad_vertices, WRITTEN: (batch, V, 3)
+ *     when vstride, else (num_vertices, 3), summed over the corner CSR of the faces' topology
+ *     (dibr_b200_mesh_topology_build of the shared or merged faces).
+ *   dibr_b200_sample_points_forward: num_samples per view -> points (batch, N, 3), face_choices
+ *     (batch, N) int64 (g - b * fstride) and, with face_features (batch * F, 3, D) (dense only),
+ *     features (batch, N, D).  The distribution is the faces' areas, or `areas` [total_faces] float64
+ *     when it is not NULL; key is one int64 on the device.  *status is an OR of
+ *     DIBR_B200_SAMPLE_BAD_INDEX and _BAD_DISTRIBUTION (an area negative, NaN or infinite, a total that
+ *     is 0 or infinite, or an empty view); such a view's samples get face -1 and NaN points and
+ *     features.
+ *   dibr_b200_sample_points_backward: the same views, key and face_choices; grad_points (batch, N, 3)
+ *     -> grad_vertices (as face_areas_backward), and grad_features (batch, N, D) -> grad_face_features
+ *     (batch * F, 3, D), each WRITTEN when not NULL.  Samples of face -1 add nothing.  No float atomics.
+ * The workspace (any alignment, else DIBR_B200_EWORKSPACE) is the forward's or the backward's size
+ * (face_areas_backward: the backward's with num_samples 0).  3 * total_faces and batch * num_samples
+ * must be below 2^31 - 1 (else DIBR_B200_ESIZE); negative sizes, a bad dtype or a NULL buffer that is
+ * used give DIBR_B200_EINVAL.  No call reads anything back to the host.
+ */
+#define DIBR_B200_SAMPLE_BAD_INDEX 1
+#define DIBR_B200_SAMPLE_BAD_DISTRIBUTION 2
+int dibr_b200_sample_points_workspace_bytes(int batch, int64_t total_faces, int num_samples, int dtype,
+                                            size_t* forward_bytes, size_t* backward_bytes);
+int dibr_b200_face_areas_forward(int batch, int64_t total_faces, int num_vertices, int64_t fstride, int64_t vstride,
+                                 int dtype, const int64_t* face_off, const int64_t* faces, const void* vertices,
+                                 void* areas, int32_t* status, dibr_b200_stream_t stream);
+int dibr_b200_face_areas_backward(int batch, int64_t total_faces, int num_vertices, int64_t fstride, int64_t vstride,
+                                  int dtype, const int64_t* face_off, const int64_t* faces, const void* vertices,
+                                  const void* grad_areas, const int32_t* corner_ptr, const int32_t* corners,
+                                  void* grad_vertices, void* workspace, size_t workspace_bytes,
+                                  dibr_b200_stream_t stream);
+int dibr_b200_sample_points_forward(int batch, int64_t total_faces, int num_vertices, int64_t fstride, int64_t vstride,
+                                    int dtype, int num_samples, int feature_dim, const int64_t* face_off,
+                                    const int64_t* faces, const void* vertices, const double* areas,
+                                    const void* face_features, const int64_t* key, void* points,
+                                    int64_t* face_choices, void* features, int32_t* status, void* workspace,
+                                    size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_sample_points_backward(int batch, int64_t total_faces, int num_vertices, int64_t fstride,
+                                     int64_t vstride, int dtype, int num_samples, int feature_dim,
+                                     const int64_t* face_off, const int64_t* key, const int64_t* face_choices,
+                                     const void* grad_points, const void* grad_features, const int32_t* corner_ptr,
+                                     const int32_t* corners, void* grad_vertices, void* grad_face_features,
+                                     void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
  * subdivide_tetmesh (kaolin/ops/mesh/tetmesh.py:85-181) on the tet topology: vertices (B, V, 3) and
  * features (B, V, channels) or NULL -> out_vertices (B, V + E, 3), out_features: rows < V copied, row
  * V + e the midpoint (y_a + y_b) * 0.5 of edge e; out_tets (8T, 4) int64 or NULL: child k of tet t at

@@ -18,7 +18,8 @@ SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline
            os.path.join(CSRC, "deftet.cu"), os.path.join(CSRC, "peer_push.cu"),
            os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu"),
            os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu"),
-           os.path.join(CSRC, "point_mesh_distance.cu"), os.path.join(CSRC, "voxelize.cu")]
+           os.path.join(CSRC, "point_mesh_distance.cu"), os.path.join(CSRC, "voxelize.cu"),
+           os.path.join(CSRC, "sample_points.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
            os.path.join(CSRC, "op_layouts.h"), os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
@@ -150,6 +151,12 @@ SIGNATURES = {
     "dibr_b200_voxelize_mark": (_i, [_i, _i64, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _sz, _vp]),
     "dibr_b200_voxelize_dense": (_i, [_i, _i64, _i, _i, _vp, _vp, _sz, _vp]),
     "dibr_b200_voxelize_sparse": (_i, [_i, _i64, _i, _i64, _vp, _vp, _sz, _vp]),
+    # face areas and surface sampling (ops.mesh.face_areas, sample_points, SurfaceSampler; csrc/sample_points.cu)
+    "dibr_b200_sample_points_workspace_bytes": (_i, [_i, _i64, _i, _i, ctypes.POINTER(_sz), ctypes.POINTER(_sz)]),
+    "dibr_b200_face_areas_forward": (_i, [_i, _i64, _i, _i64, _i64, _i] + [_vp] * 5 + [_vp]),
+    "dibr_b200_face_areas_backward": (_i, [_i, _i64, _i, _i64, _i64, _i] + [_vp] * 8 + [_sz, _vp]),
+    "dibr_b200_sample_points_forward": (_i, [_i, _i64, _i, _i64, _i64, _i, _i, _i] + [_vp] * 11 + [_sz, _vp]),
+    "dibr_b200_sample_points_backward": (_i, [_i, _i64, _i, _i64, _i64, _i, _i, _i] + [_vp] * 10 + [_sz, _vp]),
 }
 
 
@@ -292,6 +299,14 @@ def voxelize_workspace_bytes(batch, num_faces, resolution, what):
     out = _sz(0)
     check(lib().dibr_b200_voxelize_workspace_bytes(batch, num_faces, resolution, ctypes.byref(out)), what)
     return out.value
+
+
+def sample_points_workspace_bytes(batch, total_faces, num_samples, dtype, what):
+    """(forward bytes, backward bytes) of ``dibr_b200_sample_points_workspace_bytes``; raises on its status."""
+    fwd, bwd = _sz(0), _sz(0)
+    check(lib().dibr_b200_sample_points_workspace_bytes(batch, total_faces, num_samples, dtype, ctypes.byref(fwd),
+                                                        ctypes.byref(bwd)), what)
+    return fwd.value, bwd.value
 
 
 def scratch(nbytes, device):

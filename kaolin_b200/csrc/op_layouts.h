@@ -267,6 +267,51 @@ inline VoxelizeLayout voxelize_layout(int64_t nwords, int64_t faces, int64_t nch
 }
 
 // ---------------------------------------------------------------------------------------------
+// sample_points.cu, for B views of nf faces in all (packed or B x F), N samples per view, T of tsize
+// bytes.  Forward: the float64 areas scanned in place into each view's CDF [nf], and per tile of
+// kCdfTile faces the CDF at its last face (the coarse table), the tile's segmented sum and whether a
+// view starts in it, and the carry from earlier tiles; one invalid-distribution flag per view.
+// Backward: the per-corner vertex gradients [nf][3][3] T, then the samples grouped by face: counts
+// [nf], offsets [nf + 1], the scan's tile sums, the sample ids [B*N], the long-row list [nf] and its
+// counter.  face_areas' backward uses the corner gradients only.
+constexpr int kCdfTile = 4096;
+
+inline int64_t cdf_tiles(int64_t nf) { return (nf + kCdfTile - 1) / kCdfTile; }
+
+struct SamplePointsForwardLayout { Piece cdf, coarse, tile_sum, tile_flag, carry, view_flag; size_t bytes; };
+
+inline SamplePointsForwardLayout sample_points_forward_layout(int B, int64_t nf) {
+  const size_t n = (size_t)(nf > 0 ? nf : 1), tiles = (size_t)(nf > 0 ? cdf_tiles(nf) : 1);
+  Placer p;
+  SamplePointsForwardLayout L;
+  L.cdf = p.put(n * sizeof(double));
+  L.coarse = p.put(tiles * sizeof(double));
+  L.tile_sum = p.put(tiles * sizeof(double));
+  L.tile_flag = p.put(tiles * sizeof(int));
+  L.carry = p.put(tiles * sizeof(double));
+  L.view_flag = p.put((size_t)(B > 0 ? B : 1) * sizeof(int));
+  L.bytes = p.total();
+  return L;
+}
+
+struct SamplePointsBackwardLayout { Piece corner_grad, count, off, sums, ids, long_rows, long_count; size_t bytes; };
+
+inline SamplePointsBackwardLayout sample_points_backward_layout(int B, int64_t nf, int N, size_t tsize) {
+  const size_t n = (size_t)(nf > 0 ? nf : 1), np = (size_t)B * (size_t)(N > 0 ? N : 1);
+  Placer p;
+  SamplePointsBackwardLayout L;
+  L.corner_grad = p.put(n * 9 * tsize);
+  L.count = p.put(n * sizeof(int));
+  L.off = p.put((n + 1) * sizeof(int));
+  L.sums = p.put(scan_sums_bytes(nf));
+  L.ids = p.put((np > 0 ? np : 1) * sizeof(int));
+  L.long_rows = p.put(n * sizeof(int));
+  L.long_count = p.put(sizeof(int));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
 // lighting.cu: the light gradients' partial sums, `floats` per light in each of `slots` CTA slots.
 struct LightingLayout { Piece partial; size_t bytes; };
 

@@ -29,6 +29,14 @@ every point (csrc/check_sign.cu); ``CheckSign`` builds the mesh once for many po
 
     S = CheckSign(verts, faces)               # Simplicits, occupancy sampling: many point sets, one mesh
     inside = S(points)                        # (B, N) bool, no host synchronisation
+
+``sample_points``, ``packed_sample_points``, ``face_areas`` and ``packed_face_areas``
+(trianglemesh.py:30-311) sample a surface by area with a stated Philox random stream and a float64 CDF
+per view (csrc/sample_points.cu); ``SurfaceSampler`` keeps the topology its backward needs and never
+reads the host::
+
+    S = SurfaceSampler(V, faces)              # DMTet: fixed topology, sampled every step
+    points, face_choices = S(vertices, 50000)
 """
 import torch
 
@@ -37,7 +45,8 @@ from ..render.mesh import _host
 
 __all__ = ["adjacency_matrix", "uniform_laplacian", "compute_vertex_normals", "average_face_vertex_features",
            "UniformLaplacian", "subdivide_trianglemesh", "LoopSubdivision", "subdivide_tetmesh", "check_sign",
-           "CheckSign"]
+           "CheckSign", "face_areas", "packed_face_areas", "sample_points", "packed_sample_points",
+           "SurfaceSampler"]
 
 
 def _check(func, typed):
@@ -594,3 +603,371 @@ def check_sign(verts, faces, points, hash_resolution=512):
         raise ValueError(f"check_sign: expected verts and points of one batch size, "
                          f"got {verts.shape[0]} and {points.shape[0]}")
     return CheckSign(verts, faces)(points)
+
+
+# ---------------------------------------------------------------------------------------------
+# Face areas and surface sampling (csrc/sample_points.cu).
+
+_SAMPLE_DTYPES = {torch.float32: _lib.DTYPE_F32, torch.float64: _lib.DTYPE_F64}
+_BAD_INDEX, _BAD_DISTRIBUTION = 1, 2          # DIBR_B200_SAMPLE_* status bits
+
+
+def _sample_dtype(func, named):
+    """float32 or float64, one type for every named tensor (None skipped)."""
+    named = [(n, t) for n, t in named if t is not None]
+    for name, t in named:
+        if t.dtype not in _SAMPLE_DTYPES:
+            raise TypeError(f"{func}: expected {name} of type float32 or float64, got {t.dtype}")
+        if t.dtype != named[0][1].dtype:
+            raise TypeError(f"{func}: expected {name} of type {named[0][1].dtype}, got {t.dtype}")
+
+
+def _triangles(func, faces):
+    if not isinstance(faces, torch.Tensor) or faces.dim() != 2:
+        raise ValueError(f"{func}: expected faces of shape (num_faces, 3)")
+    if faces.shape[-1] != 3:
+        raise NotImplementedError(f"{func} is only implemented for triangle meshes")
+    if faces.dtype != torch.int64:
+        raise TypeError(f"{func}: expected faces of type torch.int64, got {faces.dtype}")
+
+
+class _Views:
+    """The views of one call (include/dibr_b200.h): view b owns faces [face_off[b], face_off[b + 1]) of
+    ``faces``, row g - b * fstride, vertex b * vstride + index, every index in [0, num_vertices)."""
+
+    def __init__(self, batch, faces, num_vertices, fstride, vstride, face_off):
+        self.batch, self.faces, self.face_off = batch, faces, face_off
+        self.dims = (batch, batch * fstride if fstride else faces.shape[0], num_vertices, fstride, vstride)
+
+    @staticmethod
+    def dense(vertices, faces):
+        B, V = vertices.shape[:2]
+        F = faces.shape[0]
+        off = torch.arange(B + 1, dtype=torch.int64, device=faces.device) * F
+        return _Views(B, faces, V, F, V, off)
+
+    @staticmethod
+    def packed(func, vertices, first_idx_vertices, faces, num_faces_per_mesh):
+        """The merged faces (faces + each mesh's first vertex) and their views, without a host read."""
+        dev = vertices.device
+        B, F = num_faces_per_mesh.shape[0], faces.shape[0]
+        counts = num_faces_per_mesh.reshape(-1).to(device=dev, dtype=torch.int64)
+        if not num_faces_per_mesh.is_cuda and int(num_faces_per_mesh.sum()) != F:
+            raise ValueError(f"{func}: num_faces_per_mesh sums to {int(num_faces_per_mesh.sum())}, "
+                             f"but faces has {F} rows")
+        # face_off is clamped to [0, F] and ends at F, so that inconsistent counts on the device give
+        # wrong views but never an access outside the faces
+        off = torch.zeros(B + 1, dtype=torch.int64, device=dev)
+        off[1:] = torch.cumsum(counts.clamp(min=0), 0).clamp(max=F)
+        off[B] = F
+        first = first_idx_vertices[:B].reshape(-1).to(device=dev, dtype=torch.int64)
+        merged = faces + torch.repeat_interleave(first, counts.clamp(min=0), output_size=F)[:, None]
+        return _Views(B, merged.contiguous(), vertices.shape[0], 0, 0, off)
+
+
+def _call_face_areas(func, vertices, views, status):
+    areas = vertices.new_empty(views.dims[1])
+    _lib.call("dibr_b200_face_areas_forward", vertices.device, *views.dims, _SAMPLE_DTYPES[vertices.dtype],
+              views.face_off, views.faces, vertices, areas, status, what=func)
+    return areas
+
+
+class _FaceAreas(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, vertices, views, topo, status):
+        ctx.save_for_backward(vertices)
+        ctx.views, ctx.topo = views, topo
+        return _call_face_areas("face_areas", vertices, views, status)
+
+    @staticmethod
+    def backward(ctx, grad):
+        vertices, = ctx.saved_tensors
+        views, topo = ctx.views, ctx.topo
+        dtype = _SAMPLE_DTYPES[vertices.dtype]
+        _, nbytes = _lib.sample_points_workspace_bytes(views.batch, views.dims[1], 0, dtype, "face_areas")
+        ws = _lib.scratch(nbytes, vertices.device)
+        gv = torch.empty_like(vertices)
+        _lib.call("dibr_b200_face_areas_backward", vertices.device, *views.dims, dtype, views.face_off,
+                  views.faces, vertices, grad.contiguous(), topo.corner_ptr, topo.corners, gv, ws, ws.numel(),
+                  what="face_areas")
+        return gv, None, None, None
+
+
+def _wants_grad(*tensors):
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
+def _status_errors(func, status, topo):
+    """The functional forms' one device-to-host read: the topology build's status words (when a
+    topology was built) and the sampling status word."""
+    edges, topo_error, flags = status.tolist()
+    if topo is not None:
+        topo._finish(func, edges, topo_error)
+    if flags & _BAD_INDEX:
+        raise IndexError(f"{func}: faces holds an index outside the vertices")
+    if flags & _BAD_DISTRIBUTION:
+        raise ValueError(f"{func}: the face areas are not a distribution (a negative, NaN or infinite area, "
+                         "or a zero total)")
+
+
+def _face_areas(func, vertices, views, num_vertices, topo_faces):
+    if views.dims[1] == 0:
+        return vertices.new_zeros(0)
+    status = torch.zeros(3, dtype=torch.int32, device=vertices.device)
+    topo = _Topology(func, num_vertices, topo_faces, status=status) if _wants_grad(vertices) else None
+    areas = _FaceAreas.apply(vertices.contiguous(), views, topo, status[2:])
+    _status_errors(func, status, topo)
+    return areas
+
+
+def face_areas(vertices, faces):
+    r"""kaolin.ops.mesh.face_areas: the area of every face, (B, F) of ``vertices``' type, with autograd
+    to ``vertices`` (B, V, 3) float32 or float64; ``faces`` (F, 3) int64.  The reference's rounding,
+    bit for bit; a zero-area face's gradient is NaN, as the reference's autograd gives.  One
+    device-to-host read per call.  Deliberate deviations: a face index outside [0, V) raises
+    ``IndexError``; other float types raise ``TypeError``."""
+    func = "face_areas"
+    _triangles(func, faces)
+    _sample_dtype(func, [("vertices", vertices)])
+    _host.check_tensors(func, [("vertices", vertices), ("faces", faces)], dtype=None)
+    if vertices.dim() != 3 or vertices.shape[-1] != 3:
+        raise ValueError(f"{func}: expected vertices of shape (B, V, 3), got {list(vertices.shape)}")
+    B, F = vertices.shape[0], faces.shape[0]
+    if B == 0:
+        return vertices.new_zeros((0, F))
+    faces = faces.contiguous()
+    return _face_areas(func, vertices, _Views.dense(vertices, faces), vertices.shape[1], faces).view(B, F)
+
+
+def packed_face_areas(vertices, first_idx_vertices, faces, num_faces_per_mesh):
+    r"""kaolin.ops.mesh.packed_face_areas: the area of every packed face, (sum F,), with autograd to the
+    packed ``vertices`` (sum V, 3).  ``first_idx_vertices`` (B + 1) and ``num_faces_per_mesh`` (B)
+    may live on the CPU or the GPU.  As ``face_areas``, on the merged faces."""
+    func = "packed_face_areas"
+    _triangles(func, faces)
+    _sample_dtype(func, [("vertices", vertices)])
+    _host.check_tensors(func, [("vertices", vertices), ("faces", faces)], dtype=None)
+    if vertices.dim() != 2 or vertices.shape[-1] != 3:
+        raise ValueError(f"{func}: expected vertices of shape (num_vertices, 3), got {list(vertices.shape)}")
+    if num_faces_per_mesh.shape[0] == 0:
+        return vertices.new_zeros(faces.shape[0])
+    views = _Views.packed(func, vertices, first_idx_vertices, faces, num_faces_per_mesh)
+    return _face_areas(func, vertices, views, vertices.shape[0], views.faces)
+
+
+class _SamplePoints(torch.autograd.Function):
+    """vertices, face_features (B*F, 3, D) or an empty placeholder -> points, face_choices, features
+    (an empty (B, N, 0) without face_features)."""
+
+    @staticmethod
+    def forward(ctx, vertices, face_features, views, num_samples, areas, key, topo, status):
+        dev = vertices.device
+        B, nf = views.batch, views.dims[1]
+        D = face_features.shape[-1] if face_features.dim() == 4 else 0
+        dtype = _SAMPLE_DTYPES[vertices.dtype]
+        fwd, _ = _lib.sample_points_workspace_bytes(B, nf, num_samples, dtype, "sample_points")
+        ws = _lib.scratch(fwd, dev)
+        points = vertices.new_empty((B, num_samples, 3))
+        choices = torch.empty((B, num_samples), dtype=torch.int64, device=dev)
+        features = vertices.new_empty((B, num_samples, D))
+        _lib.call("dibr_b200_sample_points_forward", dev, *views.dims, dtype, num_samples, D, views.face_off,
+                  views.faces, vertices, areas, face_features if D else None, key, points, choices,
+                  features if D else None, status, ws, ws.numel(), what="sample_points")
+        ctx.mark_non_differentiable(choices)
+        ctx.save_for_backward(choices, key)
+        ctx.views, ctx.topo, ctx.num_samples, ctx.D = views, topo, num_samples, D
+        ctx.shapes = (vertices.shape, face_features.shape)
+        return points, choices, features
+
+    @staticmethod
+    def backward(ctx, grad_points, _grad_choices, grad_features):
+        choices, key = ctx.saved_tensors
+        views, topo, N, D = ctx.views, ctx.topo, ctx.num_samples, ctx.D
+        dev = choices.device
+        dtype_t = grad_points.dtype
+        gv = torch.empty(ctx.shapes[0], dtype=dtype_t, device=dev) if ctx.needs_input_grad[0] else None
+        gf = torch.empty(ctx.shapes[1], dtype=dtype_t, device=dev) if ctx.needs_input_grad[1] and D else None
+        if gv is None and gf is None:
+            return None, None, None, None, None, None, None, None
+        dtype = _SAMPLE_DTYPES[dtype_t]
+        _, nbytes = _lib.sample_points_workspace_bytes(views.batch, views.dims[1], N, dtype, "sample_points")
+        ws = _lib.scratch(nbytes, dev)
+        _lib.call("dibr_b200_sample_points_backward", dev, *views.dims, dtype, N, D, views.face_off, key, choices,
+                  grad_points.contiguous() if gv is not None else None,
+                  grad_features.contiguous() if gf is not None else None,
+                  topo.corner_ptr if gv is not None else None, topo.corners if gv is not None else None, gv, gf,
+                  ws, ws.numel(), what="sample_points")
+        return gv, gf, None, None, None, None, None, None
+
+
+def _draw_key(device):
+    """One 64-bit Philox key drawn on the device from torch's CUDA generator: ``torch.manual_seed``
+    makes a call reproducible, and nothing is read back to the host."""
+    return torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64, device=device)
+
+
+def _sample_args(func, vertices, views, num_samples, areas, areas_shape, face_features):
+    """Checks of the sampling arguments; -> (num_samples, areas as float64 or None, face_features)."""
+    if isinstance(num_samples, bool) or not isinstance(num_samples, int) or num_samples < 0:
+        raise ValueError(f"{func}: num_samples must be an int >= 0, got {num_samples!r}")
+    _sample_dtype(func, [("vertices", vertices), ("face_features", face_features)])
+    if areas is not None:
+        _sample_dtype(func, [("areas", areas)])
+        if tuple(areas.shape) != tuple(areas_shape):
+            raise ValueError(f"{func}: expected areas of shape {list(areas_shape)}, got {list(areas.shape)}")
+        areas = areas.detach().to(torch.float64).contiguous()
+    if face_features is not None:
+        B, F = views.batch, views.dims[3]
+        if face_features.dim() != 4 or tuple(face_features.shape[:3]) != (B, F, 3):
+            raise ValueError(f"{func}: expected face_features of shape ({B}, {F}, 3, D), "
+                             f"got {list(face_features.shape)}")
+        face_features = face_features.contiguous()
+    return num_samples, areas, face_features
+
+
+def _run_sample(vertices, views, num_samples, areas, face_features, key, topo, status):
+    ff = face_features if face_features is not None else vertices.new_empty(0)
+    points, choices, features = _SamplePoints.apply(vertices.contiguous(), ff, views, num_samples, areas, key, topo,
+                                                    status)
+    return (points, choices) if face_features is None else (points, choices, features)
+
+
+def _empty_samples(vertices, B, num_samples, face_features):
+    out = (vertices.new_zeros((B, num_samples, 3)),
+           torch.zeros((B, num_samples), dtype=torch.int64, device=vertices.device))
+    if face_features is not None:
+        out += (vertices.new_zeros((B, num_samples, face_features.shape[-1])),)
+    return out
+
+
+def _sample_points(vertices, faces, num_samples, areas, face_features, key):
+    """``sample_points`` with the Philox key given (a (1,) int64 CUDA tensor)."""
+    func = "sample_points"
+    _triangles(func, faces)
+    _host.check_tensors(func, [("vertices", vertices), ("faces", faces)], dtype=None)
+    if vertices.dim() != 3 or vertices.shape[-1] != 3:
+        raise ValueError(f"{func}: expected vertices of shape (B, V, 3), got {list(vertices.shape)}")
+    B, F = vertices.shape[0], faces.shape[0]
+    for name, t in (("areas", areas), ("face_features", face_features)):
+        if t is not None:
+            _host.check_tensors(func, [("vertices", vertices), (name, t)], dtype=None)
+    if F == 0:
+        raise ValueError(f"{func}: cannot sample a mesh without faces")
+    if B == 0:
+        _sample_args(func, vertices, _Views(0, faces, 0, F, 0, None), num_samples, areas, (0, F), face_features)
+        return _empty_samples(vertices, 0, num_samples, face_features)
+    faces = faces.contiguous()
+    views = _Views.dense(vertices, faces)
+    num_samples, areas, face_features = _sample_args(func, vertices, views, num_samples, areas, (B, F), face_features)
+    status = torch.zeros(3, dtype=torch.int32, device=vertices.device)
+    topo = _Topology(func, vertices.shape[1], faces, status=status) if _wants_grad(vertices) else None
+    out = _run_sample(vertices, views, num_samples, areas, face_features, key, topo, status[2:])
+    _status_errors(func, status, topo)
+    return out
+
+
+def sample_points(vertices, faces, num_samples, areas=None, face_features=None):
+    r"""kaolin.ops.mesh.sample_points: ``num_samples`` points per view, uniformly over the surface.
+
+    ``vertices`` (B, V, 3) float32 or float64, ``faces`` (F, 3) int64 -> (points (B, N, 3), face_choices
+    (B, N) int64), and the interpolated features (B, N, D) when ``face_features`` (B, F, 3, D) of the
+    vertices' type is given.  Autograd flows to ``vertices`` and ``face_features``; ``areas`` (B, F),
+    the unnormalised distribution of the faces, gets none, as in the reference.
+
+    Each face is chosen with probability proportional to its area and each point placed with the
+    reference's barycentric rounding.  The random stream is a stated contract (csrc/sample_points.cu):
+    one 64-bit key is drawn on the device from torch's CUDA generator, so ``torch.manual_seed``
+    reproduces a call bit for bit.  The backward has no float atomics: it is bit-reproducible.  One
+    device-to-host read per call, the status word.  Views of more than 2^24 faces work.
+
+    Deliberate deviations: an invalid distribution (a negative, NaN or infinite area, a zero total,
+    NaN vertices) raises ``ValueError`` as the reference's Categorical does, and a face index outside
+    [0, V) raises ``IndexError``; F = 0 raises ``ValueError``; B = 0 gives empty outputs; only float32
+    and float64 are accepted (``TypeError``), and ``face_features`` must have the vertices' type.
+    ``SurfaceSampler`` builds the topology once and makes no host read.
+    """
+    _host.check_tensors("sample_points", [("vertices", vertices)], dtype=None)
+    return _sample_points(vertices, faces, num_samples, areas, face_features, _draw_key(vertices.device))
+
+
+def _packed_sample_points(vertices, first_idx_vertices, faces, num_faces_per_mesh, num_samples, areas, key):
+    """``packed_sample_points`` with the Philox key given."""
+    func = "packed_sample_points"
+    _triangles(func, faces)
+    _host.check_tensors(func, [("vertices", vertices), ("faces", faces)], dtype=None)
+    if vertices.dim() != 2 or vertices.shape[-1] != 3:
+        raise ValueError(f"{func}: expected vertices of shape (num_vertices, 3), got {list(vertices.shape)}")
+    if areas is not None:
+        _host.check_tensors(func, [("vertices", vertices), ("areas", areas)], dtype=None)
+    B = num_faces_per_mesh.shape[0]
+    if faces.shape[0] == 0:
+        raise ValueError(f"{func}: cannot sample a mesh without faces")
+    if B == 0:
+        _sample_args(func, vertices, _Views(0, faces, 0, 0, 0, None), num_samples, areas, (faces.shape[0],), None)
+        return _empty_samples(vertices, 0, num_samples, None)
+    views = _Views.packed(func, vertices, first_idx_vertices, faces.contiguous(), num_faces_per_mesh)
+    num_samples, areas, _ = _sample_args(func, vertices, views, num_samples, areas, (faces.shape[0],), None)
+    status = torch.zeros(3, dtype=torch.int32, device=vertices.device)
+    topo = _Topology(func, vertices.shape[0], views.faces, status=status) if _wants_grad(vertices) else None
+    out = _run_sample(vertices, views, num_samples, areas, None, key, topo, status[2:])
+    _status_errors(func, status, topo)
+    return out
+
+
+def packed_sample_points(vertices, first_idx_vertices, faces, num_faces_per_mesh, num_samples, areas=None):
+    r"""kaolin.ops.mesh.packed_sample_points: ``sample_points`` on packed meshes.
+
+    ``vertices`` (sum V, 3), ``first_idx_vertices`` (B + 1), ``faces`` (sum F, 3) int64 indexing each
+    mesh's own vertices, ``num_faces_per_mesh`` (B) -> (points (B, N, 3), the chosen faces as indices
+    of the packed faces (B, N) int64), as the reference returns them; ``areas`` (sum F,) optional.
+    Autograd flows to ``vertices``.  The errors and deviations are ``sample_points``'; an empty mesh is
+    an invalid distribution."""
+    _host.check_tensors("packed_sample_points", [("vertices", vertices)], dtype=None)
+    return _packed_sample_points(vertices, first_idx_vertices, faces, num_faces_per_mesh, num_samples, areas,
+                                 _draw_key(vertices.device))
+
+
+class SurfaceSampler:
+    r"""``sample_points`` on one fixed topology, built once.
+
+    ``S = SurfaceSampler(num_vertices, faces)`` checks ``faces`` (F, 3) int64 once (one device-to-host
+    read) and keeps the corner CSR the backward gathers over; ``S(vertices, num_samples, areas=None,
+    face_features=None)`` then returns what ``sample_points`` returns, for any batch size, with no
+    device-to-host read in the forward or the backward::
+
+        S = SurfaceSampler(V, faces)                    # DMTet-style loops, deforming a sphere
+        points, face_choices = S(vertices, 50000)        # (B, N, 3), (B, N)
+
+    Because a call never reads the host, it cannot raise on its data: a view whose areas are not a
+    distribution (a negative, NaN or infinite area, or a zero total, e.g. from NaN vertices) gets face
+    index -1, NaN points and NaN features, and contributes zero gradients.
+    """
+
+    def __init__(self, num_vertices, faces):
+        func = "SurfaceSampler"
+        _triangles(func, faces)
+        if faces.shape[0] == 0:
+            raise ValueError(f"{func}: cannot sample a mesh without faces")
+        self._topo = _Topology(func, num_vertices, faces)
+        self.num_vertices, self.faces = self._topo.num_vertices, self._topo.faces
+
+    def __call__(self, vertices, num_samples, areas=None, face_features=None):
+        func = "SurfaceSampler"
+        V, F = self.num_vertices, self.faces.shape[0]
+        _host.check_tensors(func, [("vertices", vertices), ("faces", self.faces)], dtype=None)
+        for name, t in (("areas", areas), ("face_features", face_features)):
+            if t is not None:
+                _host.check_tensors(func, [("vertices", vertices), (name, t)], dtype=None)
+        if vertices.dim() != 3 or tuple(vertices.shape[1:]) != (V, 3):
+            raise ValueError(f"{func}: expected vertices of shape (B, {V}, 3), got {list(vertices.shape)}")
+        B = vertices.shape[0]
+        if B == 0:
+            _sample_args(func, vertices, _Views(0, self.faces, 0, F, 0, None), num_samples, areas, (0, F),
+                         face_features)
+            return _empty_samples(vertices, 0, num_samples, face_features)
+        views = _Views.dense(vertices, self.faces)
+        num_samples, areas, face_features = _sample_args(func, vertices, views, num_samples, areas, (B, F),
+                                                         face_features)
+        status = torch.empty(1, dtype=torch.int32, device=vertices.device)   # written, never read
+        return _run_sample(vertices, views, num_samples, areas, face_features, _draw_key(vertices.device), self._topo,
+                           status)
