@@ -393,6 +393,9 @@ int dibr_b200_deftet_sparse_render_backward(
 #define DIBR_B200_DTYPE_F32 0
 #define DIBR_B200_DTYPE_F64 1
 #define DIBR_B200_DTYPE_U8 2     /* marching cubes: uint8 (and bool) grids */
+#define DIBR_B200_DTYPE_BOOL 3   /* voxel-grid operators, where bool and uint8 arithmetic differ */
+#define DIBR_B200_DTYPE_I32 4
+#define DIBR_B200_DTYPE_I64 5
 int dibr_b200_check_sign_workspace_bytes(int batch, int num_faces, int num_points, int dtype, size_t* build_bytes,
                                          size_t* query_bytes);
 int dibr_b200_check_sign_build(int batch, int num_vertices, int num_faces, int dtype, const void* verts,
@@ -874,6 +877,43 @@ int dibr_b200_sample_points_backward(int batch, int64_t total_faces, int num_ver
                                      const void* grad_points, const void* grad_features, const int32_t* corner_ptr,
                                      const int32_t* corners, void* grad_vertices, void* grad_face_features,
                                      void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
+ * Voxel-grid operators (kaolin/ops/voxelgrid.py; kaolin_b200/csrc/voxelgrid.cu).  Grids are (batch, X, Y,
+ * Z), read in place through element strides (stride_b, stride_x, stride_y, stride_z); a voxel is
+ * occupied when its value is nonzero (NaN is, -0.0 is not).  Outputs are contiguous, one byte (0 or
+ * 1) per voxel for the boolean ones.
+ *   dibr_b200_voxelgrid_fill: grid of `dtype` DIBR_B200_DTYPE_F32 or _U8 (bool as its bytes) -> out
+ *     (16-byte aligned): occupied, or empty in a 6-connected empty component that touches no border
+ *     face (scipy.ndimage.binary_fill_holes).  The workspace (any alignment, else
+ *     DIBR_B200_EWORKSPACE) is dibr_b200_voxelgrid_fill_workspace_bytes: 4 bytes per voxel.
+ *   dibr_b200_voxelgrid_extract_surface: grid of `dtype` _U8 (bool), _F32 or _F64 -> out: occupied
+ *     and the mean over the 3x3x3 window (thin != 0: over any of the three 3-voxel axis windows),
+ *     zero-padded, below 1, with avg_pool3d's summation order and rounding.
+ *   dibr_b200_voxelgrid_extract_odms: grid (batch, dim, dim, dim) of `dtype` _F32 or _U8 -> out
+ *     (batch, 6, dim, dim) int64, the six orthographic depth maps in the face order z_neg, z_pos,
+ *     y_neg, y_pos, x_neg, x_pos.
+ *   dibr_b200_voxelgrid_project_odms: odms (batch, 6, dim, dim), contiguous, of `odm_dtype` _I64, _I32,
+ *     _F32 or _F64, and grid (batch, dim, dim, dim) of `grid_dtype` _BOOL, _U8, _F32 or _F64, or
+ *     DIBR_B200_VOXELGRID_ALL_ONES (grid unused) -> out: voxel * votes - (masks hit) > 0, in int64
+ *     for bool and all-ones grids, uint8 (wrapping) for uint8 grids and the float type for float grids.
+ * X Y Z must be below 2^31 - 1 voxels per view (else DIBR_B200_ESIZE); negative sizes, a bad dtype or
+ * a NULL buffer that is used give DIBR_B200_EINVAL.  No call reads anything back to the host.
+ */
+#define DIBR_B200_VOXELGRID_ALL_ONES (-1)
+int dibr_b200_voxelgrid_fill_workspace_bytes(int64_t batch, int64_t X, int64_t Y, int64_t Z, size_t* workspace_bytes);
+int dibr_b200_voxelgrid_fill(int64_t batch, int64_t X, int64_t Y, int64_t Z, int dtype, const void* grid,
+                             int64_t stride_b, int64_t stride_x, int64_t stride_y, int64_t stride_z, uint8_t* out,
+                             void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+int dibr_b200_voxelgrid_extract_surface(int64_t batch, int64_t X, int64_t Y, int64_t Z, int dtype, int thin,
+                                        const void* grid, int64_t stride_b, int64_t stride_x, int64_t stride_y,
+                                        int64_t stride_z, uint8_t* out, dibr_b200_stream_t stream);
+int dibr_b200_voxelgrid_extract_odms(int64_t batch, int64_t dim, int dtype, const void* grid, int64_t stride_b,
+                                     int64_t stride_x, int64_t stride_y, int64_t stride_z, int64_t* out,
+                                     dibr_b200_stream_t stream);
+int dibr_b200_voxelgrid_project_odms(int64_t batch, int64_t dim, int odm_dtype, const void* odms, int grid_dtype,
+                                     const void* grid, int64_t stride_b, int64_t stride_x, int64_t stride_y,
+                                     int64_t stride_z, int64_t votes, uint8_t* out, dibr_b200_stream_t stream);
 
 /*
  * subdivide_tetmesh (kaolin/ops/mesh/tetmesh.py:85-181) on the tet topology: vertices (B, V, 3) and

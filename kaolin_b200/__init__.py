@@ -15,8 +15,9 @@ levels once), and DMTet's tet-grid operators (``ops.conversions.marching_tetrahe
 ``ops.mesh.CheckSign``, which builds the mesh once, and ``_C.ops.mesh.unbatched_mesh_intersection_cuda``),
 and marching cubes (``ops.conversions.voxelgrids_to_trianglemeshes``, every view in one call, and
 ``_C.ops.conversions.unbatched_mcube_forward_cuda``), and the point-to-mesh distance
-(``metrics.trianglemesh.point_to_mesh_distance``, every view in one call, and ``_C.metrics``);
-see DESIGN.md for scope.  There is no CPU fallback: every entry point
+(``metrics.trianglemesh.point_to_mesh_distance``, every view in one call, and ``_C.metrics``),
+and the voxel-grid operators (``ops.voxelgrid.{fill, extract_surface, extract_odms, project_odms,
+downsample}``, every view in one launch per kernel); see DESIGN.md for scope.  There is no CPU fallback: every entry point
 raises if the CUDA library (kaolin_b200/csrc, built in-tree) is missing or the
 tensors are not on a CUDA device.
 """

@@ -19,7 +19,7 @@ SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline
            os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu"),
            os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu"),
            os.path.join(CSRC, "point_mesh_distance.cu"), os.path.join(CSRC, "voxelize.cu"),
-           os.path.join(CSRC, "sample_points.cu")]
+           os.path.join(CSRC, "sample_points.cu"), os.path.join(CSRC, "voxelgrid.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
            os.path.join(CSRC, "op_layouts.h"), os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
@@ -34,6 +34,8 @@ LIGHT_SG_INNER_PRODUCT, LIGHT_SG_FITTED, LIGHT_SH9 = 0, 1, 2     # dibr_b200_dif
 BINS_VALID, ACCUMULATE = 1, 2      # dibr_b200_backward flags
 DTYPE_F32, DTYPE_F64 = 0, 1        # check_sign, mesh_intersection_count and point_mesh_distance
 DTYPE_U8 = 2                       # dibr_b200_marching_cubes_* (uint8 and bool grids)
+DTYPE_BOOL, DTYPE_I32, DTYPE_I64 = 3, 4, 5   # dibr_b200_voxelgrid_*
+VOXELGRID_ALL_ONES = -1            # dibr_b200_voxelgrid_project_odms without a grid
 
 _lock = threading.Lock()
 _lib = None
@@ -157,6 +159,12 @@ SIGNATURES = {
     "dibr_b200_face_areas_backward": (_i, [_i, _i64, _i, _i64, _i64, _i] + [_vp] * 8 + [_sz, _vp]),
     "dibr_b200_sample_points_forward": (_i, [_i, _i64, _i, _i64, _i64, _i, _i, _i] + [_vp] * 11 + [_sz, _vp]),
     "dibr_b200_sample_points_backward": (_i, [_i, _i64, _i, _i64, _i64, _i, _i, _i] + [_vp] * 10 + [_sz, _vp]),
+    # voxel-grid operators (ops.voxelgrid; csrc/voxelgrid.cu)
+    "dibr_b200_voxelgrid_fill_workspace_bytes": (_i, [_i64] * 4 + [ctypes.POINTER(_sz)]),
+    "dibr_b200_voxelgrid_fill": (_i, [_i64] * 4 + [_i, _vp] + [_i64] * 4 + [_vp, _vp, _sz, _vp]),
+    "dibr_b200_voxelgrid_extract_surface": (_i, [_i64] * 4 + [_i, _i, _vp] + [_i64] * 4 + [_vp, _vp]),
+    "dibr_b200_voxelgrid_extract_odms": (_i, [_i64, _i64, _i, _vp] + [_i64] * 4 + [_vp, _vp]),
+    "dibr_b200_voxelgrid_project_odms": (_i, [_i64, _i64, _i, _vp, _i, _vp] + [_i64] * 5 + [_vp, _vp]),
 }
 
 
@@ -307,6 +315,13 @@ def sample_points_workspace_bytes(batch, total_faces, num_samples, dtype, what):
     check(lib().dibr_b200_sample_points_workspace_bytes(batch, total_faces, num_samples, dtype, ctypes.byref(fwd),
                                                         ctypes.byref(bwd)), what)
     return fwd.value, bwd.value
+
+
+def voxelgrid_fill_workspace_bytes(batch, X, Y, Z, what):
+    """The workspace bytes of ``dibr_b200_voxelgrid_fill``; raises on its status."""
+    out = _sz(0)
+    check(lib().dibr_b200_voxelgrid_fill_workspace_bytes(batch, X, Y, Z, ctypes.byref(out)), what)
+    return out.value
 
 
 def scratch(nbytes, device):

@@ -312,6 +312,18 @@ inline SamplePointsBackwardLayout sample_points_backward_layout(int B, int64_t n
 }
 
 // ---------------------------------------------------------------------------------------------
+// voxelgrid.cu: fill's union-find labels, one int32 per voxel of `batch` views of `voxels` each.
+struct VoxelgridFillLayout { Piece labels; size_t bytes; };
+
+inline VoxelgridFillLayout voxelgrid_fill_layout(int64_t batch, int64_t voxels) {
+  Placer p;
+  VoxelgridFillLayout L;
+  L.labels = p.put(sizeof(int32_t) * (size_t)batch * (size_t)voxels);
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
 // lighting.cu: the light gradients' partial sums, `floats` per light in each of `slots` CTA slots.
 struct LightingLayout { Piece partial; size_t bytes; };
 

@@ -1,5 +1,7 @@
 """kaolin.ops drop-ins: the mesh Laplacian, adjacency, vertex averaging, Loop subdivision, tet-mesh
 subdivision, marching tetrahedra, marching cubes (``voxelgrids_to_trianglemeshes``) and the point-in-mesh
-test (``check_sign``) and surface sampling (``sample_points``, ``face_areas``) on sm_90a kernels."""
+test (``check_sign``), surface sampling (``sample_points``, ``face_areas``) and the voxel-grid operators
+(``voxelgrid.fill``, ``extract_surface``, ``extract_odms``, ``project_odms``) on sm_90a kernels."""
 from . import mesh  # noqa: F401
 from . import conversions  # noqa: F401
+from . import voxelgrid  # noqa: F401
