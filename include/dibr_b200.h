@@ -916,6 +916,27 @@ int dibr_b200_voxelgrid_project_odms(int64_t batch, int64_t dim, int odm_dtype, 
                                      int64_t stride_z, int64_t votes, uint8_t* out, dibr_b200_stream_t stream);
 
 /*
+ * Farthest point sampling (kaolin/ops/pointcloud.py:52-84; kaolin_b200/csrc/pointcloud.cu).  points
+ * (batch, num_points, 3) float32, read in place through element strides (stride_b, stride_n,
+ * stride_c) -> out (batch, k) int64, contiguous: per view the k indices of the contract stated in
+ * pointcloud.cu (deterministic: ties to the lowest index, points with a NaN or inf coordinate last,
+ * in index order), the same bits for any cluster size, path or run.
+ *   dibr_b200_farthest_point_sampling_workspace_bytes gives the workspace (any alignment, else
+ *   DIBR_B200_EWORKSPACE), the path (DIBR_B200_FPS_CLUSTER: one thread-block cluster per view, its
+ *   points on chip; DIBR_B200_FPS_GRID: one cooperative launch; 0: nothing to do) and the cluster
+ *   size, for the current device.
+ * Negative sizes, k > num_points or a NULL buffer that is used give DIBR_B200_EINVAL; num_points >=
+ * 2^31 - 1 gives DIBR_B200_ESIZE.  B = 0 or k = 0 is a no-op.  No call reads anything back to the host.
+ */
+#define DIBR_B200_FPS_CLUSTER 1
+#define DIBR_B200_FPS_GRID 2
+int dibr_b200_farthest_point_sampling_workspace_bytes(int64_t batch, int64_t num_points, int64_t k,
+                                                      size_t* workspace_bytes, int* path, int* cluster);
+int dibr_b200_farthest_point_sampling(int64_t batch, int64_t num_points, int64_t k, const float* points,
+                                      int64_t stride_b, int64_t stride_n, int64_t stride_c, int64_t* out,
+                                      void* workspace, size_t workspace_bytes, dibr_b200_stream_t stream);
+
+/*
  * subdivide_tetmesh (kaolin/ops/mesh/tetmesh.py:85-181) on the tet topology: vertices (B, V, 3) and
  * features (B, V, channels) or NULL -> out_vertices (B, V + E, 3), out_features: rows < V copied, row
  * V + e the midpoint (y_a + y_b) * 0.5 of edge e; out_tets (8T, 4) int64 or NULL: child k of tet t at

@@ -17,7 +17,9 @@ and marching cubes (``ops.conversions.voxelgrids_to_trianglemeshes``, every view
 ``_C.ops.conversions.unbatched_mcube_forward_cuda``), and the point-to-mesh distance
 (``metrics.trianglemesh.point_to_mesh_distance``, every view in one call, and ``_C.metrics``),
 and the voxel-grid operators (``ops.voxelgrid.{fill, extract_surface, extract_odms, project_odms,
-downsample}``, every view in one launch per kernel); see DESIGN.md for scope.  There is no CPU fallback: every entry point
+downsample}``, every view in one launch per kernel), and farthest point sampling
+(``ops.pointcloud.farthest_point_sampling``, deterministic, every view in one call, with
+``ops.pointcloud.center_points``); see DESIGN.md for scope.  There is no CPU fallback: every entry point
 raises if the CUDA library (kaolin_b200/csrc, built in-tree) is missing or the
 tensors are not on a CUDA device.
 """

@@ -19,7 +19,8 @@ SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline
            os.path.join(CSRC, "lighting.cu"), os.path.join(CSRC, "mesh_topology.cu"),
            os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu"),
            os.path.join(CSRC, "point_mesh_distance.cu"), os.path.join(CSRC, "voxelize.cu"),
-           os.path.join(CSRC, "sample_points.cu"), os.path.join(CSRC, "voxelgrid.cu")]
+           os.path.join(CSRC, "sample_points.cu"), os.path.join(CSRC, "voxelgrid.cu"),
+           os.path.join(CSRC, "pointcloud.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
            os.path.join(CSRC, "op_layouts.h"), os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
@@ -36,6 +37,7 @@ DTYPE_F32, DTYPE_F64 = 0, 1        # check_sign, mesh_intersection_count and poi
 DTYPE_U8 = 2                       # dibr_b200_marching_cubes_* (uint8 and bool grids)
 DTYPE_BOOL, DTYPE_I32, DTYPE_I64 = 3, 4, 5   # dibr_b200_voxelgrid_*
 VOXELGRID_ALL_ONES = -1            # dibr_b200_voxelgrid_project_odms without a grid
+FPS_CLUSTER, FPS_GRID = 1, 2       # dibr_b200_farthest_point_sampling paths
 
 _lock = threading.Lock()
 _lib = None
@@ -165,6 +167,10 @@ SIGNATURES = {
     "dibr_b200_voxelgrid_extract_surface": (_i, [_i64] * 4 + [_i, _i, _vp] + [_i64] * 4 + [_vp, _vp]),
     "dibr_b200_voxelgrid_extract_odms": (_i, [_i64, _i64, _i, _vp] + [_i64] * 4 + [_vp, _vp]),
     "dibr_b200_voxelgrid_project_odms": (_i, [_i64, _i64, _i, _vp, _i, _vp] + [_i64] * 5 + [_vp, _vp]),
+    # farthest point sampling (ops.pointcloud; csrc/pointcloud.cu)
+    "dibr_b200_farthest_point_sampling_workspace_bytes": (_i, [_i64] * 3 + [ctypes.POINTER(_sz)] +
+                                                          [ctypes.POINTER(_i)] * 2),
+    "dibr_b200_farthest_point_sampling": (_i, [_i64] * 3 + [_vp] + [_i64] * 3 + [_vp, _vp, _sz, _vp]),
 }
 
 
@@ -322,6 +328,17 @@ def voxelgrid_fill_workspace_bytes(batch, X, Y, Z, what):
     out = _sz(0)
     check(lib().dibr_b200_voxelgrid_fill_workspace_bytes(batch, X, Y, Z, ctypes.byref(out)), what)
     return out.value
+
+
+def farthest_point_sampling_workspace_bytes(batch, num_points, k, device, what):
+    """(bytes, path, cluster size) of ``dibr_b200_farthest_point_sampling`` on ``device``; raises on its
+    status."""
+    out, path, cluster = _sz(0), _i(0), _i(0)
+    with torch.cuda.device(device):
+        status = lib().dibr_b200_farthest_point_sampling_workspace_bytes(batch, num_points, k, ctypes.byref(out),
+                                                                         ctypes.byref(path), ctypes.byref(cluster))
+    check(status, what)
+    return out.value, path.value, cluster.value
 
 
 def scratch(nbytes, device):

@@ -324,6 +324,73 @@ inline VoxelgridFillLayout voxelgrid_fill_layout(int64_t batch, int64_t voxels) 
 }
 
 // ---------------------------------------------------------------------------------------------
+// pointcloud.cu: farthest point sampling of B views of N points, k rounds.
+//
+// A CTA of kFpsThreads threads keeps kFpsRegPoints points per thread in registers and, past that, up
+// to kFpsSmemPoints per thread in shared memory (16 B each: x, y, z and the key).  A view goes to
+// one thread-block cluster when it fits there: the cluster is the smallest that holds the view in
+// registers, and only a view that needs more than max_cluster CTAs' registers also uses their
+// shared memory.  Larger views take the grid path (one cooperative launch, a contiguous slice of a
+// view per CTA); their points past a CTA's on-chip share live in the workspace.
+//
+// Workspace: the center's chunk sums [B][chunks] (sum x, y, z and the finite count as doubles, one
+// chunk per kFpsChunk points), the centers [B] float4, and on the grid path the round slots
+// [B][3] uint64 and a float4 (x, y, z, key) per point [B][N].
+constexpr int kFpsThreads = 256;
+constexpr int kFpsRegPoints = 32;
+constexpr int kFpsSmemPoints = 48;
+constexpr int kFpsChunk = 1024;
+constexpr int64_t kFpsCtaRegs = (int64_t)kFpsThreads * kFpsRegPoints;                     // 8192
+constexpr int64_t kFpsCtaOnChip = (int64_t)kFpsThreads * (kFpsRegPoints + kFpsSmemPoints);  // 20480
+
+enum FpsPath { kFpsNothing = 0, kFpsCluster = 1, kFpsGrid = 2 };
+
+// The cluster path's CTAs per view and shared-memory points per thread for a view of N points.
+struct FpsPlan { int path, cluster, smem_points; };
+
+// Shared-memory points per thread for a CTA that owns n points.
+inline int fps_smem_points(int64_t n) {
+  const int64_t extra = n - kFpsCtaRegs;
+  if (extra <= 0) return 0;
+  const int64_t q = (extra + kFpsThreads - 1) / kFpsThreads;
+  return (int)(q < kFpsSmemPoints ? q : kFpsSmemPoints);
+}
+
+inline FpsPlan fps_plan(int64_t B, int64_t N, int64_t k, int max_cluster) {
+  FpsPlan p = {kFpsNothing, 0, 0};
+  if (B <= 0 || N <= 0 || k <= 0 || max_cluster <= 0) return p;
+  const int64_t by_regs = (N + kFpsCtaRegs - 1) / kFpsCtaRegs;
+  if (by_regs <= max_cluster) {
+    p.path = kFpsCluster;
+    p.cluster = (int)by_regs;
+  } else if (N <= max_cluster * kFpsCtaOnChip) {
+    p.path = kFpsCluster;
+    p.cluster = max_cluster;
+    p.smem_points = fps_smem_points((N + max_cluster - 1) / max_cluster);
+  } else {
+    p.path = kFpsGrid;
+  }
+  return p;
+}
+
+inline int64_t fps_chunks(int64_t N) { return (N + kFpsChunk - 1) / kFpsChunk; }
+
+struct FpsLayout { FpsPlan plan; Piece chunk_sums, centers, slots, points; size_t bytes; };
+
+inline FpsLayout fps_layout(int64_t B, int64_t N, int64_t k, int max_cluster) {
+  FpsLayout L;
+  L.plan = fps_plan(B, N, k, max_cluster);
+  const size_t views = (size_t)(B > 0 ? B : 0), grid = L.plan.path == kFpsGrid;
+  Placer p;
+  L.chunk_sums = p.put(views * (size_t)fps_chunks(N > 0 ? N : 0) * 4 * sizeof(double));
+  L.centers = p.put(views * 4 * sizeof(float));
+  L.slots = p.put(grid * views * 3 * sizeof(uint64_t));
+  L.points = p.put(grid * views * (size_t)N * 4 * sizeof(float));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
 // lighting.cu: the light gradients' partial sums, `floats` per light in each of `slots` CTA slots.
 struct LightingLayout { Piece partial; size_t bytes; };
 
