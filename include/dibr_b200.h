@@ -791,6 +791,34 @@ int dibr_b200_marching_cubes_backward(int batch, int X, int Y, int Z, int pad, c
                                       float* grad_grid, dibr_b200_stream_t stream);
 
 /*
+ * Cubic meshes (kaolin/ops/conversions/voxelgrid.py:56-156, voxelgrids_to_cubic_meshes) for B views of a
+ * grid (B, X, Y, Z) at `grid` with element strides stride_b..stride_z, float32 (DIBR_B200_DTYPE_F32) or
+ * uint8 / bool (DIBR_B200_DTYPE_U8).  Every voxel is a unit cube and only the faces between values
+ * whose difference rounds to nonzero are kept; csrc/cubic_meshes.cu states the faces, their winding
+ * and order, and the vertex order.
+ *   dibr_b200_cubic_meshes_count: fills the workspace (bit planes and the scan of their counts) and
+ *     writes totals (B, 2) int32 {quads, vertices} per view: the one value to read back to size the
+ *     outputs.
+ *   dibr_b200_cubic_meshes_emit (same workspace, after count): writes, all views in one array each,
+ *     view after view, out_vertices (sum nv, 3) f32 and out_faces, vertex ids per view: with
+ *     is_trimesh (2 sum nq, 3) int64, each view's first triangle of every quad and then its second;
+ *     else (sum nq, 4) int64.
+ * Workspace (any alignment, else DIBR_B200_EWORKSPACE) >= dibr_b200_cubic_meshes_workspace_bytes: 15 bits
+ * per lattice point (X+1)(Y+1)(Z+1) of every view (7 bit planes, and the scan's input and output of
+ * one int per 8 points).  A view's lattice, and 4 B times it,
+ * must be below 2^31 - 1 (else DIBR_B200_ESIZE); a non-positive dimension, a negative batch, a bad
+ * dtype or a NULL buffer that is used give DIBR_B200_EINVAL.
+ */
+int dibr_b200_cubic_meshes_workspace_bytes(int64_t batch, int64_t X, int64_t Y, int64_t Z, size_t* workspace_bytes);
+int dibr_b200_cubic_meshes_count(int64_t batch, int64_t X, int64_t Y, int64_t Z, int dtype, const void* grid,
+                                 int64_t stride_b, int64_t stride_x, int64_t stride_y, int64_t stride_z,
+                                 int32_t* totals, void* workspace, size_t workspace_bytes,
+                                 dibr_b200_stream_t stream);
+int dibr_b200_cubic_meshes_emit(int64_t batch, int64_t X, int64_t Y, int64_t Z, int is_trimesh, float* out_vertices,
+                                int64_t* out_faces, const void* workspace, size_t workspace_bytes,
+                                dibr_b200_stream_t stream);
+
+/*
  * Voxelization (kaolin/ops/conversions/pointcloud.py:22-141, _base_points_to_voxelgrids; and
  * kaolin/ops/conversions/trianglemesh.py:29-110 with _unbatched_subdivide_vertices,
  * kaolin/ops/mesh/trianglemesh.py:340-458) of normalised points (batch, num_points, 3) of `dtype`

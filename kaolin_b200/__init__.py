@@ -14,7 +14,8 @@ levels once), and DMTet's tet-grid operators (``ops.conversions.marching_tetrahe
 ``ops.mesh.subdivide_tetmesh``), and the point-in-mesh test (``ops.mesh.check_sign``,
 ``ops.mesh.CheckSign``, which builds the mesh once, and ``_C.ops.mesh.unbatched_mesh_intersection_cuda``),
 and marching cubes (``ops.conversions.voxelgrids_to_trianglemeshes``, every view in one call, and
-``_C.ops.conversions.unbatched_mcube_forward_cuda``), and the point-to-mesh distance
+``_C.ops.conversions.unbatched_mcube_forward_cuda``), and cubic meshes from voxel grids
+(``ops.conversions.voxelgrids_to_cubic_meshes``, every view in one call), and the point-to-mesh distance
 (``metrics.trianglemesh.point_to_mesh_distance``, every view in one call, and ``_C.metrics``),
 and the voxel-grid operators (``ops.voxelgrid.{fill, extract_surface, extract_odms, project_odms,
 downsample}``, every view in one launch per kernel), and farthest point sampling

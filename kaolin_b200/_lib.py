@@ -20,7 +20,7 @@ SOURCES = [os.path.join(CSRC, "dibr_b200.cu"), os.path.join(CSRC, "mesh_pipeline
            os.path.join(CSRC, "check_sign.cu"), os.path.join(CSRC, "marching_cubes.cu"),
            os.path.join(CSRC, "point_mesh_distance.cu"), os.path.join(CSRC, "voxelize.cu"),
            os.path.join(CSRC, "sample_points.cu"), os.path.join(CSRC, "voxelgrid.cu"),
-           os.path.join(CSRC, "pointcloud.cu")]
+           os.path.join(CSRC, "pointcloud.cu"), os.path.join(CSRC, "cubic_meshes.cu")]
 HEADERS = [os.path.join(CSRC, "dibr_math.cuh"), os.path.join(CSRC, "dibr_math_f64.cuh"),
            os.path.join(CSRC, "dibr_f64.cuh"), os.path.join(CSRC, "workspace_layout.h"),
            os.path.join(CSRC, "op_layouts.h"), os.path.join(CSRC, "grid_bins.cuh"), os.path.join(CSRC, "scan.cuh"),
@@ -146,6 +146,10 @@ SIGNATURES = {
     "dibr_b200_marching_cubes_count": (_i, [_i] * 6 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dibr_b200_marching_cubes_emit": (_i, [_i] * 6 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _vp]),
     "dibr_b200_marching_cubes_backward": (_i, [_i] * 5 + [_vp] + [_i64] * 4 + [_f, _vp, _vp, _vp, _vp, _vp]),
+    # cubic meshes (ops.conversions.voxelgrids_to_cubic_meshes; csrc/cubic_meshes.cu)
+    "dibr_b200_cubic_meshes_workspace_bytes": (_i, [_i64] * 4 + [ctypes.POINTER(_sz)]),
+    "dibr_b200_cubic_meshes_count": (_i, [_i64] * 4 + [_i, _vp] + [_i64] * 4 + [_vp, _vp, _sz, _vp]),
+    "dibr_b200_cubic_meshes_emit": (_i, [_i64] * 4 + [_i, _vp, _vp, _vp, _sz, _vp]),
     # point-to-mesh distance (metrics.trianglemesh.point_to_mesh_distance, _C.metrics; csrc/point_mesh_distance.cu)
     "dibr_b200_point_mesh_distance_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz), ctypes.POINTER(_sz)]),
     "dibr_b200_point_mesh_distance_forward": (_i, [_i, _i, _i, _i] + [_vp] * 5 + [_vp, _sz, _vp]),
@@ -288,6 +292,13 @@ def marching_cubes_workspace_bytes(batch, X, Y, Z, pad, what):
     """The workspace bytes of ``dibr_b200_marching_cubes_count``; raises on its status."""
     out = _sz(0)
     check(lib().dibr_b200_marching_cubes_workspace_bytes(batch, X, Y, Z, pad, ctypes.byref(out)), what)
+    return out.value
+
+
+def cubic_meshes_workspace_bytes(batch, X, Y, Z, what):
+    """The workspace bytes of ``dibr_b200_cubic_meshes_count`` and ``_emit``; raises on its status."""
+    out = _sz(0)
+    check(lib().dibr_b200_cubic_meshes_workspace_bytes(batch, X, Y, Z, ctypes.byref(out)), what)
     return out.value
 
 

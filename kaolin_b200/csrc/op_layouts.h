@@ -210,6 +210,31 @@ inline MarchingCubesLayout marching_cubes_layout(int64_t cubes) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// cubic_meshes.cu, for `batch` views of `lattice` corner points each.  Each view's lattice is
+// padded to kCmWordBits-point words, `cubic_meshes_words(lattice)` per view and plane.  Seven bit
+// planes [7][batch words]: the face planes x, y, z and the corner plane in the order the scan reads
+// them, then the three reversal planes; the scan's input (one popcount per scanned word) and its
+// output [4 batch words + 1]; the scan's tile sums.  Everything lives from the count call to the
+// emit call.
+constexpr int kCmWordBits = 32;
+
+inline int64_t cubic_meshes_words(int64_t lattice) { return (lattice + kCmWordBits - 1) / kCmWordBits; }
+
+struct CubicMeshesLayout { Piece bits, counts, scan, sums; size_t bytes; };
+
+inline CubicMeshesLayout cubic_meshes_layout(int64_t batch, int64_t lattice) {
+  const int64_t n = 4 * batch * cubic_meshes_words(lattice);   // scanned words
+  Placer p;
+  CubicMeshesLayout L;
+  L.bits = p.put(sizeof(uint32_t) * (size_t)(n / 4 * 7));
+  L.counts = p.put(sizeof(int) * (size_t)n);
+  L.scan = p.put(sizeof(int) * ((size_t)n + 1));
+  L.sums = p.put(scan_sums_bytes(n));
+  L.bytes = p.total();
+  return L;
+}
+
+// ---------------------------------------------------------------------------------------------
 // point_mesh_distance.cu, for B views of N points and F faces, T of tsize bytes.
 // Forward: one record of kFaceRecord T per (view, face) and one 64-bit search key per (view, point).
 // Backward: the nine face terms per (view, point), then the points grouped by (view, closest face):

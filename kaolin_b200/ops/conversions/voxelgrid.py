@@ -1,4 +1,5 @@
-"""kaolin.ops.conversions.voxelgrids_to_trianglemeshes on sm_90a kernels (csrc/marching_cubes.cu).
+"""kaolin.ops.conversions.voxelgrids_to_trianglemeshes and voxelgrids_to_cubic_meshes on sm_90a kernels
+(csrc/marching_cubes.cu, csrc/cubic_meshes.cu).
 
 The reference (voxelgrid.py:158-246) loops over the views in Python: each costs a ``torch.all``
 sync, a padded float copy, six device-to-host copies, a device synchronise and about 112 bytes of
@@ -12,7 +13,7 @@ import torch
 from ... import _lib
 from ...render.mesh import _host
 
-__all__ = ["voxelgrids_to_trianglemeshes", "unbatched_mcube_forward"]
+__all__ = ["voxelgrids_to_trianglemeshes", "voxelgrids_to_cubic_meshes", "unbatched_mcube_forward"]
 
 
 def case_table():
@@ -124,6 +125,65 @@ def voxelgrids_to_trianglemeshes(voxelgrids, iso_value=0.5):
         return empty_v, [torch.zeros((0, 3), dtype=torch.int64, device=dev) for _ in range(B)]
     grid = voxelgrids if voxelgrids.dtype in (torch.float32, torch.uint8, torch.bool) else voxelgrids.float()
     verts, faces, nv, nf = _march(func, grid, iso_value, 1)
+    return list(torch.split(verts, nv)), list(torch.split(faces, nf))
+
+
+def voxelgrids_to_cubic_meshes(voxelgrids, is_trimesh=True):
+    r"""kaolin.ops.conversions.voxelgrids_to_cubic_meshes: "Cubify" (Mesh R-CNN, ICCV 2019) on each view
+    of ``voxelgrids`` (B, X, Y, Z): every occupied voxel becomes a unit cube, and only the faces between
+    occupied and empty space are kept.
+
+    Returns ``(vertices, faces)``, two lists of B tensors: vertices (nv, 3) float32, the cube corners
+    the faces use in lattice order, and faces int64 indices into them, (nf, 3) triangles when
+    ``is_trimesh`` else (nq, 4) quads.  Wherever every voxel difference rounds to -1, 0 or 1 (every
+    binary grid of any dtype and every float grid with values in [0, 1]) the output equals the
+    reference's bit for bit.  Values are read as float32 and padded with zeros; a face lies between
+    two voxels whose difference rounds (half to even) to nonzero, NaN included, and its winding
+    follows the difference's sign (csrc/cubic_meshes.cu states the order).  uint8, bool and float32
+    grids are read as they are, contiguous or not; other dtypes go through ``.float()``.  All views
+    go through one launch per kernel, and the call makes one device-to-host read (the per-view
+    counts).  The output is not differentiable, as in the reference: its vertices are lattice points.
+
+    Deliberate deviations from the reference:
+
+    - a face whose difference rounds to 2 or more in magnitude (a uint8 grid of 0 and 255, values
+      above 1.5, infinities) is wound by the sign of the difference; the reference reverses only a
+      difference of exactly -1, so it winds the far side of such a solid inward;
+    - a batch whose every view is empty returns B pairs of empty tensors, vertices (0, 3) float32 and
+      faces (0, 3) or (0, 4) int64, where the reference raises;
+    - B = 0 returns ``([], [])``, and a grid with a zero-size axis returns B pairs of empty tensors;
+    - there is no CPU path (a CPU tensor raises NotImplementedError, as in the other voxel operators),
+      where the reference runs on the CPU;
+    - an input that is not 4-D raises ValueError.
+    """
+    func = "voxelgrids_to_cubic_meshes"
+    if not voxelgrids.is_cuda:
+        raise NotImplementedError(f"{func} does not support CPU.")
+    if voxelgrids.dim() != 4:
+        raise ValueError(f"{func}: expected voxelgrids of shape (batch_size, X, Y, Z), got {list(voxelgrids.shape)}")
+    B, X, Y, Z = voxelgrids.shape
+    if B == 0:
+        return [], []
+    dev = voxelgrids.device
+    corners = 3 if is_trimesh else 4
+    if 0 in (X, Y, Z):
+        empty_v = [torch.zeros((0, 3), dtype=torch.float32, device=dev) for _ in range(B)]
+        return empty_v, [torch.zeros((0, corners), dtype=torch.int64, device=dev) for _ in range(B)]
+    nbytes = _lib.cubic_meshes_workspace_bytes(B, X, Y, Z, func)
+    native = voxelgrids.dtype in (torch.float32, torch.uint8, torch.bool)
+    flag, g = _native(voxelgrids if native else voxelgrids.float())
+    ws = _lib.scratch(nbytes, dev)
+    totals = torch.empty((B, 2), dtype=torch.int32, device=dev)
+    _lib.call("dibr_b200_cubic_meshes_count", dev, B, X, Y, Z, flag, g, *g.stride(), totals, ws, nbytes, what=func)
+    totals = totals.tolist()                          # the call's one device-to-host read
+    per_quad = 2 if is_trimesh else 1
+    nf = [per_quad * t[0] for t in totals]
+    nv = [t[1] for t in totals]
+    verts = torch.empty((sum(nv), 3), dtype=torch.float32, device=dev)
+    faces = torch.empty((sum(nf), corners), dtype=torch.int64, device=dev)
+    if faces.numel():
+        _lib.call("dibr_b200_cubic_meshes_emit", dev, B, X, Y, Z, int(bool(is_trimesh)), verts, faces, ws, nbytes,
+                  what=func)
     return list(torch.split(verts, nv)), list(torch.split(faces, nf))
 
 
